@@ -62,6 +62,11 @@ const char* pv_last_error(void);
 int pv_device_info(int* sm_count, int* cc);
 /* Number of kernels launched by this library since load (bench.py "gpu_launches"). */
 long long pv_launch_count(void);
+/* Launches per kernel instance since load, one "name count\n" line per instance in name order, where the
+ * name carries the template arguments that select the instance (e.g. "conv3d_igemm_kernel<64,128>").
+ * Writes the NUL-terminated text to buf when it fits in len bytes (else buf[0] = 0) and returns its
+ * length without the NUL.  CUDA-graph replays are not counted. */
+int pv_kernel_counts(char* buf, int len);
 
 /* ---------------------------------------------------------------------------------------------
  * Clip transform chain, fused (one kernel):
@@ -305,8 +310,12 @@ int pv_head_reduce(const void* x, int dtype, long long row_stride, int N, long l
  * pv_attention : o = softmax((q*scale) k^T) v (+ q)    attention.py:531-539, flash-style, the
  *                N_q x N_k matrix is never materialised.  q/k/v/o are [B][N][H][D] with
  *                explicit row strides (elements between consecutive tokens), D = head dim.
- *                f16: wgmma + TMA kernel for head dims 32/64/96 with 16-byte aligned strides (csrc/pv_attention_wgmma.cu),
- *                else the mma.sync flash kernel (csrc/pv_attention_mma.cu); f32: CUDA-core flash kernel.
+ *                f16: wgmma + TMA kernel for head dims 32/64/96 (csrc/pv_attention_wgmma.cu), the mma.sync flash
+ *                kernel for D = 128 (csrc/pv_attention_mma.cu), both only with 16-byte aligned q/k/v pointers,
+ *                row and batch strides and 4-byte aligned o / even o strides, q/k/v rows of at least H*D elements,
+ *                batch strides (B > 1) of at least N rows and all strides below 2^40 bytes; everything else (and
+ *                f32) runs the CUDA-core flash kernel.  pv_attention_kernel_for tells which one a call would launch;
+ *                should the driver still refuse a tensor map, pv_attention_fwd returns PV_ERR_CUDA.
  * ------------------------------------------------------------------------------------------- */
 int pv_layernorm(const void* x, void* y, int dtype, long long rows, int groups, int C,
                  long long x_row_stride, long long y_row_stride, const float* gamma,
@@ -351,6 +360,14 @@ typedef struct pv_attention_desc {
 } pv_attention_desc;
 int pv_attention_fwd(const pv_attention_desc* d, const void* q, const void* k, const void* v,
                      void* o, void* stream);
+/* Host-only routing query, the predicate pv_attention_fwd itself uses: which kernel it would launch for these
+ * arguments (the pointers are only inspected for alignment), or a negative pv_status when it would refuse them. */
+typedef enum pv_attention_kernel {
+  PV_ATTN_WGMMA = 1,    /* f16 wgmma + TMA flash kernel                */
+  PV_ATTN_MMA = 2,      /* f16 mma.sync flash kernel                   */
+  PV_ATTN_SIMT = 3      /* CUDA-core flash kernel (f16 or f32 storage) */
+} pv_attention_kernel;
+int pv_attention_kernel_for(const pv_attention_desc* d, const void* q, const void* k, const void* v, const void* o);
 
 #ifdef __cplusplus
 }

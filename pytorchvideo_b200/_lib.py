@@ -12,6 +12,7 @@ PV_F16, PV_F32, PV_U8 = 0, 1, 2
 ACT_NONE, ACT_RELU, ACT_SWISH, ACT_GELU, ACT_SIGMOID = 0, 1, 2, 3, 4
 ALGO_AUTO, ALGO_DIRECT, ALGO_TCGEN05 = 0, 1, 2
 POOL_MAX, POOL_AVG = 0, 1
+ATTN_WGMMA, ATTN_MMA, ATTN_SIMT = 1, 2, 3
 
 c_ll = C.c_longlong
 c_vp = C.c_void_p
@@ -83,6 +84,7 @@ SIGNATURES = {
     "pv_last_error": (C.c_char_p, []),
     "pv_device_info": (C.c_int, [C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "pv_launch_count": (c_ll, []),
+    "pv_kernel_counts": (C.c_int, [C.c_char_p, C.c_int]),
     "pv_clip_transform_fwd": (C.c_int, [C.POINTER(ClipTransformDesc), c_vp, c_vp, c_vp, c_vp, c_vp,
                                         c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_clip_transform_batch": (C.c_int, [C.POINTER(ClipBatchDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
@@ -124,6 +126,7 @@ SIGNATURES = {
     "pv_add_layernorm": (C.c_int, [c_vp, C.c_int, c_ll, c_vp, c_ll, c_vp, c_ll, c_vp, c_ll, c_ll, C.c_int, c_vp, c_vp,
                                    C.c_float, c_vp]),
     "pv_attention_fwd": (C.c_int, [C.POINTER(AttentionDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_attention_kernel_for": (C.c_int, [C.POINTER(AttentionDesc), c_vp, c_vp, c_vp, c_vp]),
 }
 
 _lib = None
@@ -171,3 +174,20 @@ def require_device():
 
 def launch_count():
     return int(load().pv_launch_count())
+
+
+def kernel_counts():
+    """{kernel instance name: launches since load}, e.g. {"conv3d_igemm_kernel<64,128>": 3, ...}."""
+    lib = load()
+    n = lib.pv_kernel_counts(None, 0)
+    while True:
+        buf = C.create_string_buffer(n + 1)
+        m = lib.pv_kernel_counts(buf, n + 1)
+        if m <= n:
+            break
+        n = m                      # another thread launched a new instance in between
+    out = {}
+    for line in buf.value.decode().splitlines():
+        name, count = line.rsplit(" ", 1)
+        out[name] = int(count)
+    return out

@@ -2,12 +2,20 @@
 #include "pv_common.cuh"
 
 #include <atomic>
+#include <map>
+#include <mutex>
+#include <string>
+#include <unordered_map>
 #include <string.h>
 
 namespace pv {
 
 static thread_local char g_err[512] = "";
 static std::atomic<long long> g_launches{0};
+// per-kernel-instance launch counts, keyed by the address of the launch site's name literal (one hash update per
+// eager launch; graph replays do not come through here)
+static std::mutex g_kernel_mu;
+static std::unordered_map<const char*, long long> g_kernel_counts;
 
 void set_error(const char* fmt, ...) {
   va_list ap;
@@ -15,7 +23,11 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
-void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+void count_launch(const char* name) {
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  std::lock_guard<std::mutex> lock(g_kernel_mu);
+  ++g_kernel_counts[name];
+}
 
 int conv3d_check(const pv_conv3d_desc* d);
 int conv3d_direct_launch(const pv_conv3d_desc* d, const void* x, const void* w, const float* scale,
@@ -36,6 +48,19 @@ static bool wants_gather(const pv_conv3d_desc* d) { return d->Ci < 64 && d->ci_p
 extern "C" int pv_abi_version(void) { return PV_ABI_VERSION; }
 extern "C" const char* pv_last_error(void) { return pv::g_err; }
 extern "C" long long pv_launch_count(void) { return pv::g_launches.load(); }
+
+extern "C" int pv_kernel_counts(char* buf, int len) {
+  std::map<std::string, long long> by_name;   // the same name may be spelled at several sites: merge, sort
+  {
+    std::lock_guard<std::mutex> lock(pv::g_kernel_mu);
+    for (const auto& kv : pv::g_kernel_counts) by_name[kv.first] += kv.second;
+  }
+  std::string out;
+  for (const auto& kv : by_name) out += kv.first + " " + std::to_string(kv.second) + "\n";
+  if (buf && len > (int)out.size()) memcpy(buf, out.c_str(), out.size() + 1);
+  else if (buf && len > 0) buf[0] = '\0';
+  return (int)out.size();
+}
 
 extern "C" int pv_device_info(int* sm_count, int* cc) {
   int n = 0;

@@ -114,44 +114,74 @@ attention_kernel(pv_attention_desc d, const T* __restrict__ q, const T* __restri
 
 template <typename T, int D>
 static int launch_attention(const pv_attention_desc* d, const void* q, const void* k, const void* v,
-                            void* o, cudaStream_t s) {
+                            void* o, cudaStream_t s, const char* name) {
   const size_t smem = (size_t)((ATT_BQ + 2 * ATT_BK) * (D + 1) + ATT_WARPS * ATT_QPW * 32) * sizeof(float);
   PV_OPT_IN_SMEM((attention_kernel<T, D>), smem);
   dim3 grid((unsigned)cdiv(d->Nq, ATT_BQ), (unsigned)(d->B * d->H)), block(ATT_WARPS * 32);
   attention_kernel<T, D><<<grid, block, smem, s>>>(*d, (const T*)q, (const T*)k, (const T*)v, (T*)o);
-  PV_LAUNCH_OK("attention_kernel");
+  PV_LAUNCH_OK(name);
   return PV_OK;
 }
 
-int attention_wgmma_dispatch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
-                            cudaStream_t s);   // pv_attention_wgmma.cu
-int attention_mma_dispatch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
-                           cudaStream_t s);   // pv_attention_mma.cu
+int attention_wgmma_launch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
+                          cudaStream_t s);   // pv_attention_wgmma.cu
+int attention_mma_launch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
+                         cudaStream_t s);    // pv_attention_mma.cu
+
+// The f16 tensor-core kernels read q / k / v with 16-byte cp.async / TMA and 4-byte fragment loads from every batch,
+// head and row start, and store o as __half2: pointers, row strides and batch strides must keep that alignment.  The
+// wgmma kernel also describes q / k / v as [B][N][H*D] tensor maps, whose strides must be non-zero, must not make rows
+// or samples overlap and must stay below 2^40 bytes; both tensor-core kernels share this rule, so every call it admits
+// can be encoded.  With B == 1 the batch strides are never used and are not checked.
+static bool tc_strides_ok(long long rs, long long bs, int n, const pv_attention_desc* d) {
+  const long long limit = (1ll << 39);               // elements: 2^40 bytes of f16
+  if (rs % 8 || rs < (long long)d->H * d->D || rs >= limit) return false;
+  if (d->B == 1) return true;
+  return bs % 8 == 0 && bs >= rs * n && bs < limit;
+}
+static bool tensor_core_aligned(const pv_attention_desc* d, const void* q, const void* k, const void* v, const void* o) {
+  if (!tc_strides_ok(d->q_row_stride, d->q_batch_stride, d->Nq, d) || !tc_strides_ok(d->k_row_stride, d->k_batch_stride, d->Nk, d) ||
+      !tc_strides_ok(d->v_row_stride, d->v_batch_stride, d->Nk, d))
+    return false;
+  if (d->o_row_stride % 2 || (d->B > 1 && d->o_batch_stride % 2)) return false;
+  if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v)) & 15) return false;
+  return (reinterpret_cast<uintptr_t>(o) & 3) == 0;
+}
 
 }  // namespace pv
 
-extern "C" int pv_attention_fwd(const pv_attention_desc* d, const void* q, const void* k,
-                                const void* v, void* o, void* stream) {
+extern "C" int pv_attention_kernel_for(const pv_attention_desc* d, const void* q, const void* k, const void* v,
+                                       const void* o) {
   PV_CHECK_ARG(d && q && k && v && o, "null argument");
   PV_CHECK_ARG(d->dtype == PV_F16 || d->dtype == PV_F32, "attention dtype must be f16|f32");
   PV_CHECK_ARG(d->B > 0 && d->H > 0 && d->Nq > 0 && d->Nk > 0, "empty attention problem");
   PV_CHECK_ARG((long long)d->B * d->H <= 65535, "B*H too large");
-  cudaStream_t s = (cudaStream_t)stream;
-  if (d->dtype == PV_F16 && !getenv("PVB200_ATTN_SIMT")) {     // tensor-core paths (f16 storage)
-    int rc = pv::attention_wgmma_dispatch(d, q, k, v, o, s);         // wgmma + TMA (pv_attention_wgmma.cu)
-    if (rc != PV_ERR_UNSUPPORTED) return rc;
-    rc = pv::attention_mma_dispatch(d, q, k, v, o, s);               // mma.sync: head dims / strides the TMA path rejects
-    if (rc != PV_ERR_UNSUPPORTED) return rc;
+  if (d->D != 32 && d->D != 64 && d->D != 96 && d->D != 128) {
+    pv::set_error("attention head dim %d unsupported (32/64/96/128)", d->D);
+    return PV_ERR_UNSUPPORTED;
   }
-#define PV_ATT(DD)                                                                              \
-  if (d->D == DD)                                                                               \
-    return d->dtype == PV_F16 ? pv::launch_attention<__half, DD>(d, q, k, v, o, s)              \
-                              : pv::launch_attention<float, DD>(d, q, k, v, o, s);
+  if (d->dtype == PV_F16 && !getenv("PVB200_ATTN_SIMT") && pv::tensor_core_aligned(d, q, k, v, o))
+    return d->D == 128 ? PV_ATTN_MMA : PV_ATTN_WGMMA;
+  return PV_ATTN_SIMT;
+}
+
+extern "C" int pv_attention_fwd(const pv_attention_desc* d, const void* q, const void* k,
+                                const void* v, void* o, void* stream) {
+  const int kernel = pv_attention_kernel_for(d, q, k, v, o);
+  if (kernel < 0) return kernel;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (kernel == PV_ATTN_WGMMA) return pv::attention_wgmma_launch(d, q, k, v, o, s);
+  if (kernel == PV_ATTN_MMA) return pv::attention_mma_launch(d, q, k, v, o, s);
+#define PV_ATT(DD)                                                                                          \
+  if (d->D == DD)                                                                                           \
+    return d->dtype == PV_F16                                                                               \
+               ? pv::launch_attention<__half, DD>(d, q, k, v, o, s, "attention_kernel<__half," #DD ">")     \
+               : pv::launch_attention<float, DD>(d, q, k, v, o, s, "attention_kernel<float," #DD ">");
   PV_ATT(32)
   PV_ATT(64)
   PV_ATT(96)
   PV_ATT(128)
 #undef PV_ATT
-  pv::set_error("attention head dim %d unsupported (32/64/96/128)", d->D);
-  return PV_ERR_UNSUPPORTED;
+  pv::set_error("internal: attention head dim %d", d->D);
+  return PV_ERR_INVALID;
 }

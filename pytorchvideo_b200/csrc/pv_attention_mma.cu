@@ -198,30 +198,25 @@ attention_mma_kernel(pv_attention_desc d, const __half* __restrict__ q, const __
 
 template <int D>
 static int launch_attention_mma(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
-                                cudaStream_t s) {
+                                cudaStream_t s, const char* name) {
   const size_t smem = (size_t)4 * FA_BK * (D + 8) * sizeof(__half);
   PV_OPT_IN_SMEM(attention_mma_kernel<D>, smem);
   dim3 grid((unsigned)cdiv(d->Nq, FA_BQ), (unsigned)(d->B * d->H)), block(FA_WARPS * 32);
   attention_mma_kernel<D><<<grid, block, smem, s>>>(*d, (const __half*)q, (const __half*)k, (const __half*)v, (__half*)o);
-  PV_LAUNCH_OK("attention_mma_kernel");
+  PV_LAUNCH_OK(name);
   return PV_OK;
 }
 
-// f16 tensor-core path; returns PV_ERR_UNSUPPORTED when the shape does not qualify
-int attention_mma_dispatch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
-                           cudaStream_t s) {
-  if (d->dtype != PV_F16) return PV_ERR_UNSUPPORTED;
-  // 4-byte fragment loads / 16-byte cp.async need aligned rows
-  if (d->q_row_stride % 8 || d->k_row_stride % 8 || d->v_row_stride % 8 || d->o_row_stride % 2) return PV_ERR_UNSUPPORTED;
-  if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v)) & 15)
-    return PV_ERR_UNSUPPORTED;
+// f16 tensor-core path; pv_attention_fwd (pv_attention.cu) has checked the alignment of pointers and strides.
+// Only D = 128 is routed here: the wgmma kernel takes 32 / 64 / 96 under the same alignment rules.
+int attention_mma_launch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o, cudaStream_t s) {
+#define PV_AM(DD) \
+  case DD: return launch_attention_mma<DD>(d, q, k, v, o, s, "attention_mma_kernel<" #DD ">");
   switch (d->D) {
-    case 32: return launch_attention_mma<32>(d, q, k, v, o, s);
-    case 64: return launch_attention_mma<64>(d, q, k, v, o, s);
-    case 96: return launch_attention_mma<96>(d, q, k, v, o, s);
-    case 128: return launch_attention_mma<128>(d, q, k, v, o, s);
-    default: return PV_ERR_UNSUPPORTED;
+    PV_AM(32) PV_AM(64) PV_AM(96) PV_AM(128)
+    default: set_error("internal: mma attention head dim %d", d->D); return PV_ERR_INVALID;
   }
+#undef PV_AM
 }
 
 }  // namespace pv

@@ -5,7 +5,7 @@
 // mbarriers.  S = Q K^T is one m64n64 wgmma per 16 dims (both operands K-major in shared memory); the online softmax
 // runs on the S fragments in registers; O += P V takes P straight from registers (register-A wgmma, the P fragment is
 // the S accumulator layout re-packed to f16) and V MN-major from shared memory as it lies in memory, one m64n32 wgmma
-// per 32-dim chunk and 16 keys.  Head dims 32 / 64 / 96; other shapes use the mma.sync kernel (pv_attention_mma.cu).
+// per 32-dim chunk and 16 keys.  Head dims 32 / 64 / 96; D = 128 uses the mma.sync kernel (pv_attention_mma.cu).
 #include "pv_common.cuh"
 #include "pv_sm90.cuh"
 
@@ -198,44 +198,45 @@ attention_wgmma_kernel(const __grid_constant__ AttnWgParams P, const __half* __r
 // [B][N][H*D] f16 with the given row / batch strides (elements) -> 3-D map, box [32 dims, 64 rows, 1], SWIZZLE_64B
 static bool aw_encode(EncodeTiledFn encode, CUtensorMap* m, const void* p, const pv_attention_desc* d, int n, long long rs, long long bs) {
   cuuint64_t gdim[3] = {(cuuint64_t)d->H * d->D, (cuuint64_t)n, (cuuint64_t)d->B};
-  cuuint64_t gstr[2] = {(cuuint64_t)rs * 2, (cuuint64_t)bs * 2};
+  // one sample: the batch stride is never stepped over, give the map a valid one
+  cuuint64_t gstr[2] = {(cuuint64_t)rs * 2, (cuuint64_t)(d->B == 1 ? rs * n : bs) * 2};
   cuuint32_t box[3] = {32, 64, 1}, estr[3] = {1, 1, 1};
   return encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(p), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                 CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 template <int D>
-static int launch_attention_wgmma(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o, cudaStream_t s) {
+static int launch_attention_wgmma(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o, cudaStream_t s,
+                                  const char* name) {
   EncodeTiledFn encode = get_encode_fn();
-  if (!encode) return PV_ERR_UNSUPPORTED;
+  if (!encode) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return PV_ERR_CUDA; }
   AttnWgParams P;
   memset(&P, 0, sizeof(P));
   P.d = *d;
   if (!aw_encode(encode, &P.q_map, q, d, d->Nq, d->q_row_stride, d->q_batch_stride) ||
       !aw_encode(encode, &P.k_map, k, d, d->Nk, d->k_row_stride, d->k_batch_stride) ||
-      !aw_encode(encode, &P.v_map, v, d, d->Nk, d->v_row_stride, d->v_batch_stride))
-    return PV_ERR_UNSUPPORTED;
+      !aw_encode(encode, &P.v_map, v, d, d->Nk, d->v_row_stride, d->v_batch_stride)) {
+    set_error("cuTensorMapEncodeTiled(attention q/k/v) failed");
+    return PV_ERR_CUDA;
+  }
   constexpr size_t smem = 1024 + 5 * (size_t)(D / 32) * AW_CHUNK + 64;
   PV_OPT_IN_SMEM(attention_wgmma_kernel<D>, smem);
   dim3 grid((unsigned)cdiv(d->Nq, AW_BQ), (unsigned)(d->B * d->H)), block(128);
   attention_wgmma_kernel<D><<<grid, block, smem, s>>>(P, (const __half*)q, (__half*)o);
-  PV_LAUNCH_OK("attention_wgmma_kernel");
+  PV_LAUNCH_OK(name);
   return PV_OK;
 }
 
-// f16 wgmma path; returns PV_ERR_UNSUPPORTED when the shape does not qualify (the caller then uses the mma.sync kernel)
-int attention_wgmma_dispatch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o, cudaStream_t s) {
-  if (d->dtype != PV_F16) return PV_ERR_UNSUPPORTED;
-  // tensor maps: 16-byte aligned bases and strides; the epilogue's 4-byte stores need even output strides
-  if (d->q_row_stride % 8 || d->k_row_stride % 8 || d->v_row_stride % 8 || d->o_row_stride % 2) return PV_ERR_UNSUPPORTED;
-  if (d->q_batch_stride % 8 || d->k_batch_stride % 8 || d->v_batch_stride % 8) return PV_ERR_UNSUPPORTED;
-  if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v)) & 15) return PV_ERR_UNSUPPORTED;
+// f16 wgmma path for head dims 32 / 64 / 96; pv_attention_fwd (pv_attention.cu) has checked the alignment of pointers
+// and strides (16-byte tensor-map bases and strides, 4-byte output stores).
+int attention_wgmma_launch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o, cudaStream_t s) {
+#define PV_AW(DD) \
+  case DD: return launch_attention_wgmma<DD>(d, q, k, v, o, s, "attention_wgmma_kernel<" #DD ">");
   switch (d->D) {
-    case 32: return launch_attention_wgmma<32>(d, q, k, v, o, s);
-    case 64: return launch_attention_wgmma<64>(d, q, k, v, o, s);
-    case 96: return launch_attention_wgmma<96>(d, q, k, v, o, s);
-    default: return PV_ERR_UNSUPPORTED;
+    PV_AW(32) PV_AW(64) PV_AW(96)
+    default: set_error("internal: wgmma attention head dim %d", d->D); return PV_ERR_INVALID;
   }
+#undef PV_AW
 }
 
 }  // namespace pv

@@ -12,7 +12,9 @@ namespace pv {
 
 // ---- error plumbing -------------------------------------------------------------------------
 void set_error(const char* fmt, ...);
-void count_launch(int n = 1);
+// Counts one launch of `name`, a string literal naming the kernel with its template arguments
+// ("conv3d_igemm_kernel<64,128>"); read back with pv_kernel_counts.
+void count_launch(const char* name);
 
 #define PV_CHECK_ARG(cond, ...)            \
   do {                                     \
@@ -40,7 +42,7 @@ void count_launch(int n = 1);
       (void)cudaGetLastError();                                                            \
       return PV_ERR_CUDA;                                                                  \
     }                                                                                      \
-    pv::count_launch();                                                                    \
+    pv::count_launch(name);                                                                \
   } while (0)
 
 static inline long long cdiv(long long a, long long b) { return (a + b - 1) / b; }

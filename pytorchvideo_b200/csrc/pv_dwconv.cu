@@ -253,13 +253,15 @@ int dwconv3d_temporal_launch(const pv_conv3d_desc* d, const void* x, const void*
   dim3 grid((unsigned)blocks, (unsigned)d->N), block(128);
   const size_t smem = (size_t)(d->kt + 2) * d->Co * sizeof(float);
   if (smem > 40 * 1024) return PV_ERR_UNSUPPORTED;
-  if (d->kt == 5)
+  if (d->kt == 5) {
     dwconv_temporal_kernel<5><<<grid, block, smem, stream>>>((const __half*)x, (const __half*)w, scale, bias, (__half*)y, d->To, hw,
                                                         G, d->Co, d->x_row_stride, d->y_row_stride, xbs, ybs, d->act);
-  else
+    PV_LAUNCH_OK("dwconv_temporal_kernel<5>");
+  } else {
     dwconv_temporal_kernel<3><<<grid, block, smem, stream>>>((const __half*)x, (const __half*)w, scale, bias, (__half*)y, d->To, hw,
                                                         G, d->Co, d->x_row_stride, d->y_row_stride, xbs, ybs, d->act);
-  PV_LAUNCH_OK("dwconv_temporal_kernel");
+    PV_LAUNCH_OK("dwconv_temporal_kernel<3>");
+  }
   return PV_OK;
 }
 
@@ -331,13 +333,13 @@ int dwconv3d_tile_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   do {                                                                                                        \
     PV_OPT_IN_SMEM((dwconv3d_tile_kernel<KW_, SW_>), 110 * 1024);                                             \
     dwconv3d_tile_kernel<KW_, SW_><<<grid, block, smem, stream>>>(P, (const __half*)w, scale, bias, (__half*)y, se_sums); \
+    PV_LAUNCH_OK("dwconv3d_tile_kernel<" #KW_ "," #SW_ ">");                                                  \
   } while (0)
   if (d->kw == 3 && d->sw == 1) PV_DWT(3, 1);
   else if (d->kw == 3) PV_DWT(3, 2);
   else if (d->sw == 1) PV_DWT(1, 1);
   else PV_DWT(1, 2);
 #undef PV_DWT
-  PV_LAUNCH_OK("dwconv3d_tile_kernel");
   return PV_OK;
 }
 

@@ -244,6 +244,7 @@ int dwconv3d_lane_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
     PV_OPT_IN_SMEM((dwconv3d_lane_kernel<S_, PH_, PW_, X2_, NW_>), 110 * 1024);                               \
     dwconv3d_lane_kernel<S_, PH_, PW_, X2_, NW_><<<grid, block, smem, stream>>>(P, (const __half*)w, scale,   \
                                                                                bias, (__half*)y, se_sums);    \
+    PV_LAUNCH_OK("dwconv3d_lane_kernel<" #S_ "," #PH_ "," #PW_ "," #X2_ "," #NW_ ">");                       \
   } while (0)
 #define PV_DWL(S_, PH_, PW_)                                                                                  \
   do {                                                                                                        \
@@ -256,7 +257,6 @@ int dwconv3d_lane_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   else PV_DWL(2, 2, 7);
 #undef PV_DWL
 #undef PV_DWL2
-  PV_LAUNCH_OK("dwconv3d_lane_kernel");
   return PV_OK;
 }
 

@@ -569,17 +569,17 @@ int conv3d_tcgen05_launch(const pv_conv3d_desc* d, const void* x, const void* w,
   if (P.block_n == BN && P.kbytes == KB) {                                                     \
     PV_OPT_IN_SMEM((conv3d_igemm_kernel<BN, KB>), 227 * 1024);                                 \
     PV_CUDA_OK(cudaLaunchKernelEx(&cfg, conv3d_igemm_kernel<BN, KB>, P, scale, bias));         \
-    launched = true;                                                                           \
+    name = "conv3d_igemm_kernel<" #BN "," #KB ">";                                              \
   }
-    bool launched = false;
+    const char* name = nullptr;
     PV_IG_LAUNCH(16, 32) PV_IG_LAUNCH(16, 64) PV_IG_LAUNCH(16, 128)
     PV_IG_LAUNCH(32, 32) PV_IG_LAUNCH(32, 64) PV_IG_LAUNCH(32, 128)
     PV_IG_LAUNCH(64, 32) PV_IG_LAUNCH(64, 64) PV_IG_LAUNCH(64, 128)
     PV_IG_LAUNCH(128, 32) PV_IG_LAUNCH(128, 64) PV_IG_LAUNCH(128, 128)
 #undef PV_IG_LAUNCH
-    if (!launched) { set_error("internal: no igemm instance for BN=%d kbytes=%d", P.block_n, P.kbytes); return PV_ERR_INVALID; }
+    if (!name) { set_error("internal: no igemm instance for BN=%d kbytes=%d", P.block_n, P.kbytes); return PV_ERR_INVALID; }
+    PV_LAUNCH_OK(name);
   }
-  PV_LAUNCH_OK("conv3d_igemm_kernel");
   return PV_OK;
 }
 

@@ -396,14 +396,18 @@ int conv3d_gather_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
     cfg.attrs = attr;
     cfg.numAttrs = use_pdl ? 1 : 0;
     const __half* xh = (const __half*)x;
+#define PV_GG_LAUNCH(BN)                                                                                 \
+  PV_OPT_IN_SMEM(conv3d_igemm_gather_kernel<BN>, 225 * 1024);                                            \
+  PV_CUDA_OK(cudaLaunchKernelEx(&cfg, conv3d_igemm_gather_kernel<BN>, P, xh, scale, bias));              \
+  PV_LAUNCH_OK("conv3d_igemm_gather_kernel<" #BN ">");
     switch (P.block_n) {
-      case 16: PV_OPT_IN_SMEM(conv3d_igemm_gather_kernel<16>, 225 * 1024); PV_CUDA_OK(cudaLaunchKernelEx(&cfg, conv3d_igemm_gather_kernel<16>, P, xh, scale, bias)); break;
-      case 32: PV_OPT_IN_SMEM(conv3d_igemm_gather_kernel<32>, 225 * 1024); PV_CUDA_OK(cudaLaunchKernelEx(&cfg, conv3d_igemm_gather_kernel<32>, P, xh, scale, bias)); break;
-      case 64: PV_OPT_IN_SMEM(conv3d_igemm_gather_kernel<64>, 225 * 1024); PV_CUDA_OK(cudaLaunchKernelEx(&cfg, conv3d_igemm_gather_kernel<64>, P, xh, scale, bias)); break;
-      default: PV_OPT_IN_SMEM(conv3d_igemm_gather_kernel<128>, 225 * 1024); PV_CUDA_OK(cudaLaunchKernelEx(&cfg, conv3d_igemm_gather_kernel<128>, P, xh, scale, bias)); break;
+      case 16: PV_GG_LAUNCH(16) break;
+      case 32: PV_GG_LAUNCH(32) break;
+      case 64: PV_GG_LAUNCH(64) break;
+      default: PV_GG_LAUNCH(128) break;
     }
+#undef PV_GG_LAUNCH
   }
-  PV_LAUNCH_OK("conv3d_igemm_gather_kernel");
   return PV_OK;
 }
 

@@ -1033,13 +1033,15 @@ int conv3d_direct_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
     PV_CHECK_ARG((d->x_row_stride * esz) % (4 * esz) == 0 && (d->y_row_stride % 4) == 0,
                  "row strides must be multiples of 4 elements");
     dim3 grid((unsigned)cdiv(M, DC_BM), (unsigned)cdiv(d->Co, DC_BN)), block(256);
-    if (d->dtype == PV_F16)
+    if (d->dtype == PV_F16) {
       conv3d_direct_kernel<__half><<<grid, block, 0, s>>>(*d, (const __half*)x, (const __half*)w, scale, bias,
                                                        (const __half*)residual, (__half*)y, M);
-    else
+      PV_LAUNCH_OK("conv3d_direct_kernel<__half>");
+    } else {
       conv3d_direct_kernel<float><<<grid, block, 0, s>>>(*d, (const float*)x, (const float*)w, scale, bias,
                                                       (const float*)residual, (float*)y, M);
-    PV_LAUNCH_OK("conv3d_direct_kernel");
+      PV_LAUNCH_OK("conv3d_direct_kernel<float>");
+    }
   } else {
     PV_CHECK_ARG(d->Co % 8 == 0, "depthwise conv needs C%%8==0");
     PV_CHECK_ARG(d->x_row_stride % 8 == 0 && d->y_row_stride % 8 == 0, "row strides must be multiples of 8");
@@ -1053,7 +1055,11 @@ int conv3d_direct_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
       const int wo4 = (d->Wo + 3) / 4;
       const long long tot4 = (long long)d->N * d->To * d->Ho * wo4 * (d->Co / 8);
       dim3 g4((unsigned)cdiv(tot4, 128)), b4(128);
-#define PV_DW(TT, KW_, SW_) dwconv3d_w4_kernel<TT, KW_, SW_><<<g4, b4, 0, s>>>(*d, (const TT*)x, (const TT*)w, scale, bias, (TT*)y, tot4, wo4)
+#define PV_DW(TT, KW_, SW_)                                                                                            \
+  do {                                                                                                                 \
+    dwconv3d_w4_kernel<TT, KW_, SW_><<<g4, b4, 0, s>>>(*d, (const TT*)x, (const TT*)w, scale, bias, (TT*)y, tot4, wo4); \
+    PV_LAUNCH_OK("dwconv3d_w4_kernel<" #TT "," #KW_ "," #SW_ ">");                                                     \
+  } while (0)
       if (d->dtype == PV_F16) {
         if (d->kw == 3 && d->sw == 1) PV_DW(__half, 3, 1); else if (d->kw == 3) PV_DW(__half, 3, 2);
         else if (d->sw == 1) PV_DW(__half, 1, 1); else PV_DW(__half, 1, 2);
@@ -1062,18 +1068,19 @@ int conv3d_direct_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
         else if (d->sw == 1) PV_DW(float, 1, 1); else PV_DW(float, 1, 2);
       }
 #undef PV_DW
-      PV_LAUNCH_OK("dwconv3d_w4_kernel");
       return PV_OK;
     }
     const long long total = M * (d->Co / 8);
     dim3 grid((unsigned)cdiv(total, 256)), block(256);
-    if (d->dtype == PV_F16)
+    if (d->dtype == PV_F16) {
       dwconv3d_kernel<__half><<<grid, block, 0, s>>>(*d, (const __half*)x, (const __half*)w, scale, bias,
                                                   (const __half*)residual, (__half*)y, total);
-    else
+      PV_LAUNCH_OK("dwconv3d_kernel<__half>");
+    } else {
       dwconv3d_kernel<float><<<grid, block, 0, s>>>(*d, (const float*)x, (const float*)w, scale, bias,
                                                  (const float*)residual, (float*)y, total);
-    PV_LAUNCH_OK("dwconv3d_kernel");
+      PV_LAUNCH_OK("dwconv3d_kernel<float>");
+    }
   }
   return PV_OK;
 }

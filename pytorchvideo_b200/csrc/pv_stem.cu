@@ -277,16 +277,16 @@ extern "C" int pv_conv3d_stem_rows_fwd(const pv_conv3d_desc* d, const void* x, c
   if (block_n == BN && P.win == 16 * KS) {                                                                \
     PV_OPT_IN_SMEM((conv3d_stem_rows_kernel<BN, KS>), 227 * 1024);                                        \
     PV_CUDA_OK(cudaLaunchKernelEx(&cfg, conv3d_stem_rows_kernel<BN, KS>, P, xb, wb, zb, scale, bias));    \
-    launched = true;                                                                                      \
+    name = "conv3d_stem_rows_kernel<" #BN "," #KS ">";                                                     \
   }
-    bool launched = false;
+    const char* name = nullptr;
     PV_ST_LAUNCH(16, 1) PV_ST_LAUNCH(16, 2) PV_ST_LAUNCH(16, 4)
     PV_ST_LAUNCH(32, 1) PV_ST_LAUNCH(32, 2) PV_ST_LAUNCH(32, 4)
     PV_ST_LAUNCH(64, 1) PV_ST_LAUNCH(64, 2) PV_ST_LAUNCH(64, 4)
     PV_ST_LAUNCH(128, 1) PV_ST_LAUNCH(128, 2) PV_ST_LAUNCH(128, 4)
 #undef PV_ST_LAUNCH
-    if (!launched) { set_error("internal: no stem instance for BN=%d win=%d", block_n, P.win); return PV_ERR_INVALID; }
+    if (!name) { set_error("internal: no stem instance for BN=%d win=%d", block_n, P.win); return PV_ERR_INVALID; }
+    PV_LAUNCH_OK(name);
   }
-  PV_LAUNCH_OK("conv3d_stem_rows_kernel");
   return PV_OK;
 }

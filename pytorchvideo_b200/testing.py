@@ -260,3 +260,61 @@ def roi_align_case(seed=5):
     boxes = synthetic_boxes(7, 2, 144, 176, seed=seed + 1)
     settings = [((7, 7), 1.0 / 16.0, 0), ((7, 7), 1.0 / 16.0, 2), ((3, 5), 0.25, 0), ((1, 1), 1.0 / 16.0, 3)]
     return x, boxes, settings
+
+
+# ---- kernel-instance ledger and a float64 comparator for the kernel tests -----------------------------------------
+def kernel_counts():
+    """Snapshot of the library's per-instance launch counts ({"conv3d_igemm_kernel<64,128>": 3, ...})."""
+    from . import _lib
+    return _lib.kernel_counts()
+
+
+def kernel_count_diff(before, after):
+    """Launches per instance between two kernel_counts() snapshots (instances that did not launch are left out)."""
+    return {k: n - before.get(k, 0) for k, n in sorted(after.items()) if n != before.get(k, 0)}
+
+
+def launched_kernels(fn, *args, **kwargs):
+    """Run fn(*args, **kwargs) and return (its result, {instance: launches} of the library kernels it ran)."""
+    before = kernel_counts()
+    out = fn(*args, **kwargs)
+    return out, kernel_count_diff(before, kernel_counts())
+
+
+F16_EPS = 2.0 ** -11          # unit roundoff of f16 (one round-to-nearest of the stored result)
+ACC_EPS = 2.0 ** -20          # fp32 accumulation allowance per unit of |x|.|w| magnitude, see assert_close_to_f64
+
+
+def assert_close_to_f64(got, ref64, absref64, k_len, acc_eps=ACC_EPS, what=""):
+    """Compare an f16-storage kernel result with its float64 reference.
+
+    ref64: the operation in float64 on the exact f16-grid operands the kernel received.  absref64: the same operation
+    on |x| and |w| with |scale|, plus |bias| and |residual| - the magnitude the result is summed from.  Each element
+    may differ from ref64 by one f16 rounding of the stored result (2^-11 |ref|) plus an fp32 accumulation term
+    proportional to absref64 that grows with the reduction length K, plus half the smallest f16 subnormal step.
+    Rounding must also be unbiased: over the normal-range elements the mean error in the direction of |ref| must stay
+    well below the mean rounding step (truncation toward zero moves it to about -0.7 of a step).  Returns
+    (largest err / tol, largest share of the accumulation term used): a correctly rounded result may use nearly all of
+    the rounding term, so the second number is the margin of the accumulation constant."""
+    got64 = got.detach().double().cpu()
+    ref64, absref64 = ref64.double().cpu(), absref64.double().cpu()
+    assert got64.shape == ref64.shape, (what, tuple(got64.shape), tuple(ref64.shape))
+    assert bool(torch.isfinite(got64).all()), "%s: non-finite output" % what
+    err = got64 - ref64
+    tol = F16_EPS * ref64.abs() + acc_eps * (1.0 + k_len / 64.0) * absref64 + 2.0 ** -24
+    ratio = (err.abs() / tol)
+    worst = int(ratio.argmax())
+    acc = acc_eps * (1.0 + k_len / 64.0) * absref64
+    excess = (err.abs() - F16_EPS * ref64.abs() - 2.0 ** -24).clamp_min(0)
+    acc_ratio = float((excess / acc.clamp_min(1e-300)).max()) if bool((acc > 0).any()) else 0.0
+    assert float(ratio.max()) <= 1.0, "%s: err/tol %.3g at flat index %d (got %r, ref %r, absref %r)" % (
+        what, float(ratio.max()), worst, float(got64.reshape(-1)[worst]), float(ref64.reshape(-1)[worst]),
+        float(absref64.reshape(-1)[worst]))
+    normal = ref64.abs() >= 2.0 ** -14
+    n = int(normal.sum())
+    if n >= 256:
+        bias = float((err[normal] * ref64[normal].sign()).mean())
+        step = F16_EPS * float(ref64[normal].abs().mean())
+        limit = 0.25 * step + acc_eps * float(absref64[normal].mean())
+        assert abs(bias) <= limit, "%s: mean signed error %.3g exceeds %.3g (biased rounding)" % (what, bias, limit)
+    return float(ratio.max()), acc_ratio

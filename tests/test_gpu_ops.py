@@ -111,7 +111,8 @@ DW_CASES = [
     (1, 216, 3, 28, 28, (3, 3, 3), (1, 2, 2), (1, 1, 1)),    # stride 2 -> 14x14
     (2, 112, 3, 28, 28, (3, 3, 3), (1, 1, 1), (1, 1, 1)),    # 4x4 patches, two chunks of 56
     (1, 54, 5, 56, 56, (3, 3, 3), (1, 1, 1), (1, 1, 1)),     # X3D-M res2 plane (54 -> 56 padded channels)
-    # streaming temporal kernel (kt x 1 x 1): prefetch ring longer than the clip, T = 1, 3-tap
+    # kt x 1 x 1 with SE sums runs the TMA tile kernel (the streaming temporal kernel takes no SE sums; its own rows,
+    # same shapes without SE sums, are in tests/test_gpu_kernel_matrix.py): ring longer than the clip, T = 1, 3-tap
     (1, 40, 5, 9, 9, (3, 1, 1), (1, 1, 1), (1, 0, 0)),
     (1, 16, 1, 6, 6, (5, 1, 1), (1, 1, 1), (2, 0, 0)),
     (2, 24, 16, 28, 28, (5, 1, 1), (1, 1, 1), (2, 0, 0)),    # X3D stem geometry (16 frames)
