@@ -236,6 +236,12 @@ int pv_conv3d_stem_rows_fwd(const pv_conv3d_desc* d, const void* x, const void* 
  * x, y: NDHWC f16; weights f16 packed [n][k], k = tap * C + ci, K zero-padded to a multiple of 16:
  *   wa [Cmid][pad16(kt*Cin)], wb [Cmid][pad16(9*Cmid)], wc [Cout][pad16(Cmid)], wsc [Cout][pad16(Cin)] (or NULL);
  * folded BatchNorm (scale, bias) fp32 per output channel for each of the four convolutions.
+ * Supported: the instantiated (Cin, Cmid, kt, sb, shortcut) combinations, row strides that are multiples of 8, and
+ * H*W*x_row_stride and Ho*Wo*y_row_stride below 2^31 (in-frame offsets are 32-bit).  pv_bottleneck_fused_fwd also
+ * requires 16-byte aligned x, y, wa, wb, wc and (with a projection shortcut) wsc, else PV_ERR_INVALID.
+ * pv_bottleneck_fused_tiling is the host-only tile search pv_bottleneck_fused_fwd itself uses: for a device with
+ * sm_count SMs, each CTA computes a tile_h x tile_w output tile of frames_per_cta consecutive frames of one clip
+ * (the last frame chunk of a clip may be shorter) with smem_bytes of dynamic shared memory.
  * ------------------------------------------------------------------------------------------- */
 typedef struct pv_bottleneck_desc {
   int N, T, H, W;            /* input extents; output (T, (H-1)/sb+1, (W-1)/sb+1)                 */
@@ -250,6 +256,8 @@ int pv_bottleneck_fused_fwd(const pv_bottleneck_desc* d, const void* x, const vo
                             const void* wc, const void* wsc, const float* sa, const float* ba,
                             const float* sb, const float* bb, const float* sc, const float* bc,
                             const float* ssc, const float* bsc, void* y, void* stream);
+int pv_bottleneck_fused_tiling(const pv_bottleneck_desc* d, int sm_count, int* tile_h, int* tile_w,
+                               int* frames_per_cta, long long* smem_bytes);
 
 /* ---------------------------------------------------------------------------------------------
  * Pooling. nn.MaxPool3d stem pool (models/stem.py:94-100), nn.AvgPool3d head pools

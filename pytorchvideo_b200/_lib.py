@@ -106,6 +106,8 @@ SIGNATURES = {
     "pv_conv3d_stem_rows_fwd": (C.c_int, [C.POINTER(Conv3dDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_bottleneck_fused_supported": (C.c_int, [C.POINTER(BottleneckDesc)]),
     "pv_bottleneck_fused_fwd": (C.c_int, [C.POINTER(BottleneckDesc)] + [c_vp] * 15),
+    "pv_bottleneck_fused_tiling": (C.c_int, [C.POINTER(BottleneckDesc), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                             C.POINTER(C.c_int), C.POINTER(c_ll)]),
     "pv_pool3d_fwd": (C.c_int, [C.POINTER(Pool3dDesc), c_vp, c_vp, c_vp]),
     "pv_channel_sum": (C.c_int, [c_vp, C.c_int, c_ll, C.c_int, c_ll, C.c_int, c_vp, c_vp]),
     "pv_se_gate": (C.c_int, [c_vp, c_ll, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp,

@@ -439,18 +439,18 @@ extern "C" int pv_bottleneck_fused_supported(const pv_bottleneck_desc* d) {
   if (!d->has_shortcut && (d->Cin != d->Cout || d->sb != 1)) return 0;
   if (!(d->act == PV_ACT_RELU || d->act == PV_ACT_NONE)) return 0;
   if (d->x_row_stride % 8 || d->y_row_stride % 8 || d->x_row_stride < d->Cin || d->y_row_stride < d->Cout) return 0;
-  if ((long long)d->H * d->W * d->x_row_stride >= (1ll << 31)) return 0;       // 32-bit in-frame offsets
+  if (d->N < 0 || d->T <= 0 || d->H <= 0 || d->W <= 0) return 0;       // (T = 0 would divide by zero below)
+  // the kernel keeps in-frame element offsets of x and y in 32-bit tables
+  if ((long long)d->H * d->W * d->x_row_stride >= (1ll << 31)) return 0;
+  const long long Ho = (d->H - 1) / d->sb + 1, Wo = (d->W - 1) / d->sb + 1;
+  if (Ho * Wo * d->y_row_stride >= (1ll << 31)) return 0;
   return 1;
 }
 
-extern "C" int pv_bottleneck_fused_fwd(const pv_bottleneck_desc* d, const void* x, const void* wa, const void* wb,
-                                       const void* wc, const void* wsc, const float* sa, const float* ba,
-                                       const float* sb_, const float* bb, const float* sc, const float* bc,
-                                       const float* ssc, const float* bsc, void* y, void* stream) {
-  PV_CHECK_ARG(d && x && wa && wb && wc && sa && ba && sb_ && bb && sc && bc && y, "null argument");
-  if (!pv_bottleneck_fused_supported(d)) { set_error("fused bottleneck: unsupported configuration"); return PV_ERR_UNSUPPORTED; }
-  PV_CHECK_ARG(!d->has_shortcut || (wsc && ssc && bsc), "shortcut weights missing");
-  FbParams P;
+namespace {
+// The launch geometry of a supported descriptor on a device with sm_count SMs: tile, frame chunk, shared-memory
+// carve-up.  Host-only; pv_bottleneck_fused_fwd and pv_bottleneck_fused_tiling both use it.
+int fb_plan(const pv_bottleneck_desc* d, int sm_count, FbParams& P, size_t& smem_bytes) {
   memset(&P, 0, sizeof(P));
   P.N = d->N; P.T = d->T; P.H = d->H; P.W = d->W;
   P.Ho = (d->H + 2 - 3) / d->sb + 1; P.Wo = (d->W + 2 - 3) / d->sb + 1;
@@ -458,8 +458,6 @@ extern "C" int pv_bottleneck_fused_fwd(const pv_bottleneck_desc* d, const void* 
   P.xrs = d->x_row_stride; P.yrs = d->y_row_stride;
   P.KA = fb_pad16(d->kt * d->Cin); P.KB = fb_pad16(9 * d->Cmid); P.KC = fb_pad16(d->Cmid); P.KS = fb_pad16(d->Cin);
   P.ldwa = P.KA + 8; P.ldwb = P.KB + 8; P.ldwc = P.KC + 8; P.ldws = P.KS + 8;
-  const int sm_count = current_sm_count();
-  if (sm_count <= 0) { set_error("cannot query the SM count"); return PV_ERR_CUDA; }
   // ---- tile search: efficient tiles (little halo / m-tile padding) that still give every SM a few CTAs
   const size_t w_bytes = ((size_t)d->Cmid * P.ldwa + (size_t)d->Cmid * P.ldwb + (size_t)d->Cout * P.ldwc +
                           (d->has_shortcut ? (size_t)d->Cout * P.ldws : 0)) * 2;
@@ -496,7 +494,6 @@ extern "C" int pv_bottleneck_fused_fwd(const pv_bottleneck_desc* d, const void* 
   P.RH = (P.TH - 1) * d->sb + 3; P.RW = (P.TW - 1) * d->sb + 3;
   P.tiles_h = (int)cdiv(P.Ho, P.TH); P.tiles_w = (int)cdiv(P.Wo, P.TW);
   P.tchunks = (int)cdiv(d->T, P.TC);
-  size_t smem_bytes = 0;
   {
     unsigned off = 0;
     auto take = [&](size_t bytes) { const unsigned o = off; off += (unsigned)((bytes + 127) & ~(size_t)127); return o; };
@@ -513,6 +510,44 @@ extern "C" int pv_bottleneck_fused_fwd(const pv_bottleneck_desc* d, const void* 
     P.off_tab = take(512 * sizeof(int));
     smem_bytes = off;
   }
+  return PV_OK;
+}
+
+bool fb_aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
+}  // namespace
+
+extern "C" int pv_bottleneck_fused_tiling(const pv_bottleneck_desc* d, int sm_count, int* tile_h, int* tile_w,
+                                          int* frames_per_cta, long long* smem_bytes) {
+  PV_CHECK_ARG(d && sm_count > 0, "null descriptor or sm_count <= 0");
+  if (!pv_bottleneck_fused_supported(d)) { set_error("fused bottleneck: unsupported configuration"); return PV_ERR_UNSUPPORTED; }
+  FbParams P;
+  size_t smem = 0;
+  const int rc = fb_plan(d, sm_count, P, smem);
+  if (rc != PV_OK) return rc;
+  if (tile_h) *tile_h = P.TH;
+  if (tile_w) *tile_w = P.TW;
+  if (frames_per_cta) *frames_per_cta = P.TC;
+  if (smem_bytes) *smem_bytes = (long long)smem;
+  return PV_OK;
+}
+
+extern "C" int pv_bottleneck_fused_fwd(const pv_bottleneck_desc* d, const void* x, const void* wa, const void* wb,
+                                       const void* wc, const void* wsc, const float* sa, const float* ba,
+                                       const float* sb_, const float* bb, const float* sc, const float* bc,
+                                       const float* ssc, const float* bsc, void* y, void* stream) {
+  PV_CHECK_ARG(d && x && wa && wb && wc && sa && ba && sb_ && bb && sc && bc && y, "null argument");
+  if (!pv_bottleneck_fused_supported(d)) { set_error("fused bottleneck: unsupported configuration"); return PV_ERR_UNSUPPORTED; }
+  PV_CHECK_ARG(!d->has_shortcut || (wsc && ssc && bsc), "shortcut weights missing");
+  // x is read with 16-byte cp.async, y written and the weights loaded as uint4
+  PV_CHECK_ARG(fb_aligned16(x) && fb_aligned16(y) && fb_aligned16(wa) && fb_aligned16(wb) && fb_aligned16(wc) &&
+                   (!d->has_shortcut || fb_aligned16(wsc)),
+               "fused bottleneck: x, y and the weights must be 16-byte aligned");
+  const int sm_count = current_sm_count();
+  if (sm_count <= 0) { set_error("cannot query the SM count"); return PV_ERR_CUDA; }
+  FbParams P;
+  size_t smem_bytes = 0;
+  const int rc = fb_plan(d, sm_count, P, smem_bytes);
+  if (rc != PV_OK) return rc;
   const long long grid = (long long)d->N * P.tchunks * P.tiles_h * P.tiles_w;
   if (grid <= 0) return PV_OK;
   PV_CHECK_ARG(grid < (1ll << 31), "grid too large");
@@ -523,7 +558,7 @@ extern "C" int pv_bottleneck_fused_fwd(const pv_bottleneck_desc* d, const void* 
     bottleneck_fused_kernel<CI, CM, KT_, SB_, (SC_ != 0)><<<(unsigned)grid, FB_THREADS, smem_bytes, s>>>(           \
         P, (const __half*)x, (const __half*)wa, (const __half*)wb, (const __half*)wc, (const __half*)wsc, sa, ba,   \
         sb_, bb, sc, bc, ssc, bsc, (__half*)y);                                                                     \
-    PV_LAUNCH_OK("bottleneck_fused_kernel");                                                                        \
+    PV_LAUNCH_OK("bottleneck_fused_kernel<" #CI "," #CM "," #KT_ "," #SB_ "," #SC_ ">");                            \
     return PV_OK;                                                                                                   \
   }
   PV_FB(8, 8, 3, 1, 1) PV_FB(32, 8, 3, 1, 0) PV_FB(32, 8, 1, 1, 0)

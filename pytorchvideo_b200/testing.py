@@ -285,28 +285,42 @@ F16_EPS = 2.0 ** -11          # unit roundoff of f16 (one round-to-nearest of th
 ACC_EPS = 2.0 ** -20          # fp32 accumulation allowance per unit of |x|.|w| magnitude, see assert_close_to_f64
 
 
-def assert_close_to_f64(got, ref64, absref64, k_len, acc_eps=ACC_EPS, what=""):
+def assert_close_to_f64(got, ref64, absref64, k_len, acc_eps=ACC_EPS, what="", extra64=None):
     """Compare an f16-storage kernel result with its float64 reference.
 
     ref64: the operation in float64 on the exact f16-grid operands the kernel received.  absref64: the same operation
     on |x| and |w| with |scale|, plus |bias| and |residual| - the magnitude the result is summed from.  Each element
     may differ from ref64 by one f16 rounding of the stored result (2^-11 |ref|) plus an fp32 accumulation term
     proportional to absref64 that grows with the reduction length K, plus half the smallest f16 subnormal step.
+    extra64 (optional, same shape): a further per-element allowance, the error of rounded intermediates propagated to
+    the result (fused kernels that keep intermediates in f16, see fused_block_ref64 in the kernel-matrix tests).
     Rounding must also be unbiased: over the normal-range elements the mean error in the direction of |ref| must stay
-    well below the mean rounding step (truncation toward zero moves it to about -0.7 of a step).  Returns
-    (largest err / tol, largest share of the accumulation term used): a correctly rounded result may use nearly all of
-    the rounding term, so the second number is the margin of the accumulation constant."""
+    well below the mean rounding step (truncation toward zero moves it to about -0.7 of a step).  extra64 does not
+    enter that limit: it is a worst case (every rounding of every intermediate at its extreme, all with the same sign),
+    while the intermediates are rounded to nearest, so their share of the mean signed error is zero-mean noise that
+    shrinks like 1 / sqrt(n).  Charging the worst case would hide a truncated intermediate, whose bias is what the
+    check must see.  Returns (largest err / tol,
+    largest share of the accumulation term used, largest share of extra64 used): a correctly rounded result may use
+    nearly all of the rounding term, so the second number is the margin of the accumulation constant; the third
+    charges everything beyond the rounding term to extra64 (0.0 without extra64)."""
     got64 = got.detach().double().cpu()
     ref64, absref64 = ref64.double().cpu(), absref64.double().cpu()
     assert got64.shape == ref64.shape, (what, tuple(got64.shape), tuple(ref64.shape))
     assert bool(torch.isfinite(got64).all()), "%s: non-finite output" % what
     err = got64 - ref64
-    tol = F16_EPS * ref64.abs() + acc_eps * (1.0 + k_len / 64.0) * absref64 + 2.0 ** -24
+    acc = acc_eps * (1.0 + k_len / 64.0) * absref64
+    tol = F16_EPS * ref64.abs() + acc + 2.0 ** -24
+    if extra64 is not None:
+        extra64 = extra64.double().cpu()
+        assert extra64.shape == ref64.shape and bool((extra64 >= 0).all()), what
+        tol = tol + extra64
     ratio = (err.abs() / tol)
     worst = int(ratio.argmax())
-    acc = acc_eps * (1.0 + k_len / 64.0) * absref64
     excess = (err.abs() - F16_EPS * ref64.abs() - 2.0 ** -24).clamp_min(0)
     acc_ratio = float((excess / acc.clamp_min(1e-300)).max()) if bool((acc > 0).any()) else 0.0
+    extra_ratio = 0.0
+    if extra64 is not None and bool((extra64 > 0).any()):
+        extra_ratio = float((excess / extra64.clamp_min(1e-300)).max())
     assert float(ratio.max()) <= 1.0, "%s: err/tol %.3g at flat index %d (got %r, ref %r, absref %r)" % (
         what, float(ratio.max()), worst, float(got64.reshape(-1)[worst]), float(ref64.reshape(-1)[worst]),
         float(absref64.reshape(-1)[worst]))
@@ -317,4 +331,4 @@ def assert_close_to_f64(got, ref64, absref64, k_len, acc_eps=ACC_EPS, what=""):
         step = F16_EPS * float(ref64[normal].abs().mean())
         limit = 0.25 * step + acc_eps * float(absref64[normal].mean())
         assert abs(bias) <= limit, "%s: mean signed error %.3g exceeds %.3g (biased rounding)" % (what, bias, limit)
-    return float(ratio.max()), acc_ratio
+    return float(ratio.max()), acc_ratio, extra_ratio

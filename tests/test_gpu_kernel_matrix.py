@@ -12,6 +12,12 @@ accumulation constant; a correctly rounded f16 result may use nearly all of the 
   igemm 0.992 (0.017), window-mode igemm 0.920 (0.011), gather 0.989 (0.011), stem rows incl. the factored temporal
   stem 0.990 (0.133), depthwise 0.995 (0.020), attention wgmma 0.196 (0.097), attention mma 0.180 (0.092),
   attention CUDA-core f16 / f32 0.142 / 0.0003 (0.0001).
+
+The fused bottleneck block keeps its intermediates a and b in f16, so its bound also carries their rounding error
+propagated to y (fused_block_ref64).  Measured on an NVIDIA H100 80GB HBM3 (132 SMs, 700 W power limit) over every
+FUSED_ROWS and poison row: largest err / tol 0.583, largest share of the propagated term used 0.310 (charging all
+error beyond y's own rounding to it).  The accumulation share is not meaningful there: the f16 intermediates, not
+the fp32 sums, make up nearly all of the error.
 """
 import ctypes as C
 import math
@@ -622,6 +628,303 @@ def test_depthwise_cls_row_batch_stride(k, s, se):
         assert bool(((got_s - ref_s).abs() <= tol + 2.0 ** -22 * ref_s.abs()).all())
 
 
+# ---- fused bottleneck block (csrc/pv_fastblock.cu) -----------------------------------------------------------------
+# One launch per ResBlock: a = relu(bn_a(conv_a(x))) (kt,1,1); b = relu(bn_b(conv_b(a))) (1,3,3) stride (1,s,s);
+# y = act(bn_c(conv_c(b)) + shortcut).  The instance is bottleneck_fused_kernel<Cin,Cmid,kt,s,projection>.  Tile
+# (TH x TW outputs) and frame chunk (TC frames per CTA) come from a cost model over the SM count
+# (pv_bottleneck_fused_tiling); each row claims the tiling properties it is there for, and the test checks them with
+# the query at the device's SM count (test_fused_row_claims_hold checks them for 132- and 114-SM parts on the CPU):
+#   partial_h / partial_w  the last tile row / column of the plane is cut by the image edge
+#   chunks                 a clip is split over several CTAs, each of which reloads its halo frame
+#   short_chunk            ... and the last chunk holds fewer frames than the others
+#   single_tile            the whole plane is one tile (its halo is image border on every side)
+def _fb(cin, cmid, kt, s, proj):
+    return "bottleneck_fused_kernel<%d,%d,%d,%d,%d>" % (cin, cmid, kt, s, proj)
+
+
+FB_RES2_0, FB_RES2, FB_PW = _fb(8, 8, 3, 1, 1), _fb(32, 8, 3, 1, 0), _fb(32, 8, 1, 1, 0)
+FB_RES3_0, FB_PROJ16, FB_RES3 = _fb(32, 16, 3, 2, 1), _fb(32, 16, 3, 1, 1), _fb(64, 16, 3, 1, 0)
+PH, PW, CH, SC, ST = "partial_h", "partial_w", "chunks", "short_chunk", "single_tile"
+
+# (expected instance, N, T, H, W, act, extra x row elements, extra y row elements, claimed tiling properties)
+FUSED_ROWS = [
+    # partial tiles in both directions, several frame chunks and a short last chunk
+    (FB_RES2_0, 1, 9, 10, 9, "relu", 0, 0, (PH, PW, CH, SC)),
+    (FB_RES2, 1, 9, 10, 9, None, 8, 0, (PH, PW, CH, SC)),
+    (FB_PW, 1, 9, 9, 11, "relu", 0, 8, (PH, PW, CH, SC)),
+    (FB_RES3_0, 1, 9, 9, 11, None, 0, 0, (PH, PW, CH, SC)),
+    (FB_PROJ16, 1, 9, 10, 9, "relu", 16, 8, (PH, PW, CH, SC)),
+    (FB_RES3, 1, 9, 10, 11, "relu", 0, 0, (PH, PW, CH, SC)),
+    # clips of 1 and 2 frames: both temporal neighbours of conv_a are padding
+    (FB_RES2_0, 2, 1, 1, 1, "relu", 0, 0, (ST,)),
+    (FB_RES2_0, 1, 2, 2, 3, None, 8, 8, (ST,)),
+    (FB_RES2, 1, 1, 1, 9, None, 0, 0, ()),
+    (FB_RES2, 2, 2, 5, 6, "relu", 0, 0, ()),
+    (FB_RES3_0, 1, 1, 1, 1, "relu", 0, 0, (ST,)),
+    (FB_RES3_0, 2, 2, 2, 3, None, 8, 0, (ST,)),
+    (FB_PROJ16, 1, 1, 2, 3, None, 0, 0, (ST,)),
+    (FB_PROJ16, 2, 2, 1, 9, "relu", 0, 16, ()),
+    (FB_RES3, 1, 1, 1, 9, "relu", 0, 0, ()),
+    (FB_RES3, 1, 2, 1, 1, None, 16, 0, (ST,)),
+    # tiny planes; stride 2 with odd and even H and W
+    (FB_PW, 1, 3, 1, 1, None, 0, 0, (ST,)),
+    (FB_PW, 2, 4, 2, 3, "relu", 8, 8, (ST,)),
+    (FB_RES3_0, 1, 3, 4, 6, "relu", 0, 8, ()),
+    (FB_RES3_0, 1, 3, 5, 7, None, 0, 0, ()),
+    (FB_RES3_0, 1, 4, 6, 5, "relu", 8, 0, ()),
+    # SlowFast-R50 Fast pathway at batch 8 (32 frames): res2 block 0, res2 blocks 1-2, res3 block 0, res3 blocks 1-3
+    (FB_RES2_0, 8, 32, 56, 56, "relu", 0, 0, (CH, SC)),
+    (FB_RES2, 8, 32, 56, 56, "relu", 0, 0, (CH,)),
+    (FB_RES3_0, 8, 32, 56, 56, "relu", 0, 0, (PW, CH)),
+    (FB_RES3, 8, 32, 28, 28, "relu", 0, 0, (CH,)),
+]
+
+
+def _fused_row_id(row):
+    return "%s-%s-%s-x%d-y%d" % (row[0], "x".join(str(v) for v in row[1:5]), row[5] or "none", row[6], row[7])
+
+
+def _fused_shape(inst):
+    cin, cmid, kt, s, proj = (int(v) for v in re.match(r"bottleneck_fused_kernel<(\d+),(\d+),(\d+),(\d+),(\d+)>$",
+                                                       inst).groups())
+    return cin, cmid, 4 * cmid, kt, s, proj
+
+
+def _fused_desc(inst, N, T, H, W, act="relu", xrs=None, yrs=None):
+    from pytorchvideo_b200 import _lib as L
+    cin, cmid, cout, kt, s, proj = _fused_shape(inst)
+    d = L.BottleneckDesc()
+    d.N, d.T, d.H, d.W = N, T, H, W
+    d.Cin, d.Cmid, d.Cout, d.kt, d.sb, d.has_shortcut = cin, cmid, cout, kt, s, proj
+    d.act = L.ACT_RELU if act == "relu" else L.ACT_NONE
+    d.x_row_stride, d.y_row_stride = xrs or cin, yrs or cout
+    return d
+
+
+def fused_tiling(d, sm_count):
+    """(tile_h, tile_w, frames per CTA, shared-memory bytes) that pv_bottleneck_fused_fwd would use on sm_count SMs."""
+    from pytorchvideo_b200 import _lib as L
+    th, tw, tc, smem = C.c_int(), C.c_int(), C.c_int(), C.c_longlong()
+    L.check(L.load().pv_bottleneck_fused_tiling(C.byref(d), sm_count, C.byref(th), C.byref(tw), C.byref(tc),
+                                                C.byref(smem)), "pv_bottleneck_fused_tiling")
+    return th.value, tw.value, tc.value, smem.value
+
+
+def fused_tiling_properties(d, sm_count):
+    th, tw, tc, _ = fused_tiling(d, sm_count)
+    Ho, Wo = (d.H - 1) // d.sb + 1, (d.W - 1) // d.sb + 1
+    chunks = -(-d.T // tc)
+    props = set()
+    if Ho % th:
+        props.add(PH)
+    if Wo % tw:
+        props.add(PW)
+    if chunks > 1:
+        props.add(CH)
+        if d.T % tc:
+            props.add(SC)
+    if Ho <= th and Wo <= tw:
+        props.add(ST)
+    return props
+
+
+def _fused_operands(inst, N, T, H, W, seed):
+    """f16-grid x and weights, and the folded fp32 BatchNorm (scale, bias) of each convolution."""
+    cin, cmid, cout, kt, s, proj = _fused_shape(inst)
+    g = torch.Generator().manual_seed(seed)
+    x = TS.f16_exact(torch.randn(N, cin, T, H, W, generator=g))
+
+    def w(co, ci, k):
+        return TS.f16_exact(torch.randn(co, ci, *k, generator=g) * (2.0 / (ci * int(np.prod(k)))) ** 0.5)
+    wa, wb, wc = w(cmid, cin, (kt, 1, 1)), w(cmid, cmid, (1, 3, 3)), w(cout, cmid, (1, 1, 1))
+    ws = w(cout, cin, (1, 1, 1)) if proj else None
+    folds = []
+    for i, c in enumerate((cmid, cmid, cout, cout if proj else 0)):
+        folds += list(_scale_bias(_bn(c, seed + i), c)) if c else [None, None]
+    return x, wa, wb, wc, ws, tuple(folds)
+
+
+def _conv_bn(x, w, scale, bias, stride=1, padding=0):
+    return F.conv3d(x, w, None, stride, padding) * scale.view(1, -1, 1, 1, 1) + bias.view(1, -1, 1, 1, 1)
+
+
+def fused_block_ref64(x, wa, wb, wc, ws, folds, kt, sb, act):
+    """The fused block in float64 on the f16-grid operands and the exact fp32 folded BatchNorm the kernel uses.
+
+    Returns (y, A, B, Y, prop): y the result; A, B, Y the magnitude sums of a, b and y (the same sums over |x|, |w|,
+    |scale| and |bias|, plus |shortcut| for Y); prop the error of the kernel's f16 intermediates a and b propagated to
+    y.  Each intermediate may be off by one f16 rounding plus its fp32 accumulation term plus what it inherits (relu
+    is 1-Lipschitz, and a is exactly 0 outside the image where conv_b pads):
+      ea = F16_EPS |a| + ACC(Ka) A + 2^-24
+      eb = F16_EPS |b| + ACC(Kb) B + |sb| conv_b(ea, |wb|) + 2^-24
+      prop = |sc| conv_c(eb, |wc|)
+    with ACC(K) = 2^-20 (1 + K / 64).  The caller compares with assert_close_to_f64(got, y, Y, Kc + Ks, extra64=prop).
+    Runs on x's device."""
+    dev = x.device
+    f64 = [None if t is None else t.double().to(dev) for t in folds]
+    sa, ba, sbn, bbn, sc, bc, ssc, bsc = f64
+    x64 = x.double()
+    wa, wb, wc = (t.double().to(dev) for t in (wa, wb, wc))
+    pa, pb, st = (kt // 2, 0, 0), (0, 1, 1), (1, sb, sb)
+    cin, cmid = x.shape[1], wa.shape[0]
+
+    def acc(k):
+        return TS.ACC_EPS * (1.0 + k / 64.0)
+    a = _conv_bn(x64, wa, sa, ba, 1, pa).clamp_min(0)
+    A = _conv_bn(x64.abs(), wa.abs(), sa.abs(), ba.abs(), 1, pa)
+    b = _conv_bn(a, wb, sbn, bbn, st, pb).clamp_min(0)
+    B = _conv_bn(a, wb.abs(), sbn.abs(), bbn.abs(), st, pb)
+    ea = TS.F16_EPS * a + acc(kt * cin) * A + 2.0 ** -24
+    eb = (TS.F16_EPS * b + acc(9 * cmid) * B + sbn.abs().view(1, -1, 1, 1, 1) * F.conv3d(ea, wb.abs(), None, st, pb)
+          + 2.0 ** -24)
+    del ea
+    if ws is None:
+        short = x64[:, :, :, ::sb, ::sb]
+        S = short.abs()
+    else:
+        ws = ws.double().to(dev)
+        short = _conv_bn(x64, ws, ssc, bsc, st)
+        S = _conv_bn(x64.abs(), ws.abs(), ssc.abs(), bsc.abs(), st)
+    y = _act64(_conv_bn(b, wc, sc, bc) + short, act)
+    Y = _conv_bn(b, wc.abs(), sc.abs(), bc.abs()) + S
+    prop = sc.abs().view(1, -1, 1, 1, 1) * F.conv3d(eb, wc.abs())
+    return y, A, B, Y, prop
+
+
+def _fused_k(inst):
+    cin, cmid, cout, kt, s, proj = _fused_shape(inst)
+    return cmid + (cin if proj else 0)
+
+
+def _fused_call(d, x_ptr, y_ptr, dev_ops):
+    """pv_bottleneck_fused_fwd on raw device pointers; returns {instance: launches}."""
+    from pytorchvideo_b200 import _lib as L
+    wa, wb, wc, ws, sa, ba, sbn, bbn, sc, bc, ssc, bsc = dev_ops
+    p = lambda t: None if t is None else t.data_ptr()
+    before = TS.kernel_counts()
+    L.check(L.load().pv_bottleneck_fused_fwd(C.byref(d), x_ptr, p(wa), p(wb), p(wc), p(ws), p(sa), p(ba), p(sbn),
+                                             p(bbn), p(sc), p(bc), p(ssc), p(bsc), y_ptr,
+                                             torch.cuda.current_stream().cuda_stream), "pv_bottleneck_fused_fwd")
+    torch.cuda.synchronize()
+    return TS.kernel_count_diff(before, TS.kernel_counts())
+
+
+def _fused_device_operands(inst, wa, wb, wc, ws, folds):
+    from pytorchvideo_b200.engine import packing as PK
+    cin, cmid, cout, kt, s, proj = _fused_shape(inst)
+    packed = [PK.pack_rows_k16(wa, cin, cmid), PK.pack_rows_k16(wb, cmid, cmid), PK.pack_rows_k16(wc, cmid, cout),
+              PK.pack_rows_k16(ws, cin, cout) if ws is not None else None]
+    return tuple(None if t is None else t.to(_dev()) for t in packed + list(folds))
+
+
+def _fused_run(inst, x, dev_ops, act, xrs, yrs):
+    """x (NCDHW, f16 grid) -> (y NCDHW float on the device, launched); x and y in NDHWC buffers with the given rows."""
+    N, cin, T, H, W = x.shape
+    _, _, cout, _, s, _ = _fused_shape(inst)
+    Ho, Wo = (H - 1) // s + 1, (W - 1) // s + 1
+    xd = torch.zeros(N, T, H, W, xrs, dtype=torch.float16, device=_dev())
+    xd[..., :cin] = x.to(_dev()).permute(0, 2, 3, 4, 1).half()
+    yd = torch.zeros(N, T, Ho, Wo, yrs, dtype=torch.float16, device=_dev())
+    d = _fused_desc(inst, N, T, H, W, act, xrs, yrs)
+    launched = _fused_call(d, xd.data_ptr(), yd.data_ptr(), dev_ops)
+    return yd[..., :cout].permute(0, 4, 1, 2, 3).float(), launched
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("row", FUSED_ROWS, ids=[_fused_row_id(r) for r in FUSED_ROWS])
+def test_fused_instance(row):
+    from pytorchvideo_b200 import _lib as L
+    inst, N, T, H, W, act, xe, ye, claims = row
+    cin, cmid, cout, kt, s, proj = _fused_shape(inst)
+    sm, _ = L.require_device()
+    d = _fused_desc(inst, N, T, H, W, act, cin + xe, cout + ye)
+    props = fused_tiling_properties(d, sm)
+    assert set(claims) <= props, "row claims %s, tiling %s on %d SMs gives %s" % (claims, fused_tiling(d, sm), sm, props)
+    x, wa, wb, wc, ws, folds = _fused_operands(inst, N, T, H, W, seed=N + T * 3 + H * 5 + W * 7 + cin)
+    dev_ops = _fused_device_operands(inst, wa, wb, wc, ws, folds)
+    got, launched = _fused_run(inst, x, dev_ops, act, cin + xe, cout + ye)
+    assert launched == {inst: 1}, "expected %s, launched %s" % (inst, launched)
+    big = N * T * H * W > 100000
+    y, _, _, Y, prop = fused_block_ref64(x.to(_dev()) if big else x, wa, wb, wc, ws, folds, kt, s, act)
+    ratio = TS.assert_close_to_f64(got, y, Y, _fused_k(inst), what=inst, extra64=prop)
+    print("RATIO fused %s %.4f %.4f %.4f tiling=%s" % (_fused_row_id(row), ratio[0], ratio[1], ratio[2],
+                                                      fused_tiling(d, sm)[:3]))
+
+
+FUSED_POISON_ROWS = [
+    (FB_RES2_0, 2, 5, 9, 10, "relu"),
+    (FB_RES2, 1, 9, 10, 9, None),
+    (FB_RES3_0, 2, 4, 9, 11, "relu"),
+    (FB_RES3, 1, 6, 7, 13, None),
+]
+NAN16 = 0x7E00             # an f16 quiet NaN
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("row", FUSED_POISON_ROWS, ids=["%s-%s" % (r[0], "x".join(map(str, r[1:5]))) for r in FUSED_POISON_ROWS])
+def test_fused_poison_and_sentinel(row):
+    """x is a channel slice of wider rows between guard rows, and everything around it is f16 NaN: the kernel must
+    not read it (a NaN times a zero weight is still NaN).  y is a channel slice of a sentinel-filled buffer with
+    wider rows and guard rows: every byte outside the slice keeps its sentinel, and the slice matches float64."""
+    inst, N, T, H, W, act = row
+    cin, cmid, cout, kt, s, proj = _fused_shape(inst)
+    Ho, Wo = (H - 1) // s + 1, (W - 1) // s + 1
+    xrs, yrs, guard = cin + 8, cout + 16, 37
+    mx, my = N * T * H * W, N * T * Ho * Wo
+    x, wa, wb, wc, ws, folds = _fused_operands(inst, N, T, H, W, seed=101 + cin + H)
+    dev_ops = _fused_device_operands(inst, wa, wb, wc, ws, folds)
+    xb = torch.full((guard + mx + guard, xrs), NAN16, dtype=torch.int16).view(torch.float16)
+    xb[guard:guard + mx, :cin] = x.permute(0, 2, 3, 4, 1).reshape(mx, cin).half()
+    xg = xb.to(_dev())
+    yg = torch.full((guard + my + guard, yrs), SENTINEL, dtype=torch.int16).view(torch.float16).to(_dev())
+    d = _fused_desc(inst, N, T, H, W, act, xrs, yrs)
+    launched = _fused_call(d, xg.data_ptr() + guard * xrs * 2, yg.data_ptr() + guard * yrs * 2, dev_ops)
+    assert launched == {inst: 1}, launched
+    yb = yg.cpu().view(torch.int16)
+    inside = torch.zeros_like(yb, dtype=torch.bool)
+    inside[guard:guard + my, :cout] = True
+    assert bool((yb[~inside] == SENTINEL).all()), "the kernel wrote outside y's slice"
+    got16 = yg.cpu()[guard:guard + my, :cout]
+    assert not bool(torch.isnan(got16).any()), "NaN in y: the kernel read poisoned x bytes"
+    got = got16.float().view(N, T, Ho, Wo, cout).permute(0, 4, 1, 2, 3)
+    y, _, _, Y, prop = fused_block_ref64(x, wa, wb, wc, ws, folds, kt, s, act)
+    ratio = TS.assert_close_to_f64(got, y, Y, _fused_k(inst), what=inst, extra64=prop)
+    print("RATIO fused poison %s %.4f %.4f %.4f" % (inst, ratio[0], ratio[1], ratio[2]))
+
+
+# Rows where a batch of 8 clips and one clip alone choose different (TH, TW, TC): every output element's arithmetic
+# (mma K order, roundings of a and b) does not depend on which tile or frame chunk computes it, so clip i of the batch
+# must equal the clip run alone bit for bit; a difference is a tile, halo or chunk bug.
+FUSED_BATCH_ROWS = [
+    (FB_RES2_0, 32, 56, 56),
+    (FB_RES2, 32, 56, 56),
+    (FB_PW, 32, 56, 56),
+    (FB_RES3_0, 32, 56, 56),
+    (FB_PROJ16, 32, 56, 56),
+    (FB_RES3, 32, 28, 28),
+    (FB_RES3, 12, 17, 14),
+]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("row", FUSED_BATCH_ROWS, ids=["%s-%s" % (r[0], "x".join(map(str, r[1:]))) for r in FUSED_BATCH_ROWS])
+def test_fused_batch_invariance(row):
+    from pytorchvideo_b200 import _lib as L
+    inst, T, H, W = row
+    cin, cmid, cout, kt, s, proj = _fused_shape(inst)
+    sm, _ = L.require_device()
+    t8, t1 = fused_tiling(_fused_desc(inst, 8, T, H, W), sm)[:3], fused_tiling(_fused_desc(inst, 1, T, H, W), sm)[:3]
+    assert t8 != t1, (t8, t1)
+    x, wa, wb, wc, ws, folds = _fused_operands(inst, 8, T, H, W, seed=7 + cin + H)
+    dev_ops = _fused_device_operands(inst, wa, wb, wc, ws, folds)
+    y8, launched = _fused_run(inst, x, dev_ops, "relu", cin, cout)
+    assert launched == {inst: 1}, launched
+    for i in range(8):
+        y1, _ = _fused_run(inst, x[i:i + 1], dev_ops, "relu", cin, cout)
+        assert torch.equal(y8[i:i + 1], y1), "clip %d: batch tiling %s and single-clip tiling %s disagree at %d elements" % (
+            i, t8, t1, int((y8[i:i + 1] != y1).sum()))
+
+
 # ---- CPU: the instance ledger --------------------------------------------------------------------------------------
 UNREACHABLE = {
     # the wgmma kernel takes head dims 32 / 64 / 96 under the same alignment rules, so pv_attention_fwd never routes
@@ -660,10 +963,12 @@ def compiled_instances():
         out.add("attention_mma_kernel<%s>" % dd)
     for dd in re.findall(r"PV_ATT\((\d+)\)", src("pv_attention.cu")):
         out.update({"attention_kernel<__half,%s>" % dd, "attention_kernel<float,%s>" % dd})
+    for args in re.findall(r"PV_FB\((\d+), (\d+), (\d+), (\d+), (\d+)\)", src("pv_fastblock.cu")):
+        out.add("bottleneck_fused_kernel<%s>" % ",".join(args))
     return out
 
 
-EXPECTED_INSTANCES = {r[0] for r in IGEMM_ROWS + GATHER_ROWS + STEM_ROWS + WINDOW_ROWS + DW_ROWS + ATTN_ROWS}
+EXPECTED_INSTANCES = {r[0] for r in IGEMM_ROWS + GATHER_ROWS + STEM_ROWS + WINDOW_ROWS + DW_ROWS + ATTN_ROWS + FUSED_ROWS}
 
 
 def test_instance_ledger_covers_every_compiled_instance():
@@ -673,6 +978,7 @@ def test_instance_ledger_covers_every_compiled_instance():
     assert len([n for n in compiled if n.startswith("conv3d_igemm_gather_kernel<")]) == 4
     assert len([n for n in compiled if n.startswith("dwconv3d_tile_kernel<")]) == 4
     assert len([n for n in compiled if n.startswith("dwconv3d_lane_kernel<")]) == 16
+    assert len([n for n in compiled if n.startswith("bottleneck_fused_kernel<")]) == 6
     missing = sorted(compiled - EXPECTED_INSTANCES - set(UNREACHABLE))
     assert not missing, "compiled instances no matrix row reaches: %s" % missing
     assert not (set(UNREACHABLE) & EXPECTED_INSTANCES)
@@ -685,7 +991,8 @@ def test_launch_sites_name_their_instances():
                    ("pv_stem.cu", r'"conv3d_stem_rows_kernel<" #BN "," #KS ">"'),
                    ("pv_igemm_gather.cu", r'"conv3d_igemm_gather_kernel<" #BN ">"'),
                    ("pv_dwconv.cu", r'"dwconv3d_tile_kernel<" #KW_ "," #SW_ ">"'),
-                   ("pv_attention_wgmma.cu", r'"attention_wgmma_kernel<" #DD ">"')):
+                   ("pv_attention_wgmma.cu", r'"attention_wgmma_kernel<" #DD ">"'),
+                   ("pv_fastblock.cu", r'"bottleneck_fused_kernel<" #CI "," #CM "," #KT_ "," #SB_ "," #SC_ ">"')):
         assert pat in open(os.path.join(CSRC, f)).read(), f
 
 
@@ -812,3 +1119,180 @@ def test_comparator_rejects_kernel_bugs(mutation):
         got = _unrows(r, ref)
     with pytest.raises(AssertionError):
         TS.assert_close_to_f64(got.half().double() if mutation != "round_toward_zero" else got, ref, absref, K)
+
+
+# ---- CPU: the fused block's comparator has teeth -------------------------------------------------------------------
+# Two small cases with partial tiles and T = 5, each with thousands of normal-range outputs (so the bias check applies):
+# stride 1 with the identity shortcut, and stride 2 with a projection shortcut.
+FUSED_CPU_CASES = {
+    "identity": (FB_RES2, 1, 5, 7, 9),
+    "stride2_projection": (FB_RES3_0, 1, 5, 9, 7),
+}
+FUSED_CPU_CHUNK = 2          # frames per CTA of the emulated chunk-boundary bug
+FUSED_CPU_TILE_H = 4         # tile rows of the emulated edge-tile bug (H_out = 7 / 5: the last tile row is partial)
+
+
+def _h16(t):
+    return t.half().float()
+
+
+def fused_block_emulate(x, wa, wb, wc, ws, folds, kt, sb, act, mutation=None):
+    """The kernel's rounding points on the CPU: fp32 accumulation and BatchNorm, a and b stored as f16, y rounded to
+    f16.  `mutation` plants one kernel-specific bug (see test_fused_comparator_rejects_kernel_bugs)."""
+    sa, ba, sbn, bbn, sc, bc, ssc, bsc = folds
+    v = lambda t: t.view(1, -1, 1, 1, 1)
+    pa = kt // 2
+    x = x.float()
+    T = x.shape[2]
+    pad_b = (0, 1, 1)
+    if mutation == "edge_frame_replicated":              # conv_a repeats the first / last frame instead of zeros
+        a_pre = F.conv3d(F.pad(x, (0, 0, 0, 0, pa, pa), mode="replicate"), wa)
+    elif mutation == "halo_a_bn0":                        # a = relu(bn_a(0)) outside the image instead of 0
+        a_pre, pad_b = F.conv3d(F.pad(x, (1, 1, 1, 1)), wa, padding=(pa, 0, 0)), (0, 0, 0)
+    else:
+        a_pre = F.conv3d(x, wa, padding=(pa, 0, 0))
+    a = _h16((a_pre * v(sa) + v(ba)).clamp_min(0))
+    if mutation == "chunk_halo_zero":                    # a chunk's leading halo frame read as zeros
+        for t0 in range(FUSED_CPU_CHUNK, T, FUSED_CPU_CHUNK):
+            x2 = x.clone()
+            x2[:, :, t0 - 1] = 0
+            a[:, :, t0] = _h16((F.conv3d(x2, wa, padding=(pa, 0, 0)) * v(sa) + v(ba)).clamp_min(0))[:, :, t0]
+    if mutation == "drop_conv_b_tap":                    # the last (dh, dw) = (2, 2) tap of conv_b skipped
+        wb = wb.clone()
+        wb[:, :, :, 2, 2] = 0
+    b32 = (F.conv3d(a, wb, None, (1, sb, sb), pad_b) * v(sbn) + v(bbn)).clamp_min(0)
+    b = _h16(b32)
+    if mutation == "b_truncated":                        # b rounded toward zero instead of to nearest (b >= 0)
+        bits = b32.half().view(torch.int16)
+        b = torch.where(b > b32, (bits - 1).view(torch.float16), bits.view(torch.float16)).float()
+    xs = x
+    if mutation == "shortcut_prev_frame":                # the shortcut reads frame t-1 (ring slot off by one)
+        xs = torch.cat([torch.zeros_like(x[:, :, :1]), x[:, :, :-1]], 2)
+    if mutation == "stride2_shortcut_odd":               # the stride-2 shortcut samples 2i+1 instead of 2i
+        xs = F.pad(x[:, :, :, 1:, 1:], (0, 1, 0, 1))
+    xs = xs[:, :, :, ::sb, ::sb]
+    short = xs if ws is None else F.conv3d(xs, ws) * v(ssc) + v(bsc)
+    y = F.conv3d(b, wc) * v(sc) + v(bc) + short
+    y = _h16(y.clamp_min(0) if act == "relu" else y)
+    if mutation == "edge_tile_last_row":                 # the last row of the partial bottom tiles is not stored
+        assert y.shape[3] % FUSED_CPU_TILE_H
+        y[:, :, :, -1] = 0
+    return y
+
+
+def _fused_cpu_case(name, act):
+    inst, N, T, H, W = FUSED_CPU_CASES[name]
+    cin, cmid, cout, kt, s, proj = _fused_shape(inst)
+    x, wa, wb, wc, ws, folds = _fused_operands(inst, N, T, H, W, seed=5)
+    y, _, _, Y, prop = fused_block_ref64(x, wa, wb, wc, ws, folds, kt, s, act)
+    assert int((y.abs() >= 2.0 ** -14).sum()) >= 256
+    return inst, (x, wa, wb, wc, ws, folds, kt, s, act), y, Y, prop
+
+
+@pytest.mark.parametrize("act", ["relu", None])
+@pytest.mark.parametrize("case", sorted(FUSED_CPU_CASES))
+def test_fused_comparator_accepts_the_kernel_rounding(case, act):
+    inst, args, y, Y, prop = _fused_cpu_case(case, act)
+    got = fused_block_emulate(*args)
+    ratio = TS.assert_close_to_f64(got, y, Y, _fused_k(inst), what=case, extra64=prop)
+    print("RATIO fused emulation %s %s %.4f %.4f %.4f" % (case, act, *ratio))
+
+
+FUSED_MUTATIONS = ["halo_a_bn0", "edge_frame_replicated", "chunk_halo_zero", "shortcut_prev_frame",
+                   "stride2_shortcut_odd", "drop_conv_b_tap", "b_truncated", "edge_tile_last_row"]
+
+
+@pytest.mark.parametrize("case,mutation", [(c, m) for c in sorted(FUSED_CPU_CASES) for m in FUSED_MUTATIONS
+                                           if not (c == "identity" and m == "stride2_shortcut_odd")])
+def test_fused_comparator_rejects_kernel_bugs(case, mutation):
+    inst, args, y, Y, prop = _fused_cpu_case(case, "relu")
+    got = fused_block_emulate(*args, mutation=mutation)
+    with pytest.raises(AssertionError):
+        TS.assert_close_to_f64(got, y, Y, _fused_k(inst), what=case, extra64=prop)
+
+
+# ---- CPU: the fused block's host checks and tile search ------------------------------------------------------------
+def test_fused_supported_rejects_32_bit_output_offsets():
+    """In-frame y offsets live in a 32-bit table: H_out * W_out * y_row_stride must stay below 2^31 even when the
+    input frame (8 channels) is 4x smaller."""
+    from pytorchvideo_b200 import _lib as L
+    lib = L.load()
+    big = _fused_desc(FB_RES2_0, 1, 4, 8192, 8192, xrs=8, yrs=32)
+    assert 8192 * 8192 * 8 < 2 ** 31 <= 8192 * 8192 * 32
+    assert lib.pv_bottleneck_fused_supported(C.byref(big)) == 0
+    half = _fused_desc(FB_RES2_0, 1, 4, 8192, 4096, xrs=8, yrs=32)
+    assert lib.pv_bottleneck_fused_supported(C.byref(half)) == 1
+    wide = _fused_desc(FB_RES2_0, 1, 4, 4096, 4096, xrs=8, yrs=128)
+    assert lib.pv_bottleneck_fused_supported(C.byref(wide)) == 0
+
+
+@pytest.mark.parametrize("inst", [FB_RES2_0, FB_RES2])
+@pytest.mark.parametrize("which", ["x", "y", "wa", "wb", "wc", "wsc"])
+def test_fused_rejects_misaligned_pointers(inst, which):
+    """Every pointer the kernel reads or writes 16 bytes at a time must be 16-byte aligned: PV_ERR_INVALID, decided
+    before any CUDA call.  N = 0, so no call here can launch a kernel whatever the library decides."""
+    from pytorchvideo_b200 import _lib as L
+    lib = L.load()
+    cin, cmid, cout, kt, s, proj = _fused_shape(inst)
+    d = _fused_desc(inst, 0, 4, 8, 8)
+    assert lib.pv_bottleneck_fused_supported(C.byref(d)) == 1
+    ptrs = dict(x=0x10000, y=0x20000, wa=0x30000, wb=0x40000, wc=0x50000, wsc=0x60000 if proj else None)
+    f32 = 0x70000
+
+    def call(**kw):
+        p = dict(ptrs, **kw)
+        return lib.pv_bottleneck_fused_fwd(C.byref(d), p["x"], p["wa"], p["wb"], p["wc"], p["wsc"], f32, f32, f32,
+                                           f32, f32, f32, f32 if proj else None, f32 if proj else None, p["y"], None)
+    assert call() != -1, L.last_error()             # aligned: past the argument checks (no device, or N = 0: no launch)
+    if which == "wsc" and not proj:
+        assert call(wsc=0x60008) != -1               # the identity shortcut has no weights to check
+        return
+    for off in (8, 2):
+        assert call(**{which: ptrs[which] + off}) == -1, (which, off)
+        assert "aligned" in L.last_error()
+
+
+# (TH, TW, TC) of the parent commit's tile search at 132 SMs (H100 SXM) for SlowFast-R50's Fast pathway at batch 8
+FUSED_BENCH_TILINGS = {
+    (FB_RES2_0, 56): (8, 14, 7),
+    (FB_RES2, 56): (14, 14, 7),
+    (FB_RES3_0, 56): (4, 8, 11),
+    (FB_RES3, 28): (10, 14, 6),
+}
+
+
+def test_fused_tiling_pinned_bench_geometry():
+    for (inst, hw), want in FUSED_BENCH_TILINGS.items():
+        cin, cmid, cout, kt, s, proj = _fused_shape(inst)
+        th, tw, tc, smem = fused_tiling(_fused_desc(inst, 8, 32, hw, hw), 132)
+        assert (th, tw, tc) == want, (inst, hw, (th, tw, tc))
+        assert 0 < smem <= 200 * 1024
+
+
+def test_fused_tiling_rejects_bad_arguments():
+    from pytorchvideo_b200 import _lib as L
+    lib = L.load()
+    th, tw, tc, smem = C.c_int(), C.c_int(), C.c_int(), C.c_longlong()
+    d = _fused_desc(FB_RES2, 1, 4, 8, 8)
+    assert lib.pv_bottleneck_fused_tiling(C.byref(d), 0, C.byref(th), C.byref(tw), C.byref(tc), C.byref(smem)) == -1
+    bad = _fused_desc(FB_RES2, 1, 4, 8, 8, xrs=36)
+    assert lib.pv_bottleneck_fused_tiling(C.byref(bad), 132, C.byref(th), C.byref(tw), C.byref(tc), C.byref(smem)) == -3
+
+
+@pytest.mark.parametrize("sm_count", [132, 114])
+def test_fused_row_claims_hold(sm_count):
+    """On an H100 SXM (132 SMs) and PCIe (114 SMs) every fused row's claimed tiling property holds, and every
+    batch-invariance row tiles a batch of 8 differently from one clip."""
+    for row in FUSED_ROWS:
+        inst, N, T, H, W, act, xe, ye, claims = row
+        cin, cmid, cout, kt, s, proj = _fused_shape(inst)
+        d = _fused_desc(inst, N, T, H, W, act, cin + xe, cout + ye)
+        props = fused_tiling_properties(d, sm_count)
+        assert set(claims) <= props, (_fused_row_id(row), claims, props, fused_tiling(d, sm_count))
+    for inst in {r[0] for r in FUSED_ROWS}:
+        for claim in (PH, PW, CH, SC):
+            assert any(r[0] == inst and claim in r[8] for r in FUSED_ROWS), (inst, claim)
+    for inst, T, H, W in FUSED_BATCH_ROWS:
+        t8 = fused_tiling(_fused_desc(inst, 8, T, H, W), sm_count)[:3]
+        t1 = fused_tiling(_fused_desc(inst, 1, T, H, W), sm_count)[:3]
+        assert t8 != t1, (inst, T, H, W, t8)
