@@ -160,14 +160,22 @@ int pv_ndhwc_to_ncdhw(const void* src, int src_dtype, long long src_row_stride, 
  * layers/convolutions.py:191-237 (Conv2plus1d), models/stem.py:330-337 (PatchEmbed) and the
  * residual add + ReLU of models/resnet.py:1179-1189.
  *   y = act( conv(x, w) * scale[co] + bias[co] (+ residual) )
- * groups must be 1 (dense) or == Ci == Co (depthwise).
+ * groups must divide Ci and Co.  groups == 1 is dense, groups == Ci == Co depthwise (PV_ALGO_DIRECT or
+ * pv_dwconv3d_fwd).  Other group counts (models/resnet.py conv_b_num_groups, models/csn.py width per group) run
+ * only in the grouped mode of PV_ALGO_TCGEN05: f16, 1 < groups < Ci, Ci == Co, Ci % 8 == 0, more than one group
+ * span (see pv_conv3d_group_span), the dense limits on taps, strides, offsets and row strides, and ci_pad64 equal to
+ * the span width span_k.  PV_ALGO_DIRECT returns PV_ERR_UNSUPPORTED for them; a caller runs what grouped mode does
+ * not take as the dense convolution with block-diagonal weights.
  *
  * Packed weights (host-side, see pytorchvideo_b200/engine/packing.py):
  *   PV_ALGO_DIRECT, dense : w[tap][ci][co]        (storage dtype, Ci/Co padded)
  *   depthwise (any algo)  : w[tap][c]             (storage dtype)
  *   PV_ALGO_TCGEN05       : w[co][tap][ci_pad64]  (f16, K-major rows of length taps*ci_pad64;
  *                           C_in < 64: ci_pad64 = Ci, row padded to a multiple of 64;
- *                           window mode: w[co][kt*kh][win] with win = 16|32|64 >= kw*Ci)
+ *                           window mode: w[co][kt*kh][win] with win = 16|32|64 >= kw*Ci;
+ *                           grouped mode: ci_pad64 = span_k, row co holds the weights of its group
+ *                           g = co / Cg at offset (g mod span_groups) * Cg of every tap's span_k block,
+ *                           zeros elsewhere)
  * ------------------------------------------------------------------------------------------- */
 typedef struct pv_conv3d_desc {
   int dtype;                 /* storage dtype of x, y, residual, w: PV_F16 | PV_F32          */
@@ -217,6 +225,14 @@ int pv_dwconv3d_fwd(const pv_conv3d_desc* d, const void* x, const void* w, const
 
 /* 1 if PV_ALGO_TCGEN05 supports this descriptor (pure host-side check, no GPU needed). */
 int pv_conv3d_tcgen05_supported(const pv_conv3d_desc* d);
+/* Group span of a grouped convolution (host only): span_groups = 64 / gcd(Cg, 64) consecutive groups of
+ * Cg = Ci / groups channels, whose span_k = span_groups * Cg input channels fill whole 64-channel boxes;
+ * span_n = span_groups * (Co / groups).  The last span may hold fewer groups.  Each output tile of grouped mode
+ * reads the input channels of its own span, so it does taps * span_k * Co multiply-adds per output position, 1/spans
+ * of the dense convolution of the same width.  Returns 1 when grouped mode takes the descriptor with its weights
+ * packed at ci_pad64 = span_k (whatever d->ci_pad64 holds), else 0.  The outputs are filled whenever groups > 1
+ * divides Ci and Co, and are 0 otherwise. */
+int pv_conv3d_group_span(const pv_conv3d_desc* d, int* span_groups, int* span_k, int* span_n);
 
 /* Stem convolutions (ResNetBasicStem.forward models/stem.py:252-260 conv; X3D stem conv_t models/x3d.py:83-88) on the
  * 4-channel, W-padded network input, stride 2 along W: zero-copy im2col - the A operand of a filter row is the RAW

@@ -102,6 +102,7 @@ SIGNATURES = {
     "pv_temporal_tap_sum": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_ll, C.c_int, C.c_int,
                                       C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, c_ll, c_ll, c_vp]),
     "pv_conv3d_tcgen05_supported": (C.c_int, [C.POINTER(Conv3dDesc)]),
+    "pv_conv3d_group_span": (C.c_int, [C.POINTER(Conv3dDesc), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "pv_conv3d_stem_rows_supported": (C.c_int, [C.POINTER(Conv3dDesc)]),
     "pv_conv3d_stem_rows_fwd": (C.c_int, [C.POINTER(Conv3dDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_bottleneck_fused_supported": (C.c_int, [C.POINTER(BottleneckDesc)]),
@@ -176,6 +177,13 @@ def require_device():
 
 def launch_count():
     return int(load().pv_launch_count())
+
+
+def group_span(desc):
+    """(taken, span_groups, span_k, span_n) of a grouped Conv3dDesc (pv_conv3d_group_span, host only)."""
+    sg, sk, sn = C.c_int(0), C.c_int(0), C.c_int(0)
+    ok = load().pv_conv3d_group_span(C.byref(desc), C.byref(sg), C.byref(sk), C.byref(sn))
+    return bool(ok), sg.value, sk.value, sn.value
 
 
 def kernel_counts():

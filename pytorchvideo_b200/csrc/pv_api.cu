@@ -33,6 +33,7 @@ int conv3d_check(const pv_conv3d_desc* d);
 int conv3d_direct_launch(const pv_conv3d_desc* d, const void* x, const void* w, const float* scale,
                          const float* bias, const void* residual, void* y, cudaStream_t s);
 int conv3d_tcgen05_supported(const pv_conv3d_desc* d, char* why, size_t why_len);
+int conv3d_group_span(const pv_conv3d_desc* d, int* span_groups, int* span_k, int* span_n);   // pv_igemm.cu
 int conv3d_tcgen05_launch(const pv_conv3d_desc* d, const void* x, const void* w, const float* scale,
                           const float* bias, const void* residual, void* y, cudaStream_t s);
 int conv3d_gather_supported(const pv_conv3d_desc* d);
@@ -89,6 +90,18 @@ extern "C" int pv_conv3d_tcgen05_supported(const pv_conv3d_desc* d) {
   return pv::conv3d_tcgen05_supported(d, nullptr, 0);
 }
 
+extern "C" int pv_conv3d_group_span(const pv_conv3d_desc* d, int* span_groups, int* span_k, int* span_n) {
+  int sg = 0, sk = 0, sn = 0;
+  const bool known = d && d->groups > 1 && pv::conv3d_group_span(d, &sg, &sk, &sn);
+  if (span_groups) *span_groups = sg;
+  if (span_k) *span_k = sk;
+  if (span_n) *span_n = sn;
+  if (!known) return 0;
+  pv_conv3d_desc q = *d;
+  q.ci_pad64 = sk;             // grouped mode packs the weights at the span width
+  return pv::conv3d_tcgen05_supported(&q, nullptr, 0);
+}
+
 extern "C" int pv_conv3d_fwd(const pv_conv3d_desc* d, int algo, const void* x, const void* w,
                              const float* scale, const float* bias, const void* residual, void* y,
                              void* stream) {
@@ -97,8 +110,8 @@ extern "C" int pv_conv3d_fwd(const pv_conv3d_desc* d, int algo, const void* x, c
   PV_CHECK_ARG(x && w && scale && bias && y, "null pointer");
   PV_CHECK_ARG(!d->has_residual || residual, "has_residual set but residual is null");
   cudaStream_t s = (cudaStream_t)stream;
-  if (algo == PV_ALGO_AUTO)
-    algo = (d->groups == 1 && pv_conv3d_tcgen05_supported(d)) ? PV_ALGO_TCGEN05 : PV_ALGO_DIRECT;
+  if (algo == PV_ALGO_AUTO)   // dense or grouped mode on the tensor cores when they take it; depthwise never does
+    algo = pv_conv3d_tcgen05_supported(d) ? PV_ALGO_TCGEN05 : PV_ALGO_DIRECT;
   if (algo == PV_ALGO_TCGEN05) {
     if (pv::wants_gather(d)) return pv::conv3d_gather_launch(d, x, w, scale, bias, residual, y, s);
     return pv::conv3d_tcgen05_launch(d, x, w, scale, bias, residual, y, s);

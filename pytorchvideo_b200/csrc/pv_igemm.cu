@@ -59,10 +59,16 @@ struct IgemmParams {
 // KB = kbytes.  A stage always holds 64 K elements (G = 128 / KB k-blocks, four k16 steps), so the wgmma sequence of a
 // stage is unrolled at compile time: no branch between the wgmma of a stage keeps them asynchronous.  The last chunk of
 // a tile is padded with k-blocks whose TMA loads lie entirely out of bounds (zero fill).
-template <int BN, int KB>
-__global__ void __launch_bounds__(IG_THREADS, 1)
-conv3d_igemm_kernel(const __grid_constant__ IgemmParams P, const float* __restrict__ scale,
-                    const float* __restrict__ bias) {
+//
+// GROUPED (grouped convolution, see conv3d_group_span): the output channels form spans of span_tiles N tiles, and the
+// N tiles of span s read input channels [s * K_span, (s + 1) * K_span) with K_span = num_kc * 64, i.e. the A box of
+// channel chunk kc starts at channel c0 + kc * 64 with c0 = (n_tile / span_tiles) * K_span.  The packed weights of a
+// span are block-diagonal over its groups (zeros elsewhere), so the B operand, the epilogue and the stores are those of
+// the dense kernel.  Grouped mode runs with 128-byte k-blocks only (G = 1): no padding k-block is ever loaded, whose
+// channel coordinate num_kc * 64 would lie inside the next span.
+template <int BN, int KB, bool GROUPED>
+__device__ __forceinline__ void igemm_body(const IgemmParams& P, const float* __restrict__ scale,
+                                           const float* __restrict__ bias, int span_tiles) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -127,6 +133,7 @@ conv3d_igemm_kernel(const __grid_constant__ IgemmParams P, const float* __restri
         int n_tile, o[4];
         tile_coords(tile, n_tile, o);
         const int n0 = n_tile * BN;
+        const int c0 = GROUPED ? (n_tile / span_tiles) * num_kc * k_elems : 0;   // first input channel of the span
         int tap = 0, kc = 0;                  // (tap, channel chunk) of the next k-block, stepped without a divide
         for (int ch = 0; ch < cpt; ++ch) {
           const int kb0 = ch * G;
@@ -141,7 +148,8 @@ conv3d_igemm_kernel(const __grid_constant__ IgemmParams P, const float* __restri
               const int t = pad ? P.taps - 1 : tp;
               if ((2 * j) % nsplit == pw) {
                 const void* amap = &P.a_maps[P.tap_map[t]];
-                tma_load_5d(st_base + (uint32_t)j * a_bytes, amap, full_bar(stage), pad ? num_kc * k_elems : kk * k_elems,
+                tma_load_5d(st_base + (uint32_t)j * a_bytes, amap, full_bar(stage),
+                            (pad ? num_kc * k_elems : kk * k_elems) + c0,
                             o[0] + P.tap_q[t][0], o[1] + P.tap_q[t][1], o[2] + P.tap_q[t][2], o[3] + P.tap_q[t][3]);
               }
               if ((2 * j + 1) % nsplit == pw)
@@ -201,6 +209,21 @@ conv3d_igemm_kernel(const __grid_constant__ IgemmParams P, const float* __restri
     }
     if (ctid == 0) tma_store_wait_all();   // smem must outlive the bulk stores
   }
+}
+
+template <int BN, int KB>
+__global__ void __launch_bounds__(IG_THREADS, 1)
+conv3d_igemm_kernel(const __grid_constant__ IgemmParams P, const float* __restrict__ scale,
+                    const float* __restrict__ bias) {
+  igemm_body<BN, KB, false>(P, scale, bias, 1);
+}
+
+// span_tiles: N tiles per group span (N_span / BN)
+template <int BN, int KB>
+__global__ void __launch_bounds__(IG_THREADS, 1)
+conv3d_igemm_grouped_kernel(const __grid_constant__ IgemmParams P, const float* __restrict__ scale,
+                            const float* __restrict__ bias, int span_tiles) {
+  igemm_body<BN, KB, true>(P, scale, bias, span_tiles);
 }
 
 // =============================================================================================
@@ -299,6 +322,21 @@ static void reduce_dims(const pv_conv3d_desc* d, IgemmPlan* pl) {
 
 static int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
 
+// Group span of a grouped convolution: S = 64 / gcd(Cg_in, 64) consecutive groups, so that the span's K_span = S * Cg_in
+// input channels fill whole 64-channel TMA boxes (no box reaches into the next span); N_span = S * Cg_out.  The last
+// span may hold fewer groups: it ends at Ci, and TMA out-of-bounds fill covers its tail.  Returns 0 when groups does
+// not divide both channel counts.
+int conv3d_group_span(const pv_conv3d_desc* d, int* span_groups, int* span_k, int* span_n) {
+  if (d->groups < 1 || d->Ci % d->groups || d->Co % d->groups) return 0;
+  const int cgi = d->Ci / d->groups, cgo = d->Co / d->groups;
+  int a = cgi, b = 64;
+  while (b) { const int t = a % b; a = b; b = t; }   // gcd(Cg_in, 64)
+  *span_groups = 64 / a;
+  *span_k = *span_groups * cgi;
+  *span_n = *span_groups * cgo;
+  return 1;
+}
+
 int conv3d_tcgen05_supported(const pv_conv3d_desc* d, char* why, size_t why_len) {
 #define NOPE(...)                          \
   do {                                     \
@@ -306,7 +344,19 @@ int conv3d_tcgen05_supported(const pv_conv3d_desc* d, char* why, size_t why_len)
     return 0;                              \
   } while (0)
   if (d->dtype != PV_F16) NOPE("tcgen05 path needs f16 storage");
-  if (d->groups != 1) NOPE("tcgen05 path is dense only (groups=%d)", d->groups);
+  const bool grouped = d->groups != 1;
+  int span_g = 0, span_k = 0, span_n = 0;
+  if (grouped) {
+    // grouped mode: several spans, each a block-diagonal GEMM over whole 64-channel boxes of its own input channels
+    if (!conv3d_group_span(d, &span_g, &span_k, &span_n))
+      NOPE("groups=%d does not divide Ci=%d and Co=%d", d->groups, d->Ci, d->Co);
+    if (d->groups >= d->Ci) NOPE("depthwise (groups=%d) runs on pv_dwconv3d_fwd", d->groups);
+    if (d->Ci != d->Co) NOPE("grouped mode needs square groups (Ci=%d, Co=%d)", d->Ci, d->Co);
+    if (d->groups <= span_g) NOPE("one group span (%d groups): run as a dense convolution", span_g);
+    if (span_n % 64) NOPE("span output width %d is not a multiple of 64", span_n);
+    if (d->x_w_pad > 0) NOPE("grouped mode has no window mode");
+    if (d->ci_pad64 != span_k) NOPE("grouped mode: ci_pad64 must equal the span width %d", span_k);
+  }
   if (window_mode(d)) {
     if (d->Ci != 4 && d->Ci != 8) NOPE("window mode needs Ci in {4,8}");
     if (d->Co % 8) NOPE("Co must be a multiple of 8");
@@ -328,7 +378,8 @@ int conv3d_tcgen05_supported(const pv_conv3d_desc* d, char* why, size_t why_len)
     NOPE("row strides must be multiples of 8 elements (16 B)");
   if (d->kt * d->kh * d->kw > IG_MAX_TAPS) NOPE("too many taps");
   if (d->st * d->sh * d->sw > IG_MAX_MAPS) NOPE("stride product > %d", IG_MAX_MAPS);
-  if (!conv3d_tma_narrow(d) && (d->ci_pad64 < d->Ci || d->ci_pad64 % 64)) NOPE("ci_pad64 must be a multiple of 64 >= Ci");
+  if (!grouped && !conv3d_tma_narrow(d) && (d->ci_pad64 < d->Ci || d->ci_pad64 % 64))
+    NOPE("ci_pad64 must be a multiple of 64 >= Ci");
   const long long M = (long long)d->N * d->To * d->Ho * d->Wo;
   if (M >= (1ll << 31)) NOPE("too many output positions");
   for (int off : {d->pt, d->ph, d->pw, d->dt * (d->kt - 1), d->dh * (d->kh - 1), d->dw * (d->kw - 1)})
@@ -392,12 +443,16 @@ int conv3d_tcgen05_launch(const pv_conv3d_desc* d, const void* x, const void* w,
   }
 
   // ---- BLOCK_N (a wgmma width, <= 128): minimise waves * per-tile cost
+  const bool grouped = d->groups != 1;
+  int span_g = 0, span_k = 0, span_n = 0;
+  if (grouped) conv3d_group_span(d, &span_g, &span_k, &span_n);
   {
     const int co16 = (int)cdiv(d->Co, 16) * 16;
     const int cands[4] = {128, 64, 32, 16};
     double best = 1e30;
     int bn = 16;
     for (int c : cands) {
+      if (grouped && (c < 64 || span_n % c)) continue;   // grouped: an N tile never straddles two spans
       if (c > round_block_n(co16)) continue;
       if (c < co16 && (c % 64)) continue;   // several N tiles: TMA-store sub-tiles are 64 channels wide
       const long long tiles = (long long)P.m_tiles * cdiv(d->Co, c);
@@ -435,6 +490,12 @@ int conv3d_tcgen05_launch(const pv_conv3d_desc* d, const void* x, const void* w,
     P.split_ab = G >= 2 ? 4 : 2;
     P.cpt = (num_kb + G - 1) / G;
     P.stages = st;
+    // a padding k-block would load channel num_kc * 64 of the span, i.e. the next span's first channels
+    if (grouped && (G != 1 || P.block_n > span_n || span_n % P.block_n)) {
+      set_error("internal: grouped mode needs one k-block per stage and BLOCK_N | N_span (G=%d BN=%d N_span=%d)", G,
+                P.block_n, span_n);
+      return PV_ERR_INVALID;
+    }
   }
   const int stage_bytes = P.G * kb_bytes;
   const size_t smem_bytes = (size_t)P.stages * stage_bytes + smem_fixed + 8 * (2 * P.stages + 1);
@@ -572,6 +633,20 @@ int conv3d_tcgen05_launch(const pv_conv3d_desc* d, const void* x, const void* w,
     name = "conv3d_igemm_kernel<" #BN "," #KB ">";                                              \
   }
     const char* name = nullptr;
+    if (grouped) {
+      const int span_tiles = span_n / P.block_n;
+#define PV_IG_GROUPED_LAUNCH(BN, KB)                                                                     \
+  if (P.block_n == BN && P.kbytes == KB) {                                                               \
+    PV_OPT_IN_SMEM((conv3d_igemm_grouped_kernel<BN, KB>), 227 * 1024);                                   \
+    PV_CUDA_OK(cudaLaunchKernelEx(&cfg, conv3d_igemm_grouped_kernel<BN, KB>, P, scale, bias, span_tiles)); \
+    name = "conv3d_igemm_grouped_kernel<" #BN "," #KB ">";                                               \
+  }
+      PV_IG_GROUPED_LAUNCH(64, 128) PV_IG_GROUPED_LAUNCH(128, 128)
+#undef PV_IG_GROUPED_LAUNCH
+      if (!name) { set_error("internal: no grouped igemm instance for BN=%d kbytes=%d", P.block_n, P.kbytes); return PV_ERR_INVALID; }
+      PV_LAUNCH_OK(name);
+      return PV_OK;
+    }
     PV_IG_LAUNCH(16, 32) PV_IG_LAUNCH(16, 64) PV_IG_LAUNCH(16, 128)
     PV_IG_LAUNCH(32, 32) PV_IG_LAUNCH(32, 64) PV_IG_LAUNCH(32, 128)
     PV_IG_LAUNCH(64, 32) PV_IG_LAUNCH(64, 64) PV_IG_LAUNCH(64, 128)

@@ -1012,9 +1012,8 @@ int conv3d_check(const pv_conv3d_desc* d) {
   PV_CHECK_ARG(to == d->To && ho == d->Ho && wo == d->Wo,
                "output dims (%d,%d,%d) inconsistent with conv arithmetic (%d,%d,%d)", d->To, d->Ho,
                d->Wo, to, ho, wo);
-  PV_CHECK_ARG(d->groups == 1 || (d->groups == d->Ci && d->Ci == d->Co),
-               "groups must be 1 or Ci==Co (depthwise); got groups=%d Ci=%d Co=%d", d->groups,
-               d->Ci, d->Co);
+  PV_CHECK_ARG(d->groups >= 1 && d->Ci % d->groups == 0 && d->Co % d->groups == 0,
+               "groups must divide Ci and Co; got groups=%d Ci=%d Co=%d", d->groups, d->Ci, d->Co);
   PV_CHECK_ARG(d->x_row_stride >= d->Ci && d->y_row_stride >= d->Co, "row stride < channels");
   PV_CHECK_ARG(!d->has_residual || d->res_row_stride >= d->Co, "residual row stride < Co");
   return PV_OK;
@@ -1043,6 +1042,11 @@ int conv3d_direct_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
       PV_LAUNCH_OK("conv3d_direct_kernel<float>");
     }
   } else {
+    if (d->groups != d->Ci || d->Ci != d->Co) {
+      set_error("PV_ALGO_DIRECT runs dense (groups=1) and depthwise (groups==Ci==Co) convolutions only; got groups=%d "
+                "Ci=%d Co=%d", d->groups, d->Ci, d->Co);
+      return PV_ERR_UNSUPPORTED;
+    }
     PV_CHECK_ARG(d->Co % 8 == 0, "depthwise conv needs C%%8==0");
     PV_CHECK_ARG(d->x_row_stride % 8 == 0 && d->y_row_stride % 8 == 0, "row strides must be multiples of 8");
     // TMA-fed shared-memory stencil (pv_dwconv.cu) whenever it applies

@@ -75,6 +75,33 @@ def pack_dense_tcgen05(w, ci_pad64, co_pad):
     return out.contiguous()
 
 
+def pack_grouped_tcgen05(w, groups, span_groups, span_k):
+    """Grouped mode of the TMA-fed kernel: [Co, Cg_in, kt, kh, kw] -> f16 [Co, taps * span_k], K-major
+    (k = tap * span_k + c).  Output channel co belongs to group g = co // Cg_out, which sits at input offset
+    (g % span_groups) * Cg_in of its span; the rest of the row is zero (a block-diagonal GEMM per span)."""
+    co, cgi, kt, kh, kw = w.shape
+    cgo = co // groups
+    taps = kt * kh * kw
+    out = torch.zeros(co, taps, span_k, dtype=torch.float16)
+    src = w.detach().cpu().permute(0, 2, 3, 4, 1).reshape(co, taps, cgi).to(torch.float16)
+    for g in range(groups):
+        off = (g % span_groups) * cgi
+        out[g * cgo:(g + 1) * cgo, :, off:off + cgi] = src[g * cgo:(g + 1) * cgo]
+    return out.reshape(co, taps * span_k).contiguous()
+
+
+def expand_grouped_dense(w, groups):
+    """[Co, Cg_in, kt, kh, kw] -> the block-diagonal dense weight [Co, groups * Cg_in, kt, kh, kw] (same dtype): a
+    grouped convolution as an ordinary one, for the shapes the grouped mode does not take."""
+    co, cgi = w.shape[:2]
+    cgo = co // groups
+    src = w.detach().cpu()
+    out = torch.zeros((co, groups * cgi) + tuple(w.shape[2:]), dtype=src.dtype)
+    for g in range(groups):
+        out[g * cgo:(g + 1) * cgo, g * cgi:(g + 1) * cgi] = src[g * cgo:(g + 1) * cgo]
+    return out
+
+
 def window_lead(w_pad, pw, ci_pad):
     """Leading zero pixels of the window so that its first byte is 16-byte aligned (see pv_igemm.cu)."""
     return 1 if ((w_pad - pw) * ci_pad * 2) % 16 else 0

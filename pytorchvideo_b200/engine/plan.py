@@ -310,6 +310,20 @@ class Plan:
         if min(To, Ho, Wo) <= 0:
             raise RuntimeError("conv %s: kernel larger than (padded) input" % name)
         co_pad = PK.pad8(co)
+        depthwise = groups != 1 and groups == ci == co
+        span = None
+        if groups != 1 and not depthwise:
+            # grouped conv (ResNeXt-style group counts, CSN with several channels per group): the grouped mode of the
+            # TMA-fed kernel when the library takes the shape, else the dense convolution with block-diagonal weights
+            # (one group span, C % 8 != 0, non-square groups, f32, forced CUDA-core algorithm)
+            if self.use_tcgen05 and force_algo in (None, L.ALGO_TCGEN05) and x.Cp == ci and co_pad == co:
+                probe = self._conv_desc(x, (To, Ho, Wo), co_pad, (kt, kh, kw), stride, padding, dilation, groups, act,
+                                        residual, co_pad, 0)
+                taken, span_g, span_k, _ = L.group_span(probe)
+                span = (span_g, span_k) if taken else None
+            if span is None:
+                return self.emit_conv(x, PK.expand_grouped_dense(weight, groups), conv_bias, bn, stride, padding,
+                                      dilation, 1, act, residual, name, force_algo=force_algo, se_sums=se_sums)
         if residual is not None:
             self.materialize_input(residual)
         # ---- narrow stems with a temporal extent: factor (kt,kh,kw) -> (1,kh,kw) with kt*Co channels
@@ -355,27 +369,15 @@ class Plan:
         y = self.new_tensor(x.N, To, Ho, Wo, co, Cp=co_pad)
         scale, bias = PK.fold_bn(conv_bias, bn, co, co_pad)
         scale_d, bias_d = self.const(scale), self.const(bias)
-        depthwise = groups != 1
-        if depthwise and not (groups == ci == co):
-            raise RuntimeError("conv %s: only groups==1 or depthwise (groups==Cin==Cout) is supported" % name)
         tdt = _TORCH_DT[self.dt]
         ci_pad = x.Cp
         ci_pad64 = ci_pad if ci_pad < 64 else PK.pad_to(ci_pad, 64)   # < 64: gather-fed kernel, un-padded taps
+        if span is not None:
+            ci_pad64 = span[1]                                          # grouped mode: weights packed at the span width
 
-        d = L.Conv3dDesc()
-        d.dtype = self.dt
-        d.N, d.Ti, d.Hi, d.Wi, d.Ci = x.N, x.T, x.H, x.W, ci_pad
-        d.To, d.Ho, d.Wo, d.Co = To, Ho, Wo, co_pad
-        d.kt, d.kh, d.kw = kt, kh, kw
-        d.st, d.sh, d.sw = st, sh, sw
-        d.pt, d.ph, d.pw = pt, ph, pw
-        d.dt, d.dh, d.dw = dlt, dlh, dlw
-        d.groups = ci_pad if depthwise else 1
-        d.act = act
-        d.has_residual = 1 if residual is not None else 0
-        d.x_row_stride, d.y_row_stride = x.row_stride, y.row_stride
-        d.res_row_stride = residual.row_stride if residual is not None else 0
-        d.ci_pad64 = ci_pad64
+        d = self._conv_desc(x, (To, Ho, Wo), co_pad, (kt, kh, kw), stride, padding, dilation,
+                            ci_pad if depthwise else (groups if span is not None else 1), act, residual, y.row_stride,
+                            ci_pad64)
         if window:
             d.x_w_pad, d.x_w_phys = x.padw
             w_lead = PK.window_lead(x.padw[0], pw, x.Cp)
@@ -385,6 +387,9 @@ class Plan:
         if depthwise:
             algo, kind = L.ALGO_DIRECT, "depthwise"
             w_d = self.const(PK.pack_depthwise(weight, co_pad, tdt))
+        elif span is not None:
+            algo, kind = L.ALGO_TCGEN05, "grouped"
+            w_d = self.const(PK.pack_grouped_tcgen05(weight, groups, span[0], span[1]))
         else:
             want_tc = self.use_tcgen05 and bool(self.lib.pv_conv3d_tcgen05_supported(C.byref(d)))
             if force_algo is not None:
@@ -442,6 +447,25 @@ class Plan:
         self.add(name, fn_stem if stem_rows else (fn_dw if (depthwise and residual is None) else fn), kind, flops, nbytes,
                  reads=(x,) + ((residual,) if residual is not None else ()), writes=(y,) + ((sums,) if sums is not None else ()))
         return y
+
+    def _conv_desc(self, x, out_thw, co_pad, kernel, stride, padding, dilation, groups, act, residual, y_row_stride,
+                   ci_pad64):
+        d = L.Conv3dDesc()
+        d.dtype = self.dt
+        d.N, d.Ti, d.Hi, d.Wi, d.Ci = x.N, x.T, x.H, x.W, x.Cp
+        d.To, d.Ho, d.Wo = out_thw
+        d.Co = co_pad
+        d.kt, d.kh, d.kw = kernel
+        d.st, d.sh, d.sw = stride
+        d.pt, d.ph, d.pw = padding
+        d.dt, d.dh, d.dw = dilation
+        d.groups = groups
+        d.act = act
+        d.has_residual = 1 if residual is not None else 0
+        d.x_row_stride, d.y_row_stride = x.row_stride, y_row_stride
+        d.res_row_stride = residual.row_stride if residual is not None else 0
+        d.ci_pad64 = ci_pad64
+        return d
 
     def fused_bottleneck_desc(self, x, cin_pad, cmid, cout, kt, sb, has_shortcut, act):
         d = L.BottleneckDesc()

@@ -147,6 +147,25 @@ def build_case(case, hub_module, weight_seed=1234, input_seed=42):
     return model, (slowfast_inputs(clip) if is_sf else clip), is_sf
 
 
+# Grouped conv_b (ResNeXt-style group counts, CSN with several channels per group): the builders' own arguments on the
+# hub entries.  Kept apart from MODEL_CASES, whose host lowering test counts every groups > 1 conv as depthwise.
+# name: (hub builder name, kwargs, batch, T, H, W, is_slowfast, f16_grid) -> tests/golden/model_grouped_<name>.pt
+GROUPED_MODEL_CASES = {
+    "slow_r50_g32": ("slow_r50", {"stage_conv_b_num_groups": (32,) * 4}, 1, 8, 224, 224, False, False),
+    "csn_r101_w8": ("csn_r101", {"stage_conv_b_width_per_group": 8}, 1, 32, 224, 224, False, False),
+    "slowfast_r50_g": ("slowfast_r50", {"stage_conv_b_num_groups": ((32,) * 4, (2,) * 4)}, 1, 32, 224, 224, True, False),
+    "slow_r50_g32_f16w": ("slow_r50", {"stage_conv_b_num_groups": (32,) * 4}, 2, 8, 224, 224, False, True),
+}
+
+
+def build_grouped_case(case, hub_module, weight_seed=1234, input_seed=42):
+    """(model, inputs, is_slowfast) of a GROUPED_MODEL_CASES entry, built from ``hub_module``."""
+    hub, kw, B, T, H, W, is_sf, grid = GROUPED_MODEL_CASES[case]
+    model = randomize_model(getattr(hub_module, hub)(**kw), seed=weight_seed, f16_weights=grid).eval()
+    clip = synthetic_clip(B, T, H, W, seed=input_seed, f16_values=grid)
+    return model, (slowfast_inputs(clip) if is_sf else clip), is_sf
+
+
 
 # The layer goldens are stored in two files (tests/golden/layers.pt, layers_conv.pt) to keep each under 1 MB.
 LAYER_GOLDEN_FILES = ("layers.pt", "layers_conv.pt")
