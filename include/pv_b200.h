@@ -128,6 +128,57 @@ int pv_clip_transform_batch(const pv_clip_batch_desc* d, const void* src, const 
                             const int32_t* slow_pos, const int32_t* geom, void* dst, void* dst_slow,
                             void* stream);
 
+/* RandomResizedCrop mode of the batched chain (transforms/functional.py random_resized_crop): every kept frame j of
+ * clip b reads its own source window boxes[(b*n_t + j)*5 + {0..4}] = {top, left, h, w, hflip} of the in_h x in_w frame
+ * and resizes it to out_h x out_w with ATen's bilinear taps relative to the window, after the optional /255 and
+ * normalisation of the descriptor.  new_h/new_w/top/left/hflip/n_slow/d_slow_clip of the descriptor are ignored.
+ * C must be 3; src PV_U8 or PV_F32, dst PV_F16 or PV_F32.  boxes is a DEVICE int32 array; the caller keeps every
+ * window inside the frame.                                                                                            */
+int pv_clip_transform_rrc(const pv_clip_batch_desc* d, const void* src, const int32_t* idx_t, const int32_t* boxes,
+                          void* dst, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Video augmentation (transforms/augmentations.py, rand_augment.py, augmix.py): a batch of clips of (T, 3, H, W)
+ * frames, each clip with its own op per layer step.
+ *   src[(clip / src_div)*s_clip + t*st + c*sc + h*sh + w*sw]  (any strides; src_div > 1 feeds several AugMix chains
+ *   from one clip)  ->  dst contiguous [n_clips][T][3][H][W] of the same dtype (PV_U8 or PV_F32).
+ * pv_augment_stats fills one pv_aug_frame_stats per (clip, frame): per-channel min / max, the Equalize table and the
+ * grayscale sum of AdjustContrast; integer histogram atomics and a fixed-order reduction make it deterministic.
+ * pv_augment_apply runs ops[clip] on every clip (ops and stats are DEVICE arrays; stats may be NULL when no op needs it).
+ * pv_augment_mix: dst[b] = m*x[b] + (1-m)*sum_k w_k*chains[b*width + k] with mix[b*(width+2)] = {w_0.., m, 1-m}.    */
+typedef enum pv_aug_kind {
+  PV_AUG_NONE = 0, PV_AUG_BRIGHTNESS = 1, PV_AUG_CONTRAST = 2, PV_AUG_SATURATION = 3, PV_AUG_SHARPNESS = 4,
+  PV_AUG_AUTOCONTRAST = 5, PV_AUG_EQUALIZE = 6, PV_AUG_INVERT = 7, PV_AUG_POSTERIZE = 8, PV_AUG_SOLARIZE = 9,
+  PV_AUG_AFFINE = 10
+} pv_aug_kind;
+
+typedef struct pv_aug_op {
+  int kind;        /* pv_aug_kind                                                                      */
+  int ival;        /* Posterize: bit mask; Solarize on uint8: threshold                                */
+  float ratio;     /* _blend ratio (Brightness/Contrast/Saturation/Sharpness); Solarize on f32: threshold */
+  float omr;       /* _blend: float(1 - ratio) rounded once from the double, as torchvision's scalar   */
+  float theta[6];  /* Affine: the grid matrix already divided by (W/2, H/2), row-major 2x3             */
+  float fill[3];   /* Affine: fill colour                                                              */
+} pv_aug_op;
+
+typedef struct pv_aug_frame_stats {
+  float mn[3], mx[3];
+  double gray_sum;
+  unsigned char lut[3][256];
+} pv_aug_frame_stats;
+
+typedef struct pv_augment_desc {
+  int n_clips, src_div, T, C, H, W;
+  long long s_clip, st, sc, sh, sw;  /* source strides in elements */
+  int dtype;                         /* PV_U8 | PV_F32             */
+} pv_augment_desc;
+
+int pv_augment_stats(const pv_augment_desc* d, const void* src, pv_aug_frame_stats* stats, void* stream);
+int pv_augment_apply(const pv_augment_desc* d, const void* src, const pv_aug_op* ops, const pv_aug_frame_stats* stats,
+                     void* dst, void* stream);
+int pv_augment_mix(const pv_augment_desc* d, const void* src, const void* chains, int width, const float* mix,
+                   void* dst, void* stream);
+
 /* Test-time multi-view ensembling (pytorchvideo_trainer/module/video_classification.py:290-311, docs model_zoo.md:63
  * "3 spatial x 10 temporal views"): out[v][k] = reduce over the n_views consecutive rows of video v;
  * mode 0 = sum, 1 = mean (sum / clip count), 2 = max.  preds: [n_videos * n_views][K] f32.                    */

@@ -36,6 +36,21 @@ class ClipBatchDesc(C.Structure):
                 ("div255", C.c_int), ("normalize", C.c_int), ("src_dtype", C.c_int), ("dst_dtype", C.c_int)]
 
 
+class AugOp(C.Structure):
+    _fields_ = [("kind", C.c_int), ("ival", C.c_int), ("ratio", C.c_float), ("omr", C.c_float),
+                ("theta", C.c_float * 6), ("fill", C.c_float * 3)]
+
+
+class AugFrameStats(C.Structure):
+    _fields_ = [("mn", C.c_float * 3), ("mx", C.c_float * 3), ("gray_sum", C.c_double), ("lut", (C.c_ubyte * 256) * 3)]
+
+
+class AugmentDesc(C.Structure):
+    _fields_ = [("n_clips", C.c_int), ("src_div", C.c_int), ("T", C.c_int), ("C", C.c_int), ("H", C.c_int),
+                ("W", C.c_int), ("s_clip", c_ll), ("st", c_ll), ("sc", c_ll), ("sh", c_ll), ("sw", c_ll),
+                ("dtype", C.c_int)]
+
+
 class BottleneckDesc(C.Structure):
     _fields_ = [("N", C.c_int), ("T", C.c_int), ("H", C.c_int), ("W", C.c_int),
                 ("Cin", C.c_int), ("Cmid", C.c_int), ("Cout", C.c_int), ("kt", C.c_int), ("sb", C.c_int),
@@ -88,6 +103,10 @@ SIGNATURES = {
     "pv_clip_transform_fwd": (C.c_int, [C.POINTER(ClipTransformDesc), c_vp, c_vp, c_vp, c_vp, c_vp,
                                         c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_clip_transform_batch": (C.c_int, [C.POINTER(ClipBatchDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_clip_transform_rrc": (C.c_int, [C.POINTER(ClipBatchDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_augment_stats": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, c_vp]),
+    "pv_augment_apply": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_augment_mix": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp]),
     "pv_view_reduce": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp]),
     "pv_ncdhw_to_ndhwc": (C.c_int, [c_vp, C.c_int, c_vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_int, C.c_int, c_ll, c_vp]),

@@ -120,11 +120,13 @@ template <typename T> __device__ __forceinline__ void st_out2(T* p, float a, flo
 constexpr int TB_ROWS = 8;
 constexpr int TB_THREADS = 256;
 
-template <typename SrcT, typename OutT, int NC, bool LUT>
-__global__ void __launch_bounds__(TB_THREADS)
-clip_transform_batch_kernel(pv_clip_batch_desc d, const SrcT* __restrict__ src, const int32_t* __restrict__ idx_t,
-                            const int32_t* __restrict__ slow_pos, const int32_t* __restrict__ geom,
-                            OutT* __restrict__ dst, OutT* __restrict__ dst_slow) {
+// RRC (RandomResizedCrop mode, pv_clip_transform_rrc): geom holds one {top, left, h, w, hflip} source window per
+// (clip, kept frame); the taps are ATen's for an h x w -> out_h x out_w resize, offset by the window origin.
+template <typename SrcT, typename OutT, int NC, bool LUT, bool RRC>
+__device__ __forceinline__ void
+clip_transform_batch_body(const pv_clip_batch_desc& d, const SrcT* __restrict__ src, const int32_t* __restrict__ idx_t,
+                          const int32_t* __restrict__ slow_pos, const int32_t* __restrict__ geom,
+                          OutT* __restrict__ dst, OutT* __restrict__ dst_slow) {
   constexpr int PX = 2;
   __shared__ float lut[LUT ? NC * 256 : 1];
   if constexpr (LUT) {
@@ -140,7 +142,12 @@ clip_transform_batch_kernel(pv_clip_batch_desc d, const SrcT* __restrict__ src, 
   const int clip = blockIdx.z / d.n_t, j = blockIdx.z - clip * d.n_t;
   int new_h = d.new_h, new_w = d.new_w, top = d.top, left = d.left, flip = d.hflip;
   int t_off = 0;
-  if (geom != nullptr) {        // per-clip (new_h, new_w, top, left, hflip, first frame)
+  int win_h = 0, win_w = 0;                 // RRC source window size
+  if constexpr (RRC) {          // per-(clip, frame) source window
+    const int32_t* g = geom + 5 * blockIdx.z;
+    top = __ldg(g); left = __ldg(g + 1); win_h = __ldg(g + 2); win_w = __ldg(g + 3); flip = __ldg(g + 4);
+    new_h = d.out_h; new_w = d.out_w;
+  } else if (geom != nullptr) {        // per-clip (new_h, new_w, top, left, hflip, first frame)
     const int32_t* g = geom + 6 * clip;
     new_h = __ldg(g); new_w = __ldg(g + 1); top = __ldg(g + 2); left = __ldg(g + 3); flip = __ldg(g + 4);
     t_off = __ldg(g + 5);
@@ -157,7 +164,8 @@ clip_transform_batch_kernel(pv_clip_batch_desc d, const SrcT* __restrict__ src, 
   const int n_rows = min(TB_ROWS, d.out_h - y_base);
   const int plane = d.out_h * d.out_w;                 // host checks C*n_t*plane < 2^31
   const unsigned sh = (unsigned)d.sh, sw = (unsigned)d.sw;
-  const float scale_y = bilinear_scale(d.in_h, new_h), scale_x = bilinear_scale(d.in_w, new_w);
+  const float scale_y = RRC ? bilinear_scale(win_h, new_h) : bilinear_scale(d.in_h, new_h);
+  const float scale_x = RRC ? bilinear_scale(win_w, new_w) : bilinear_scale(d.in_w, new_w);
   OutT* const dclip = dst + (long long)clip * d.d_clip + (long long)j * plane;
   OutT* const sclip = sp >= 0 ? dst_slow + (long long)clip * d.d_slow_clip + (long long)sp * plane : nullptr;
   const int cstep = d.n_t * plane, cstep_slow = d.n_slow * plane;
@@ -171,6 +179,12 @@ clip_transform_batch_kernel(pv_clip_batch_desc d, const SrcT* __restrict__ src, 
 #pragma unroll
     for (int i = 0; i < PX; ++i) {
       const int xo = min(xb + i, d.out_w - 1);
+      if constexpr (RRC) {      // taps relative to the window, then its origin
+        const TapXY t = bilinear_tap(flip ? d.out_w - 1 - xo : xo, win_w, scale_x);
+        xo0[i] = (left + t.i0) * sw; xo1[i] = (left + t.i1) * sw;
+        lx1[i] = t.l1; lx0[i] = 1.f - t.l1;
+        continue;
+      }
       const TapXY t = bilinear_tap(left + (flip ? d.out_w - 1 - xo : xo), d.in_w, scale_x);
       xo0[i] = t.i0 * sw; xo1[i] = t.i1 * sw;
       lx1[i] = t.l1; lx0[i] = 1.f - t.l1;
@@ -178,9 +192,9 @@ clip_transform_batch_kernel(pv_clip_batch_desc d, const SrcT* __restrict__ src, 
     const bool two = (xb + 1 < d.out_w);
     for (int r = threadIdx.y; r < n_rows; r += blockDim.y) {
       const int y = y_base + r;
-      const TapXY ty = bilinear_tap(top + y, d.in_h, scale_y);
+      const TapXY ty = RRC ? bilinear_tap(y, win_h, scale_y) : bilinear_tap(top + y, d.in_h, scale_y);
       const float ly1 = ty.l1, ly0 = 1.f - ly1;
-      const unsigned ro0 = ty.i0 * sh, ro1 = ty.i1 * sh;
+      const unsigned ro0 = ((RRC ? top : 0) + ty.i0) * sh, ro1 = ((RRC ? top : 0) + ty.i1) * sh;
       unsigned off[PX][4];
 #pragma unroll
       for (int i = 0; i < PX; ++i) {
@@ -230,6 +244,21 @@ clip_transform_batch_kernel(pv_clip_batch_desc d, const SrcT* __restrict__ src, 
       }
     }
   }
+}
+
+template <typename SrcT, typename OutT, int NC, bool LUT>
+__global__ void __launch_bounds__(TB_THREADS)
+clip_transform_batch_kernel(pv_clip_batch_desc d, const SrcT* __restrict__ src, const int32_t* __restrict__ idx_t,
+                            const int32_t* __restrict__ slow_pos, const int32_t* __restrict__ geom,
+                            OutT* __restrict__ dst, OutT* __restrict__ dst_slow) {
+  clip_transform_batch_body<SrcT, OutT, NC, LUT, false>(d, src, idx_t, slow_pos, geom, dst, dst_slow);
+}
+
+template <typename SrcT, typename OutT, bool LUT>
+__global__ void __launch_bounds__(TB_THREADS)
+clip_transform_rrc_kernel(pv_clip_batch_desc d, const SrcT* __restrict__ src, const int32_t* __restrict__ idx_t,
+                          const int32_t* __restrict__ boxes, OutT* __restrict__ dst) {
+  clip_transform_batch_body<SrcT, OutT, 3, LUT, true>(d, src, idx_t, nullptr, boxes, dst, nullptr);
 }
 
 }  // namespace pv
@@ -352,5 +381,39 @@ extern "C" int pv_clip_transform_batch(const pv_clip_batch_desc* d, const void* 
 #undef PV_TBC
 #undef PV_TB
   PV_LAUNCH_OK("clip_transform_batch_kernel");
+  return PV_OK;
+}
+
+extern "C" int pv_clip_transform_rrc(const pv_clip_batch_desc* d, const void* src, const int32_t* idx_t,
+                                     const int32_t* boxes, void* dst, void* stream) {
+  PV_CHECK_ARG(d && src && idx_t && boxes && dst, "null argument");
+  PV_CHECK_ARG(d->C == 3, "RandomResizedCrop mode needs 3 channels (got %d)", d->C);
+  PV_CHECK_ARG(d->n_clips >= 1 && d->n_t >= 1 && d->out_h >= 1 && d->out_w >= 1, "empty output");
+  PV_CHECK_ARG((long long)d->n_clips * d->n_t <= 65535, "grid too large");
+  PV_CHECK_ARG(d->in_h >= 1 && d->in_w >= 1, "bad frame size");
+  PV_CHECK_ARG(d->src_dtype == PV_U8 || d->src_dtype == PV_F32, "RandomResizedCrop mode reads uint8 or f32 clips");
+  PV_CHECK_ARG(d->dst_dtype == PV_F16 || d->dst_dtype == PV_F32, "RandomResizedCrop mode writes f16 or f32");
+  auto absll = [](long long v) { return v < 0 ? -v : v; };
+  PV_CHECK_ARG((long long)d->in_h * absll(d->sh) + (long long)d->in_w * absll(d->sw) < (1ll << 31) && d->sh >= 0 && d->sw >= 0,
+               "frame too large for 32-bit in-plane offsets");
+  PV_CHECK_ARG(3ll * d->n_t * d->out_h * d->out_w < (1ll << 31), "output clip too large for 32-bit offsets");
+  const int half_w = (d->out_w + 1) / 2;
+  const unsigned bx = (unsigned)(half_w >= pv::TB_THREADS ? pv::TB_THREADS : half_w);
+  const unsigned by = (unsigned)(pv::TB_THREADS / bx >= pv::TB_ROWS ? pv::TB_ROWS : (pv::TB_THREADS / bx < 1 ? 1 : pv::TB_THREADS / bx));
+  dim3 grid(1, (unsigned)pv::cdiv(d->out_h, pv::TB_ROWS), d->n_clips * d->n_t), block(bx, by);
+  PV_CHECK_ARG(grid.y <= 65535, "grid too large");
+  cudaStream_t s = (cudaStream_t)stream;
+  const bool h = d->dst_dtype == PV_F16;
+#define PV_RRC(ST, OT, LUT_)                                                                                         \
+  do {                                                                                                               \
+    pv::clip_transform_rrc_kernel<ST, OT, LUT_><<<grid, block, 0, s>>>(*d, (const ST*)src, idx_t, boxes, (OT*)dst); \
+    PV_LAUNCH_OK("clip_transform_rrc_kernel<" #ST "," #OT ">");                                                      \
+  } while (0)
+  if (d->src_dtype == PV_U8) {
+    if (h) PV_RRC(uint8_t, __half, true); else PV_RRC(uint8_t, float, true);
+  } else {
+    if (h) PV_RRC(float, __half, false); else PV_RRC(float, float, false);
+  }
+#undef PV_RRC
   return PV_OK;
 }

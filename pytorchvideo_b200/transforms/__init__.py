@@ -1,5 +1,5 @@
 from .transforms import (ApplyTransformToKey, CenterCropVideo, ConvertUint8ToFloat, Div255,  # noqa: F401
                          FusedClipTransform, Normalize, RandomCropVideo, RandomShortSideScale, ShortSideScale,
                          UniformCropVideo, UniformTemporalSubsample, create_video_transform, SlowFastPackPathway,
-                         RemoveKey)
+                         RemoveKey, RandomResizedCrop, Permute, RandAugment, AugMix)
 from . import functional  # noqa: F401

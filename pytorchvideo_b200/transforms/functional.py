@@ -349,3 +349,131 @@ def div_255(x):
 def uniform_crop(images, size, spatial_idx):
     y, xo, h, w = uniform_crop_window(images.shape[2], images.shape[3], size, spatial_idx)
     return images[:, :, y:y + h, xo:xo + w]   # a view, exactly like the reference's slicing
+
+
+# ---- RandomResizedCrop (functional.py random_resized_crop) --------------------------------------------------------
+def random_resized_crop_window(scale, ratio, height, width, log_uniform_ratio=True, num_tries=10):
+    """(top, left, h, w) of an Inception-style crop, drawn from torch's global RNG like the reference's
+    _get_param_spatial_crop: up to num_tries (area, aspect ratio) draws, then a central crop."""
+    assert num_tries >= 1, "num_tries must be at least 1"
+    if scale[0] > scale[1]:
+        scale = (scale[1], scale[0])
+    if ratio[0] > ratio[1]:
+        ratio = (ratio[1], ratio[0])
+    for _ in range(num_tries):
+        target_area = height * width * (scale[0] + torch.rand(1).item() * (scale[1] - scale[0]))
+        if log_uniform_ratio:
+            lo, hi = math.log(ratio[0]), math.log(ratio[1])
+            aspect = math.exp(lo + torch.rand(1).item() * (hi - lo))
+        else:
+            aspect = ratio[0] + torch.rand(1).item() * (ratio[1] - ratio[0])
+        w = int(round(math.sqrt(target_area * aspect)))
+        h = int(round(math.sqrt(target_area / aspect)))
+        if 0 < w <= width and 0 < h <= height:
+            i = torch.randint(0, height - h + 1, (1,)).item()
+            j = torch.randint(0, width - w + 1, (1,)).item()
+            return i, j, h, w
+    in_ratio = float(width) / float(height)
+    if in_ratio < min(ratio):
+        w, h = width, int(round(width / min(ratio)))
+    elif in_ratio > max(ratio):
+        h, w = height, int(round(height * max(ratio)))
+    else:
+        w, h = width, height
+    return (height - h) // 2, (width - w) // 2, h, w
+
+
+def random_resized_crop_boxes(t, height, width, scale, aspect_ratio, shift=False, log_uniform_ratio=True, num_tries=10):
+    """Per-frame (top, left, h, w) of one clip of t frames: one window for every frame, or with ``shift`` a second
+    window for the last frame and torch.linspace(...) + int() in between, as the reference."""
+    assert scale[0] > 0 and scale[1] > 0, "min and max of scale range must be greater than 0"
+    assert aspect_ratio[0] > 0 and aspect_ratio[1] > 0, "min and max of aspect_ratio range must be greater than 0"
+    box = random_resized_crop_window(scale, aspect_ratio, height, width, log_uniform_ratio, num_tries)
+    if not shift:
+        return [box] * t
+    box2 = random_resized_crop_window(scale, aspect_ratio, height, width, log_uniform_ratio, num_tries)
+    cols = [[int(v) for v in torch.linspace(a, b, steps=t).tolist()] for a, b in zip(box, box2)]
+    return list(zip(*cols))
+
+
+def clip_transform_rrc(x, boxes, target_hw, frame_idx=None, flips=None, mean=None, std=None, div255=False,
+                       out_dtype=torch.float32):
+    """The batched chain in RandomResizedCrop mode (pv_clip_transform_rrc): frame selection, /255, normalisation and
+    a per-(clip, kept frame) window resized to target_hw, then an optional per-clip horizontal flip, in ONE launch.
+
+    x     : (B, 3, T, H, W) or (3, T, H, W) uint8 / float32 CUDA clip(s), any strides
+    boxes : per clip, a list of (top, left, h, w) per kept frame
+    flips : per clip bool (None = no flip)"""
+    squeeze = torch.is_tensor(x) and x.dim() == 4
+    if squeeze:
+        x, boxes, flips = x.unsqueeze(0), [boxes], None if flips is None else [flips]
+    if not torch.is_tensor(x) or x.dim() != 5:
+        raise RuntimeError("expected a (B, C, T, H, W) or (C, T, H, W) tensor")
+    if x.device.type != "cuda":
+        raise RuntimeError("pytorchvideo_b200 transforms run on the GPU only (no CPU path)")
+    if x.dtype not in (torch.uint8, torch.float32):
+        raise RuntimeError("RandomResizedCrop reads uint8 or float32 clips (got %s)" % x.dtype)
+    if out_dtype not in (torch.float16, torch.float32):
+        raise RuntimeError("RandomResizedCrop writes float16 or float32 (got %s)" % out_dtype)
+    B, Cc, T, H, W = x.shape
+    if Cc != 3:
+        raise RuntimeError("RandomResizedCrop needs 3-channel clips (got %d)" % Cc)
+    idx = torch.arange(T) if frame_idx is None else torch.as_tensor(frame_idx).long().cpu()
+    if idx.numel() == 0 or int(idx.min()) < 0 or int(idx.max()) >= T:
+        raise RuntimeError("frame index out of range")
+    n_t = int(idx.numel())
+    oh, ow = int(target_hw[0]), int(target_hw[1])
+    if len(boxes) != B or any(len(b) != n_t for b in boxes):
+        raise RuntimeError("boxes needs one window per kept frame of every clip")
+    flat = []
+    for b in range(B):
+        f = 1 if flips is not None and flips[b] else 0
+        for top, left, h, w in boxes[b]:
+            if top < 0 or left < 0 or h < 1 or w < 1 or top + h > H or left + w > W:
+                raise RuntimeError("crop window (%d, %d, %d, %d) outside the %dx%d frame" % (top, left, h, w, H, W))
+            flat += [int(top), int(left), int(h), int(w), f]
+    lib = L.load()
+    dev = x.device
+    d = L.ClipBatchDesc()
+    d.C, d.n_clips, d.n_t = Cc, B, n_t
+    d.in_h, d.in_w, d.new_h, d.new_w = H, W, oh, ow
+    d.out_h, d.out_w = oh, ow
+    d.s_clip, d.sc, d.st, d.sh, d.sw = x.stride(0), x.stride(1), x.stride(2), x.stride(3), x.stride(4)
+    normalize = mean is not None or std is not None
+    mean_l = [float(m) for m in (mean if mean is not None else [0.0] * Cc)]
+    std_l = [float(v) for v in (std if std is not None else [1.0] * Cc)]
+    mean_l = mean_l * Cc if len(mean_l) == 1 else mean_l
+    std_l = std_l * Cc if len(std_l) == 1 else std_l
+    for i in range(4):
+        d.mean[i] = mean_l[i] if i < len(mean_l) else 0.0
+        d.stdv[i] = std_l[i] if i < len(std_l) else 1.0
+    d.div255, d.normalize = 1 if div255 else 0, 1 if normalize else 0
+    d.src_dtype, d.dst_dtype = _DT[x.dtype], _DT[out_dtype]
+    out = torch.empty((B, Cc, n_t, oh, ow), dtype=out_dtype, device=dev)
+    d.d_clip = out.stride(0)
+    idx_d = _dev_i32(idx.tolist(), dev)
+    boxes_d = torch.tensor(flat, dtype=torch.int32).to(dev)
+    L.check(lib.pv_clip_transform_rrc(C.byref(d), x.data_ptr(), idx_d.data_ptr(), boxes_d.data_ptr(), out.data_ptr(),
+                                      torch.cuda.current_stream(dev).cuda_stream), "pv_clip_transform_rrc")
+    out._pv_keepalive = (idx_d, boxes_d)
+    return out[0] if squeeze else out
+
+
+def random_resized_crop(frames, target_height, target_width, scale, aspect_ratio, shift=False, log_uniform_ratio=True,
+                        interpolation="bilinear", num_tries=10):
+    """Reference functional.random_resized_crop on a float32 (C, T, H, W) CUDA clip, or a (B, C, T, H, W) batch with
+    one independent draw per clip in clip order.  Bilinear only."""
+    if interpolation != "bilinear":
+        raise NotImplementedError("only bilinear RandomResizedCrop has a kernel (got %r)" % (interpolation,))
+    if not torch.is_tensor(frames) or frames.dim() not in (4, 5):
+        raise RuntimeError("expected a (C, T, H, W) or (B, C, T, H, W) tensor")
+    if frames.device.type != "cuda":
+        raise RuntimeError("pytorchvideo_b200 transforms run on the GPU only (no CPU path)")
+    if frames.dtype != torch.float32:
+        raise RuntimeError("random_resized_crop takes float32 clips (got %s)" % frames.dtype)
+    x = frames.unsqueeze(0) if frames.dim() == 4 else frames
+    T, H, W = x.shape[2], x.shape[3], x.shape[4]
+    boxes = [random_resized_crop_boxes(T, H, W, scale, aspect_ratio, shift, log_uniform_ratio, num_tries)
+             for _ in range(x.shape[0])]
+    out = clip_transform_rrc(x, boxes, (target_height, target_width))
+    return out[0] if frames.dim() == 4 else out

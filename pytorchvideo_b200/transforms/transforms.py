@@ -9,6 +9,7 @@ import torch
 import torch.nn as nn
 
 from . import functional as Fv
+from .augment import AugMix, RandAugment  # noqa: F401
 
 
 class ApplyTransformToKey:
@@ -109,13 +110,58 @@ class UniformCropVideo(nn.Module):
         return x
 
 
+class RandomResizedCrop(nn.Module):
+    """Reference RandomResizedCrop on float32 (C, T, H, W) clips, or (B, C, T, H, W) with one draw per clip."""
+
+    def __init__(self, target_height, target_width, scale, aspect_ratio, shift=False, log_uniform_ratio=True,
+                 interpolation="bilinear", num_tries=10):
+        super().__init__()
+        self._args = (target_height, target_width, scale, aspect_ratio, shift, log_uniform_ratio, interpolation,
+                      num_tries)
+
+    def forward(self, x):
+        return Fv.random_resized_crop(x, *self._args)
+
+
+class Permute(nn.Module):
+    """x.permute(*dims): a view, which the augmentation and transform kernels read without a copy."""
+
+    def __init__(self, dims):
+        super().__init__()
+        if sorted(dims) != list(range(len(dims))):
+            raise ValueError("dims must contain every dimension (0, 1, 2, ...) once")
+        self._dims = tuple(dims)
+
+    def forward(self, x):
+        return x.permute(*self._dims)
+
+
+_RRC_KEYS = ("target_height", "target_width", "scale", "aspect_ratio", "shift", "log_uniform_ratio", "interpolation",
+             "num_tries")
+
+
 class FusedClipTransform(nn.Module):
     """One-kernel eval/train chain.  crop: None | ("center", size) | ("random", size) |
-    ("uniform", size, spatial_idx).  Input: uint8 (or float) CUDA clip (C, T, H, W)."""
+    ("uniform", size, spatial_idx).  Input: uint8 (or float) CUDA clip (C, T, H, W).
+
+    random_resized_crop: dict of RandomResizedCrop's arguments (target_height, target_width, scale, aspect_ratio and
+    optionally shift, log_uniform_ratio, interpolation, num_tries).  It replaces short_side / crop: frame selection,
+    /255, normalisation, the random resized crop and the flip run as one launch; a batch draws per clip."""
 
     def __init__(self, num_samples=None, mean=None, std=None, short_side=None, crop=None, div255=True,
-                 out_dtype=torch.float16, random_short_side=None, hflip_prob=0.0, slowfast_alpha=None):
+                 out_dtype=torch.float16, random_short_side=None, hflip_prob=0.0, slowfast_alpha=None,
+                 random_resized_crop=None):
         super().__init__()
+        if random_resized_crop is not None:
+            unknown = set(random_resized_crop) - set(_RRC_KEYS)
+            if unknown:
+                raise ValueError("unknown random_resized_crop arguments %s" % sorted(unknown))
+            if short_side is not None or crop is not None or random_short_side is not None or slowfast_alpha is not None:
+                raise ValueError("random_resized_crop replaces short_side / random_short_side / crop and has no "
+                                 "slow pathway output")
+            if random_resized_crop.get("interpolation", "bilinear") != "bilinear":
+                raise NotImplementedError("only bilinear RandomResizedCrop has a kernel")
+        self.random_resized_crop = random_resized_crop
         self.num_samples, self.mean, self.std = num_samples, mean, std
         self.short_side, self.crop, self.div255, self.out_dtype = short_side, crop, div255, out_dtype
         self.random_short_side = random_short_side
@@ -151,10 +197,31 @@ class FusedClipTransform(nn.Module):
             flip = bool(torch.rand(1) < self.hflip_prob)
         return idx, hw, win, flip
 
+    def _forward_rrc(self, x):
+        rrc = dict(self.random_resized_crop)
+        clips = x.unsqueeze(0) if x.dim() == 4 else x
+        _, _, T, H, W = clips.shape
+        idx = None if self.num_samples is None else Fv.temporal_indices(T, self.num_samples)
+        n_t = T if idx is None else int(idx.numel())
+        boxes, flips = [], []
+        for _ in range(clips.shape[0]):      # per clip: the crop's draws, then the flip's
+            boxes.append(Fv.random_resized_crop_boxes(n_t, H, W, rrc["scale"], rrc["aspect_ratio"],
+                                                      rrc.get("shift", False), rrc.get("log_uniform_ratio", True),
+                                                      rrc.get("num_tries", 10)))
+            flips.append(bool(torch.rand(1) < self.hflip_prob) if self.hflip_prob > 0.0 else False)
+        out = Fv.clip_transform_rrc(clips, boxes, (rrc["target_height"], rrc["target_width"]), frame_idx=idx,
+                                    flips=flips, mean=self.mean, std=self.std, div255=self.div255,
+                                    out_dtype=self.out_dtype)
+        return out[0] if x.dim() == 4 else out
+
     def forward(self, x, out=None):
         """x: one clip (C, T, H, W) or a batch (B, C, T, H, W) - ONE launch either way (a batch in train mode
         draws short side / crop / flip per clip, in clip order).  Returns the clip(s), or [slow, fast] when
         ``slowfast_alpha`` is set."""
+        if self.random_resized_crop is not None:
+            if out is not None:
+                raise ValueError("out= is not supported with random_resized_crop")
+            return self._forward_rrc(x)
         if x.dim() == 5 and self._is_random():
             plans = [self.plan(x.shape[1:]) for _ in range(x.shape[0])]
             idx, hw, win, _ = plans[0]
