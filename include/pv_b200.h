@@ -179,6 +179,39 @@ int pv_augment_apply(const pv_augment_desc* d, const void* src, const pv_aug_op*
 int pv_augment_mix(const pv_augment_desc* d, const void* src, const void* chains, int width, const float* mix,
                    void* dst, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Batch mixing (transforms/mix.py: MixUp, CutMix, MixVideo), in place on a batch of B clips.  Clip b pairs with clip
+ * B-1-b.  Element e of clip b sits at x[b*s_batch + sum_i idx_i*stride[i]] over the per-clip dims size[0..3]
+ * (outermost first, padded with 1 at the front); any strides, but no two elements may share memory.
+ * pv_mixup: x[b] = T(T(x[b]*lam) + T(x[B-1-b]*oml)) for every b at once (the middle clip of an odd B mixes with
+ *   itself), one rounding to the element type T (PV_F32 | PV_F16) per product and per sum; fp32 products.
+ * pv_cutmix: swaps x[b][..., yl:yh, xl:xh] with x[B-1-b][..., yl:yh, xl:xh]; size[2], size[3] are H, W.  Any element
+ *   size (PV_U8 | PV_F16 | PV_F32).  An empty box launches nothing.
+ * pv_mix_labels: the (B, K) float32 label mix out[b] = f(f(l1*lam) + f(l2*oml)), l1 / l2 the label rows of clips b and
+ *   B-1-b: one-hot rows (on at the class, off elsewhere) built from int64 indices, or float32 rows given (one_hot).
+ *   mode 1 / 2 writes the one-hot row of clip b alone, as float32 / int64 (convert_to_one_hot).  Indices are checked:
+ *   *flag |= 1 for an index >= K, |= 2 for a negative one (flag is zeroed first, on the stream).                      */
+typedef struct pv_mix_desc {
+  int B;                  /* clips in the batch                  */
+  int dtype;              /* PV_F32 | PV_F16 | PV_U8             */
+  long long size[4];      /* per-clip dims, outermost first      */
+  long long stride[4];    /* their strides in elements           */
+  long long s_batch;      /* stride between clips in elements    */
+} pv_mix_desc;
+
+typedef struct pv_mix_label_desc {
+  int B, K;
+  int one_hot;            /* labels are float32 (B, K) rows, not int64 indices             */
+  int mode;               /* 0: mix; 1: one-hot rows as float32; 2: one-hot rows as int64   */
+  float lam, oml;         /* the two weights, each already rounded to float32              */
+  float on, off;          /* one-hot values: 1 - ls + ls/K and ls/K, rounded from double   */
+  long long s_row, s_col; /* label strides in elements (s_col unused for indices)          */
+} pv_mix_label_desc;
+
+int pv_mixup(const pv_mix_desc* d, void* x, float lam, float oml, void* stream);
+int pv_cutmix(const pv_mix_desc* d, void* x, int yl, int yh, int xl, int xh, void* stream);
+int pv_mix_labels(const pv_mix_label_desc* d, const void* labels, void* out, int* flag, void* stream);
+
 /* Test-time multi-view ensembling (pytorchvideo_trainer/module/video_classification.py:290-311, docs model_zoo.md:63
  * "3 spatial x 10 temporal views"): out[v][k] = reduce over the n_views consecutive rows of video v;
  * mode 0 = sum, 1 = mean (sum / clip count), 2 = max.  preds: [n_videos * n_views][K] f32.                    */

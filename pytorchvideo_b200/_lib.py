@@ -51,6 +51,16 @@ class AugmentDesc(C.Structure):
                 ("dtype", C.c_int)]
 
 
+class MixDesc(C.Structure):
+    _fields_ = [("B", C.c_int), ("dtype", C.c_int), ("size", c_ll * 4), ("stride", c_ll * 4), ("s_batch", c_ll)]
+
+
+class MixLabelDesc(C.Structure):
+    _fields_ = [("B", C.c_int), ("K", C.c_int), ("one_hot", C.c_int), ("mode", C.c_int),
+                ("lam", C.c_float), ("oml", C.c_float), ("on", C.c_float), ("off", C.c_float),
+                ("s_row", c_ll), ("s_col", c_ll)]
+
+
 class BottleneckDesc(C.Structure):
     _fields_ = [("N", C.c_int), ("T", C.c_int), ("H", C.c_int), ("W", C.c_int),
                 ("Cin", C.c_int), ("Cmid", C.c_int), ("Cout", C.c_int), ("kt", C.c_int), ("sb", C.c_int),
@@ -107,6 +117,9 @@ SIGNATURES = {
     "pv_augment_stats": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, c_vp]),
     "pv_augment_apply": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_augment_mix": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp]),
+    "pv_mixup": (C.c_int, [C.POINTER(MixDesc), c_vp, C.c_float, C.c_float, c_vp]),
+    "pv_cutmix": (C.c_int, [C.POINTER(MixDesc), c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp]),
+    "pv_mix_labels": (C.c_int, [C.POINTER(MixLabelDesc), c_vp, c_vp, c_vp, c_vp]),
     "pv_view_reduce": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp]),
     "pv_ncdhw_to_ndhwc": (C.c_int, [c_vp, C.c_int, c_vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_int, C.c_int, c_ll, c_vp]),

@@ -2,4 +2,5 @@ from .transforms import (ApplyTransformToKey, CenterCropVideo, ConvertUint8ToFlo
                          FusedClipTransform, Normalize, RandomCropVideo, RandomShortSideScale, ShortSideScale,
                          UniformCropVideo, UniformTemporalSubsample, create_video_transform, SlowFastPackPathway,
                          RemoveKey, RandomResizedCrop, Permute, RandAugment, AugMix)
+from .mix import CutMix, MixUp, MixVideo  # noqa: F401
 from . import functional  # noqa: F401

@@ -11,6 +11,7 @@ import numpy as np
 import torch
 
 from .. import _lib as L
+from .mix import convert_to_one_hot  # noqa: F401
 
 _DT = {torch.uint8: L.PV_U8, torch.float32: L.PV_F32, torch.float16: L.PV_F16}
 _TABLE_CACHE = {}
