@@ -424,6 +424,12 @@ int pv_head_reduce(const void* x, int dtype, long long row_stride, int N, long l
  *                batch strides (B > 1) of at least N rows and all strides below 2^40 bytes; everything else (and
  *                f32) runs the CUDA-core flash kernel.  pv_attention_kernel_for tells which one a call would launch;
  *                should the driver still refuse a tensor map, pv_attention_fwd returns PV_ERR_CUDA.
+ *                Wide heads and the linear mode (Non-local block, layers/nonlocal_net.py:55-94): normalize = 1
+ *                replaces the softmax by o = ((q k^T) * scale / Nk) v (the "dot_product" instantiation; no q
+ *                residual, PV_ERR_INVALID otherwise).  Head dims 256 / 512 (either mode) and 64 / 128 with
+ *                normalize = 1 run csrc/pv_attention_wide.cu: the f16 wgmma + TMA kernel (PV_ATTN_WIDE) under the
+ *                alignment rules above, its CUDA-core twin for f32 and everything else.  normalize = 0 keeps the
+ *                routing and results of the head dims 32-128 unchanged; other head dims are PV_ERR_UNSUPPORTED.
  * ------------------------------------------------------------------------------------------- */
 int pv_layernorm(const void* x, void* y, int dtype, long long rows, int groups, int C,
                  long long x_row_stride, long long y_row_stride, const float* gamma,
@@ -465,6 +471,7 @@ typedef struct pv_attention_desc {
   long long q_batch_stride, k_batch_stride, v_batch_stride, o_batch_stride;
   float scale;
   int add_q_residual;   /* residual_pool=True: o += q (cls row included, attention.py:535-536) */
+  int normalize;        /* 0 = softmax (today's behaviour), 1 = divide by Nk */
 } pv_attention_desc;
 int pv_attention_fwd(const pv_attention_desc* d, const void* q, const void* k, const void* v,
                      void* o, void* stream);
@@ -473,7 +480,8 @@ int pv_attention_fwd(const pv_attention_desc* d, const void* q, const void* k, c
 typedef enum pv_attention_kernel {
   PV_ATTN_WGMMA = 1,    /* f16 wgmma + TMA flash kernel                */
   PV_ATTN_MMA = 2,      /* f16 mma.sync flash kernel                   */
-  PV_ATTN_SIMT = 3      /* CUDA-core flash kernel (f16 or f32 storage) */
+  PV_ATTN_SIMT = 3,     /* CUDA-core flash kernel (f16 or f32 storage) */
+  PV_ATTN_WIDE = 4      /* f16 wgmma + TMA kernel for wide heads / the linear mode */
 } pv_attention_kernel;
 int pv_attention_kernel_for(const pv_attention_desc* d, const void* q, const void* k, const void* v, const void* o);
 

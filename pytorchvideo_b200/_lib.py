@@ -12,7 +12,7 @@ PV_F16, PV_F32, PV_U8 = 0, 1, 2
 ACT_NONE, ACT_RELU, ACT_SWISH, ACT_GELU, ACT_SIGMOID = 0, 1, 2, 3, 4
 ALGO_AUTO, ALGO_DIRECT, ALGO_TCGEN05 = 0, 1, 2
 POOL_MAX, POOL_AVG = 0, 1
-ATTN_WGMMA, ATTN_MMA, ATTN_SIMT = 1, 2, 3
+ATTN_WGMMA, ATTN_MMA, ATTN_SIMT, ATTN_WIDE = 1, 2, 3, 4
 
 c_ll = C.c_longlong
 c_vp = C.c_void_p
@@ -99,7 +99,7 @@ class AttentionDesc(C.Structure):
                 ("o_row_stride", c_ll),
                 ("q_batch_stride", c_ll), ("k_batch_stride", c_ll), ("v_batch_stride", c_ll),
                 ("o_batch_stride", c_ll),
-                ("scale", C.c_float), ("add_q_residual", C.c_int)]
+                ("scale", C.c_float), ("add_q_residual", C.c_int), ("normalize", C.c_int)]
 
 
 # name -> (restype, argtypes); mirrors include/pv_b200.h one to one (tests check this list

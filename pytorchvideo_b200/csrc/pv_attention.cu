@@ -127,6 +127,16 @@ int attention_wgmma_launch(const pv_attention_desc* d, const void* q, const void
                           cudaStream_t s);   // pv_attention_wgmma.cu
 int attention_mma_launch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
                          cudaStream_t s);    // pv_attention_mma.cu
+int attention_wide_launch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
+                          cudaStream_t s);   // pv_attention_wide.cu
+int attention_wide_simt_launch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
+                               cudaStream_t s);   // pv_attention_wide.cu
+
+// Calls the kernels of pv_attention_wide.cu take: head dims 256 / 512 in either mode, and the linear mode
+// (normalize = 1) at 64 / 128.
+static bool wide_family(const pv_attention_desc* d) {
+  return d->D == 256 || d->D == 512 || d->normalize != 0;
+}
 
 // The f16 tensor-core kernels read q / k / v with 16-byte cp.async / TMA and 4-byte fragment loads from every batch,
 // head and row start, and store o as __half2: pointers, row strides and batch strides must keep that alignment.  The
@@ -156,12 +166,19 @@ extern "C" int pv_attention_kernel_for(const pv_attention_desc* d, const void* q
   PV_CHECK_ARG(d->dtype == PV_F16 || d->dtype == PV_F32, "attention dtype must be f16|f32");
   PV_CHECK_ARG(d->B > 0 && d->H > 0 && d->Nq > 0 && d->Nk > 0, "empty attention problem");
   PV_CHECK_ARG((long long)d->B * d->H <= 65535, "B*H too large");
-  if (d->D != 32 && d->D != 64 && d->D != 96 && d->D != 128) {
-    pv::set_error("attention head dim %d unsupported (32/64/96/128)", d->D);
+  PV_CHECK_ARG(d->normalize == 0 || d->normalize == 1, "attention normalize must be 0 (softmax) or 1 (divide by Nk)");
+  PV_CHECK_ARG(!(d->normalize && d->add_q_residual), "attention normalize = 1 takes no q residual");
+  if (d->D != 32 && d->D != 64 && d->D != 96 && d->D != 128 && d->D != 256 && d->D != 512) {
+    pv::set_error("attention head dim %d unsupported (32/64/96/128/256/512)", d->D);
     return PV_ERR_UNSUPPORTED;
   }
-  if (d->dtype == PV_F16 && !getenv("PVB200_ATTN_SIMT") && pv::tensor_core_aligned(d, q, k, v, o))
-    return d->D == 128 ? PV_ATTN_MMA : PV_ATTN_WGMMA;
+  if (d->normalize && d->D != 64 && d->D != 128 && d->D != 256 && d->D != 512) {
+    pv::set_error("linear attention (normalize = 1) head dim %d unsupported (64/128/256/512)", d->D);
+    return PV_ERR_UNSUPPORTED;
+  }
+  const bool tc = d->dtype == PV_F16 && !getenv("PVB200_ATTN_SIMT") && pv::tensor_core_aligned(d, q, k, v, o);
+  if (pv::wide_family(d)) return tc ? PV_ATTN_WIDE : PV_ATTN_SIMT;
+  if (tc) return d->D == 128 ? PV_ATTN_MMA : PV_ATTN_WGMMA;
   return PV_ATTN_SIMT;
 }
 
@@ -172,7 +189,9 @@ extern "C" int pv_attention_fwd(const pv_attention_desc* d, const void* q, const
   cudaStream_t s = (cudaStream_t)stream;
   if (kernel == PV_ATTN_WGMMA) return pv::attention_wgmma_launch(d, q, k, v, o, s);
   if (kernel == PV_ATTN_MMA) return pv::attention_mma_launch(d, q, k, v, o, s);
-#define PV_ATT(DD)                                                                                          \
+  if (kernel == PV_ATTN_WIDE) return pv::attention_wide_launch(d, q, k, v, o, s);
+  if (pv::wide_family(d)) return pv::attention_wide_simt_launch(d, q, k, v, o, s);
+#define PV_ATT(DD)                                                                                         \
   if (d->D == DD)                                                                                           \
     return d->dtype == PV_F16                                                                               \
                ? pv::launch_attention<__half, DD>(d, q, k, v, o, s, "attention_kernel<__half," #DD ">")     \

@@ -261,6 +261,58 @@ class Lowering:
                                          _act_code(m.act_b), name + ".se")
         return self.conv(h, m.conv_c, m.norm_c, final_act, shortcut, name + ".conv_c")
 
+    # head widths of the Non-local attention core (csrc/pv_attention.cu routing): softmax also runs on the MViT
+    # kernels' 32 / 96, the linear ("dot_product") mode only on the widths of csrc/pv_attention_wide.cu
+    _NL_DIMS = {"softmax": (32, 64, 96, 128, 256, 512), "dot_product": (64, 128, 256, 512)}
+
+    def lower_NonLocal(self, m, x, name):
+        # layers/nonlocal_net.py:55-94: theta from x, phi / g from pool(x), one single-head attention of width
+        # dim_inner, conv_out (+ norm) with x as the fused residual; no activation
+        name = name or "nonlocal"
+        convs = (m.conv_theta, m.conv_phi, m.conv_g, m.conv_out)
+        for cn, c in zip(("conv_theta", "conv_phi", "conv_g", "conv_out"), convs):
+            if not isinstance(c, nn.Conv3d) or _t3(c.kernel_size) != (1, 1, 1) or _t3(c.stride) != (1, 1, 1) \
+                    or isinstance(c.padding, str) or _t3(c.padding) != (0, 0, 0) or _t3(c.dilation) != (1, 1, 1) \
+                    or c.groups != 1:
+                raise NotImplementedError("%s.%s: NonLocal needs 1x1x1 convolutions of stride 1, groups 1" % (name, cn))
+        if m.norm is not None and not _is_bn(m.norm):
+            raise NotImplementedError("%s: norm %s unsupported (BatchNorm only)" % (name, type(m.norm).__name__))
+        if m.instantiation not in self._NL_DIMS:
+            raise NotImplementedError("%s: instantiation %r unsupported" % (name, m.instantiation))
+        di = m.conv_theta.out_channels
+        if di not in self._NL_DIMS[m.instantiation]:
+            raise NotImplementedError("%s: dim_inner %d unsupported for %s (supported: %s)" % (
+                name, di, m.instantiation, self._NL_DIMS[m.instantiation]))
+        if m.conv_theta.in_channels != x.C:
+            raise RuntimeError("conv %s.conv_theta expects %d input channels, got %d" % (name, m.conv_theta.in_channels, x.C))
+
+        def fused(cs):
+            w = torch.cat([c.weight for c in cs], 0)
+            if all(c.bias is None for c in cs):
+                return w, None
+            return w, torch.cat([c.bias if c.bias is not None else torch.zeros(c.out_channels) for c in cs], 0)
+
+        p = self.p
+        if m.pool is not None:
+            w, b = fused((m.conv_theta,))
+            theta = p.emit_conv(x, w, b, None, (1, 1, 1), (0, 0, 0), (1, 1, 1), 1, L.ACT_NONE, None, name + ".conv_theta")
+            xp = self.pool(x, m.pool, name + ".pool")
+            w, b = fused((m.conv_phi, m.conv_g))
+            pg = p.emit_conv(xp, w, b, None, (1, 1, 1), (0, 0, 0), (1, 1, 1), 1, L.ACT_NONE, None, name + ".conv_phi_g")
+            phi, g = PL.channel_slice(pg, 0, di), PL.channel_slice(pg, di, di)
+        else:
+            w, b = fused((m.conv_theta, m.conv_phi, m.conv_g))
+            tpg = p.emit_conv(x, w, b, None, (1, 1, 1), (0, 0, 0), (1, 1, 1), 1, L.ACT_NONE, None,
+                              name + ".conv_theta_phi_g")
+            theta, phi, g = (PL.channel_slice(tpg, i * di, di) for i in range(3))
+        if m.instantiation == "softmax":
+            o = PL.emit_attention(p, theta, phi, g, 1, di ** -0.5, False, name + ".attention")
+        else:
+            o = PL.emit_attention(p, theta, phi, g, 1, 1.0, False, name + ".attention", normalize=1)
+        # the attention output is token-major [N][T*H*W][dim_inner]: the same rows as x, so give it x's grid back
+        o = TRef(o.buf, x.N, x.T, x.H, x.W, o.C, Cp=o.Cp, ch_off=o.ch_off, row_stride=o.row_stride)
+        return self.conv(o, m.conv_out, m.norm, None, x, name + ".conv_out")
+
     def lower_MultiPathWayWithFuse(self, m, x, name):
         # models/net.py:107-122
         assert isinstance(x, list), "input for MultiPathWayWithFuse needs to be a list of tensors"

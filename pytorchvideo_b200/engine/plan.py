@@ -80,6 +80,7 @@ class Plan:
         self.use_tcgen05 = bool(use_tcgen05) and dt == L.PV_F16
         self.ops = []          # (name, closure(stream_ptr))
         self.meta = []         # per-op {name, kind, flops, bytes} (algorithmic figures for the roofline)
+        self.attention_calls = []   # per attention op: its problem (B, H, Nq, Nk, D, scale, normalize, residual)
         self.bufs = []
         self.consts = []       # keep device parameter tensors alive
         self.zero_bufs = []    # f32 accumulators that must be cleared every run (SE sums)
@@ -895,7 +896,8 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool"):
     return y, (To, Ho, Wo)
 
 
-def emit_attention(plan, q, k, v, heads, scale, residual_pool, name="attn"):
+def emit_attention(plan, q, k, v, heads, scale, residual_pool, name="attn", normalize=0):
+    """normalize = 1: the linear mode of pv_attention_fwd (scores * scale / Nk, no softmax)."""
     import ctypes as C_
     B, Nq, Nk, dim = q.N, q.npos, k.npos, q.C
     assert k.C == dim and v.C == dim and v.npos == Nk and dim % heads == 0
@@ -903,6 +905,7 @@ def emit_attention(plan, q, k, v, heads, scale, residual_pool, name="attn"):
     d = L.AttentionDesc()
     d.dtype, d.B, d.H, d.Nq, d.Nk, d.D = plan.dt, B, heads, Nq, Nk, dim // heads
     d.scale, d.add_q_residual = float(scale), 1 if residual_pool else 0
+    d.normalize = int(normalize)
     lib = plan.lib
 
     def fn(stream):
@@ -912,6 +915,8 @@ def emit_attention(plan, q, k, v, heads, scale, residual_pool, name="attn"):
         L.check(lib.pv_attention_fwd(C_.byref(d), q.ptr(), k.ptr(), v.ptr(), o.ptr(), stream), "pv_attention_fwd(%s)" % name)
     plan.add(name, fn, "attention", 4.0 * B * heads * Nq * Nk * (dim // heads),
              (B * Nq * dim * 2 + 2 * B * Nk * dim) * _ESIZE[plan.dt])
+    plan.attention_calls.append({"name": name, "B": B, "H": heads, "Nq": Nq, "Nk": Nk, "D": dim // heads,
+                                 "scale": d.scale, "normalize": d.normalize, "add_q_residual": d.add_q_residual})
     return o
 
 

@@ -351,3 +351,35 @@ def assert_close_to_f64(got, ref64, absref64, k_len, acc_eps=ACC_EPS, what="", e
         limit = 0.25 * step + acc_eps * float(absref64[normal].mean())
         assert abs(bias) <= limit, "%s: mean signed error %.3g exceeds %.3g (biased rounding)" % (what, bias, limit)
     return float(ratio.max()), acc_ratio, extra_ratio
+
+
+# ---- Non-local block cases (tests/golden/nonlocal.pt): name -> (create_nonlocal kwargs, input shape) ---------------
+NONLOCAL_CASES = {
+    # I3D-NLN res3 / res4 widths (softmax, (1,2,2) pool): the wide tensor-core kernel at D = 256 / 512
+    "softmax_pool_512_256": (dict(dim_in=512, dim_inner=256, pool_size=(1, 2, 2)), (1, 512, 1, 6, 8)),
+    "softmax_pool_1024_512": (dict(dim_in=1024, dim_inner=512, pool_size=(1, 2, 2)), (1, 1024, 1, 4, 6)),
+    # the remaining cases keep dim_in narrow (it only sets the GEMM widths and the size of the stored output) and
+    # dim_inner at the head width under test
+    # "dot_product" without a pool: one theta|phi|g GEMM, the linear mode at D = 256
+    "dot_product_nopool_64_256": (dict(dim_in=64, dim_inner=256, pool_size=None, instantiation="dot_product"),
+                                  (1, 64, 2, 6, 6)),
+    "softmax_pool_norm_none": (dict(dim_in=64, dim_inner=256, pool_size=(1, 2, 2), norm=None), (1, 64, 2, 8, 8)),
+    # ragged grid the pool floors: 3x7x9 -> 3x3x4 keys
+    "softmax_pool_ragged": (dict(dim_in=64, dim_inner=256, pool_size=(1, 2, 2)), (1, 64, 3, 7, 9)),
+    # narrow heads: softmax on the MViT kernels, the linear mode on the wide family
+    "softmax_pool_32_64": (dict(dim_in=32, dim_inner=64, pool_size=(1, 2, 2)), (1, 32, 2, 8, 8)),
+    "softmax_pool_32_128": (dict(dim_in=32, dim_inner=128, pool_size=(1, 2, 2)), (1, 32, 2, 8, 8)),
+    "dot_product_pool_32_64": (dict(dim_in=32, dim_inner=64, pool_size=(1, 2, 2), instantiation="dot_product"),
+                               (1, 32, 2, 8, 8)),
+}
+
+
+def build_nonlocal_case(name, create_nonlocal, seed=91):
+    """(module, input) of a NONLOCAL_CASES entry built with ``create_nonlocal`` (this package's or the reference's);
+    weights and input on the f16 grid, random BatchNorm statistics."""
+    kw, shape = NONLOCAL_CASES[name]
+    torch.manual_seed(seed)
+    m = randomize_model(create_nonlocal(**kw), seed=seed, f16_weights=True).eval()
+    g = torch.Generator(device="cpu")
+    g.manual_seed(seed + 1)
+    return m, f16_exact(torch.randn(shape, generator=g))
