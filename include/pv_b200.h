@@ -282,6 +282,19 @@ typedef struct pv_conv3d_desc {
    * not T*H*W*row_stride apart (MViT token tensors carry a cls row in front of every sample's
    * T*H*W patch tokens).  0 = densely packed.                                                   */
   long long x_batch_stride, y_batch_stride;
+  /* Post-activation addend, constant over (h, w) (the audio fusion add of FuseAudioToFastSlow,
+   * models/audio_visual_slowfast.py:406-418):
+   *   y[n][t][h][w][c] = act(conv * scale + bias (+ residual)) + addend[n * add_n_stride + t * add_t_stride + add_ch_off + c]
+   * for output sample n and frame t; add_t_stride = 0 broadcasts one row over every frame.  Storage dtype of y,
+   * Co elements from add_ch_off on.  Co, add_n_stride, add_t_stride and add_ch_off are multiples of 8 elements, the
+   * pointer is 16-byte aligned and the output has fewer than 2^31 positions (else PV_ERR_INVALID from
+   * pv_conv3d_fwd; pv_conv3d_tcgen05_supported and pv_conv3d_stem_rows_supported return 0).  Dense (PV_ALGO_DIRECT, PV_ALGO_TCGEN05 incl. grouped mode) and stem-rows
+   * convolutions take it; depthwise convolutions return PV_ERR_UNSUPPORTED.  On the tensor cores the addend is
+   * added to the f16 result in the staged output tile (one more f16 rounding); PV_ALGO_DIRECT adds it in fp32.
+   * NULL = no addend (a zero-initialised descriptor behaves as without these fields).                     */
+  const void* addend;
+  long long add_n_stride, add_t_stride;
+  int add_ch_off;
 } pv_conv3d_desc;
 
 /* Temporal tap reduction used to factor a (kt,kh,kw) stem convolution with few output channels into

@@ -47,6 +47,14 @@ void count_launch(const char* name);
 
 static inline long long cdiv(long long a, long long b) { return (a + b - 1) / b; }
 
+// Layout rules of pv_conv3d_desc.addend (16-byte vectors of 8 channels on every path that takes it, so Co % 8 == 0:
+// the last vector of a row must not reach past the Co channels of the addend slice).
+static inline bool conv3d_addend_ok(const pv_conv3d_desc* d) {
+  return !d->addend || ((uintptr_t)d->addend % 16 == 0 && d->Co % 8 == 0 && d->add_n_stride >= 0 && d->add_t_stride >= 0 &&
+                        d->add_ch_off >= 0 && d->add_n_stride % 8 == 0 && d->add_t_stride % 8 == 0 &&
+                        d->add_ch_off % 8 == 0 && (long long)d->N * d->To * d->Ho * d->Wo < (1ll << 31));
+}
+
 // ---- per-device launch state -------------------------------------------------------------------
 // Function attributes (opt-in dynamic shared memory) and the SM count are PER DEVICE: a process that runs a
 // plan on cuda:0 and later on cuda:1 must opt in again on the second device.  One flag word per launch site,

@@ -353,6 +353,7 @@ extern "C" int pv_dwconv3d_fwd(const pv_conv3d_desc* d, const void* x, const voi
   PV_CHECK_ARG(d && x && w && scale && bias && y, "null pointer");
   PV_CHECK_ARG(d->groups == d->Ci && d->Ci == d->Co, "pv_dwconv3d_fwd is depthwise only");
   PV_CHECK_ARG(!d->has_residual, "pv_dwconv3d_fwd has no residual input");
+  PV_CHECK_ARG(!d->addend, "pv_dwconv3d_fwd has no addend input");
   int rc = pv::conv3d_check(d);
   if (rc != PV_OK) return rc;
   cudaStream_t s = (cudaStream_t)stream;

@@ -1,7 +1,7 @@
 // Fused epilogue shared by the implicit-GEMM kernels (TMA-fed, gather-fed, stem rows).
 //
 // Two consumer warpgroups (256 threads) hold a 128-row x BN tile of fp32 accumulators in wgmma fragments
-// (warpgroup g: rows [64 g, 64 g + 64)) -> y = act(acc*scale+bias (+residual)) -> f16 -> 128B-swizzled shared
+// (warpgroup g: rows [64 g, 64 g + 64)) -> y = act(acc*scale+bias (+residual)) (+ addend[n][t][c]) -> f16 -> 128B-swizzled shared
 // staging -> TMA tensor store.  The residual tile is brought in by a TMA tensor load into the SAME staging buffer
 // (requested before the tile's main loop, so its latency hides behind the MMAs) and updated in place, so both the
 // residual read and the output write are full-line bulk transfers issued by one thread, with the tile-edge and
@@ -23,7 +23,25 @@ struct EpiParams {
   CUtensorMap y_map;    // output  [Co, d1, d2, d3, d4], box [64, b1, b2, b3, b4], SWIZZLE_128B
   CUtensorMap r_map;    // residual, same geometry
   int block_n, Co, rows, act, has_residual;
+  // post-activation addend (pv_conv3d_desc.addend; nullptr = none): a[n * add_n + t * add_t + add_off + c]
+  const __half* addend;
+  long long add_n, add_t;
+  int add_off;
+  // y_map's outer dims d1..d4: extents, tile box and the flat output position (n, t, h, w) of one step along each;
+  // a staged row -> its output position -> (n, t) = (pos / hw / To, pos / hw % To)
+  int o_ext[4], o_box[4], o_pos[4];
+  int hw, To;        // a conv output has fewer than 2^31 positions (checked by every launch that takes an addend)
 };
+
+// Host: fill the addend fields from the descriptor (o_ext / o_box / o_pos are set by the launch, which knows its map).
+inline void epi_set_addend(EpiParams& E, const pv_conv3d_desc* d) {
+  E.addend = static_cast<const __half*>(d->addend);
+  E.add_n = d->add_n_stride;
+  E.add_t = d->add_t_stride;
+  E.add_off = d->add_ch_off;
+  E.hw = d->Ho * d->Wo;
+  E.To = d->To;
+}
 
 __device__ __forceinline__ void tma_store_5d(const void* tmap, uint32_t src, int c0, int c1, int c2, int c3,
                                              int c4) {
@@ -102,6 +120,45 @@ __device__ __forceinline__ void epi_math_res(bool res, const float (&d)[BN / 2],
   else epi_math<BN, ACT, false>(d, stg, scale, bias, Co, n0, ctid);
 }
 
+// Post-activation addend on the staged f16 tile: a second pass over the staging buffer once epi_math has written it,
+// one 16-byte cell (8 channels of one row) per step.  It runs after the fragment math, so the accumulator-holding code
+// and its register allocation are those of a launch without an addend.  Rows past the tensor edge (clipped by the TMA
+// store) and cells at or past Co are skipped.
+template <int BN>
+__device__ __forceinline__ void epi_addend(const EpiParams& E, uint8_t* stg, int ctid, int n0, int c1, int c2, int c3,
+                                           int c4) {
+  constexpr int CELLS = BN / 8;                 // a thread keeps one 8-channel column and walks rows
+  const int col = (ctid % CELLS) * 8;
+  if (n0 + col >= E.Co) return;
+  const __half* acol = E.addend + E.add_off + n0 + col;
+#pragma unroll 1
+  for (int row = ctid / CELLS; row < E.rows; row += EPI_THREADS / CELLS) {
+    unsigned r = row, pos = 0;
+    bool inside = true;
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+      const unsigned v = (unsigned)(m == 0 ? c1 : m == 1 ? c2 : m == 2 ? c3 : c4) + r % (unsigned)E.o_box[m];
+      r /= (unsigned)E.o_box[m];
+      inside &= v < (unsigned)E.o_ext[m];
+      pos += v * (unsigned)E.o_pos[m];
+    }
+    if (!inside) continue;
+    const unsigned nt = pos / (unsigned)E.hw;
+    const unsigned n = nt / (unsigned)E.To, t = nt - n * (unsigned)E.To;
+    const uint4 av = __ldg(reinterpret_cast<const uint4*>(acol + n * E.add_n + t * E.add_t));
+    uint4* cell = reinterpret_cast<uint4*>(stg + (col >> 6) * 16384 + row * 128 + ((((col & 63) >> 3) ^ (row & 7)) << 4));
+    uint4 sv = *cell;
+    __half2* s2 = reinterpret_cast<__half2*>(&sv);
+    const __half2* a2 = reinterpret_cast<const __half2*>(&av);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 f = __half22float2(s2[k]), g = __half22float2(a2[k]);
+      s2[k] = __floats2half2_rn(f.x + g.x, f.y + g.y);
+    }
+    *cell = sv;
+  }
+}
+
 // Called by the 256 consumer threads once the accumulators of the tile are complete (wgmma_wait<0>).
 // (c1..c4): tile origin in the store tensor map's outer dims; n0: first output channel of the tile.
 template <int BN>
@@ -120,6 +177,10 @@ __device__ __forceinline__ void epilogue_tile(const EpiParams& E, const float* _
     case PV_ACT_SWISH: epi_math_res<BN, PV_ACT_SWISH>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid); break;
     case PV_ACT_GELU: epi_math_res<BN, PV_ACT_GELU>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid); break;
     default: epi_math_res<BN, PV_ACT_SIGMOID>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid); break;
+  }
+  if (E.addend) {
+    epi_bar_sync(EPI_BAR_ID, EPI_THREADS);   // the cells of a row were written by other threads
+    epi_addend<BN>(E, staging_gen, ctid, n0, c1, c2, c3, c4);
   }
   // publish the staged tile to the async proxy and store it
   fence_proxy_async_smem();

@@ -344,6 +344,7 @@ int conv3d_tcgen05_supported(const pv_conv3d_desc* d, char* why, size_t why_len)
     return 0;                              \
   } while (0)
   if (d->dtype != PV_F16) NOPE("tcgen05 path needs f16 storage");
+  if (!conv3d_addend_ok(d)) NOPE("addend layout (16-byte pointer, Co and strides multiples of 8, < 2^31 positions)");
   const bool grouped = d->groups != 1;
   int span_g = 0, span_k = 0, span_n = 0;
   if (grouped) {
@@ -475,6 +476,7 @@ int conv3d_tcgen05_launch(const pv_conv3d_desc* d, const void* x, const void* w,
   P.epi.rows = P.rows;
   P.epi.act = d->act;
   P.epi.has_residual = d->has_residual;
+  epi_set_addend(P.epi, d);
   // k-blocks per pipeline stage: 64 K elements (the kernel's compile-time wgmma sequence, see conv3d_igemm_kernel)
   const int kb_bytes = (IG_BM + P.block_n) * P.kbytes;
   const size_t smem_fixed = 2048 /*align*/ + EPI_STAGING_BYTES + 16;
@@ -583,6 +585,11 @@ int conv3d_tcgen05_launch(const pv_conv3d_desc* d, const void* x, const void* w,
     for (int o = 0; o < 4; ++o) {
       const int m = pl.orig2m[o];
       if (!seen[m]) { seen[m] = true; ostr[m] = ostr_orig[o]; }
+    }
+    for (int m = 0; m < 4; ++m) {
+      P.epi.o_ext[m] = P.O[m];
+      P.epi.o_box[m] = P.box[m];
+      P.epi.o_pos[m] = seen[m] ? (int)ostr[m] : 0;
     }
     for (int pass = 0; pass < 2; ++pass) {
       if (pass == 1 && !d->has_residual) break;

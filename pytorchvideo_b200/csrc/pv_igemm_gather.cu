@@ -342,6 +342,12 @@ int conv3d_gather_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   P.epi.rows = GG_BM;
   P.epi.act = d->act;
   P.epi.has_residual = d->has_residual;
+  epi_set_addend(P.epi, d);
+  for (int m = 0; m < 4; ++m) {      // output as [Co, M, 1, 1, 1]: a row's position is its GEMM row
+    P.epi.o_ext[m] = m == 0 ? (int)P.M : 1;
+    P.epi.o_box[m] = m == 0 ? GG_BM : 1;
+    P.epi.o_pos[m] = m == 0 ? 1 : 0;
+  }
   const int stage_bytes = GG_A_BYTES + P.block_n * GG_BK * 2;
   {
     int st = (227 * 1024 - 2048 - 2048 /*static tables*/ - EPI_STAGING_BYTES - 512) / stage_bytes;

@@ -204,6 +204,14 @@ conv3d_direct_kernel(pv_conv3d_desc d, const T* __restrict__ x, const T* __restr
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) v[j] = apply_act(v[j], d.act);
+    if (d.addend) {     // post-activation addend of output sample n, frame t (constant over h, w)
+      const long long nt = m / ((long long)d.Ho * d.Wo);
+      const long long n = nt / d.To, t = nt - n * d.To;
+      float a[4];
+      ld4<T>(static_cast<const T*>(d.addend) + n * d.add_n_stride + t * d.add_t_stride + d.add_ch_off + co, a);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) v[j] += a[j];
+    }
     st4<T>(y + m * d.y_row_stride + co, v);
   }
 }
@@ -1016,6 +1024,8 @@ int conv3d_check(const pv_conv3d_desc* d) {
                "groups must divide Ci and Co; got groups=%d Ci=%d Co=%d", d->groups, d->Ci, d->Co);
   PV_CHECK_ARG(d->x_row_stride >= d->Ci && d->y_row_stride >= d->Co, "row stride < channels");
   PV_CHECK_ARG(!d->has_residual || d->res_row_stride >= d->Co, "residual row stride < Co");
+  PV_CHECK_ARG(conv3d_addend_ok(d), "addend: 16-byte aligned pointer and non-negative strides / channel offset that "
+               "are multiples of 8 elements required");
   return PV_OK;
 }
 
@@ -1042,6 +1052,10 @@ int conv3d_direct_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
       PV_LAUNCH_OK("conv3d_direct_kernel<float>");
     }
   } else {
+    if (d->addend) {
+      set_error("depthwise convolutions take no addend");
+      return PV_ERR_UNSUPPORTED;
+    }
     if (d->groups != d->Ci || d->Ci != d->Co) {
       set_error("PV_ALGO_DIRECT runs dense (groups=1) and depthwise (groups==Ci==Co) convolutions only; got groups=%d "
                 "Ci=%d Co=%d", d->groups, d->Ci, d->Co);

@@ -195,6 +195,7 @@ extern "C" int pv_conv3d_stem_rows_supported(const pv_conv3d_desc* d) {
   if (run > 64 || d->ci_pad64 != win) return 0;
   if (d->Co % 8 || d->Co > MAX_BN || d->y_row_stride % 8) return 0;
   if (d->kt * d->kh > ST_MAX_ROWS) return 0;
+  if (!conv3d_addend_ok(d)) return 0;
   const long long base_off = (long long)(d->x_w_pad - d->pw - lead) * 8;
   if (base_off < 0 || base_off % 16) return 0;
   // every window of the last output pixel must lie inside the physical row
@@ -246,6 +247,12 @@ extern "C" int pv_conv3d_stem_rows_fwd(const pv_conv3d_desc* d, const void* x, c
   const long long ostr[4] = {1, d->Wo, (long long)d->Wo * d->Ho, (long long)d->Wo * d->Ho * d->To};
   const int O[4] = {d->Wo, d->Ho, d->To, d->N};
   const int box[4] = {P.epi.rows, 1, 1, 1};
+  epi_set_addend(P.epi, d);
+  for (int m = 0; m < 4; ++m) {
+    P.epi.o_ext[m] = O[m];
+    P.epi.o_box[m] = box[m];
+    P.epi.o_pos[m] = (int)ostr[m];
+  }
   {
     cuuint64_t gdim[5] = {(cuuint64_t)d->Co, (cuuint64_t)O[0], (cuuint64_t)O[1], (cuuint64_t)O[2], (cuuint64_t)O[3]};
     cuuint64_t gstr[4];

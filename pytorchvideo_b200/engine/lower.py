@@ -9,6 +9,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib as L
+from . import packing as PK
 from .plan import Plan, TRef
 
 
@@ -36,6 +37,45 @@ def _act_code(m):
     raise NotImplementedError("activation %s has no B200 kernel" % n)
 
 
+def _union_taps(convs, name):
+    """Common tap box of parallel convolutions of one input (ConvReduce3D(sum) stems, the separable conv_b):
+    (kernel, stride, padding, dilation, places) with places[i] the index slices of branch i inside the box.  Along
+    each axis the branches with more than one tap must agree on (k, p, d); a one-tap branch sits at the box tap that
+    reads the same input offset.  Anything else has no common box."""
+    strides = {_t3(c.stride) for c in convs}
+    if len(strides) != 1:
+        raise NotImplementedError("%s: parallel convolutions with different strides %s" % (name, sorted(strides)))
+    geo = [(_t3(c.kernel_size), _t3(c.padding), _t3(c.dilation)) for c in convs]
+    kernel, padding, dilation = [], [], []
+    for ax in range(3):
+        multi = {(k[ax], p[ax], d[ax]) for k, p, d in geo if k[ax] > 1}
+        if len(multi) > 1:
+            raise NotImplementedError("%s: parallel convolutions with different taps along axis %d" % (name, ax))
+        if multi:
+            k, p, d = multi.pop()
+        else:
+            pads = {p[ax] for _, p, _ in geo}
+            if len(pads) != 1:
+                raise NotImplementedError("%s: one-tap branches with different paddings along axis %d" % (name, ax))
+            k, p, d = 1, pads.pop(), 1
+        kernel.append(k)
+        padding.append(p)
+        dilation.append(d)
+    places = []
+    for kb, pb, _ in geo:
+        sl = []
+        for ax in range(3):
+            if kb[ax] > 1:
+                sl.append(slice(0, kernel[ax]))
+                continue
+            j, r = divmod(padding[ax] - pb[ax], dilation[ax])     # box tap j reads input offset j * d - p = -pb
+            if r or not 0 <= j < kernel[ax]:
+                raise NotImplementedError("%s: branch padding is not centre-consistent along axis %d" % (name, ax))
+            sl.append(slice(j, j + 1))
+        places.append(tuple(sl))
+    return tuple(kernel), strides.pop(), tuple(padding), tuple(dilation), places
+
+
 def _is_bn(m):
     return isinstance(m, nn.modules.batchnorm._BatchNorm) or type(m).__name__.startswith("NaiveSyncBatchNorm")
 
@@ -47,8 +87,10 @@ class Lowering:
         self.aux_out = None           # host-side second result of the root module (pooled thw)
 
     # ---- leaf helpers --------------------------------------------------------------------
-    def conv(self, x: TRef, conv: nn.Conv3d, bn=None, act=None, residual=None, name="conv", se_sums=False):
+    def conv(self, x: TRef, conv: nn.Conv3d, bn=None, act=None, residual=None, name="conv", se_sums=False, addend=None):
         if type(conv).__name__ == "Conv2plus1d":
+            if addend is not None:
+                raise NotImplementedError("%s: Conv2plus1d takes no addend" % name)
             return self.conv2plus1d(x, conv, bn, act, residual, name)
         if not isinstance(conv, nn.Conv3d):
             raise NotImplementedError("%s: conv module %s unsupported" % (name, type(conv).__name__))
@@ -59,7 +101,8 @@ class Lowering:
         if bn is not None and not _is_bn(bn):
             raise NotImplementedError("%s: norm %s unsupported (BatchNorm only)" % (name, type(bn).__name__))
         return self.p.emit_conv(x, conv.weight, conv.bias, bn, _t3(conv.stride), _t3(conv.padding),
-                                _t3(conv.dilation), conv.groups, _act_code(act), residual, name, se_sums=se_sums)
+                                _t3(conv.dilation), conv.groups, _act_code(act), residual, name, se_sums=se_sums,
+                                addend=addend)
 
     def conv2plus1d(self, x, m, bn, act, residual, name):
         # layers/convolutions.py:232-237: conv_t -> norm -> activation -> conv_xy, or conv_xy first when
@@ -164,16 +207,57 @@ class Lowering:
             x = self.lower(blk, x, "%s.%d" % (name, i))
         return x
 
-    def lower_ResNetBasicStem(self, m, x, name):
+    def lower_ResNetBasicStem(self, m, x, name, addend=None):
         # models/stem.py:252-260: conv -> norm -> activation -> pool
-        x = self.conv(x, m.conv, m.norm, m.activation, None, name + ".conv")
-        if getattr(m, "pool", None) is not None:
-            x = self.pool(x, m.pool, name + ".pool")
+        pool = getattr(m, "pool", None)
+        if addend is not None and pool is not None:
+            # the addend is constant over (h, w) and max pooling pads with -inf, so maxpool(y) + a == maxpool(y + a)
+            # for a pool that does not mix frames: the add moves into the conv's epilogue
+            if type(pool).__name__ != "MaxPool3d" or _t3(pool.kernel_size)[0] != 1 or \
+                    _t3(pool.stride if pool.stride is not None else pool.kernel_size)[0] != 1 or _t3(pool.padding)[0] != 0:
+                raise NotImplementedError("%s: an audio fusion after the stem needs a spatial-only MaxPool3d" % name)
+        if type(m.conv).__name__ == "ConvReduce3D":
+            x = self.conv_reduce_sum(x, m.conv, m.norm, m.activation, name + ".conv", addend)
+        else:
+            x = self.conv(x, m.conv, m.norm, m.activation, None, name + ".conv", addend=addend)
+        if pool is not None:
+            x = self.pool(x, pool, name + ".pool")
         return x
 
-    def lower_ResStage(self, m, x, name):
+    def conv_reduce_sum(self, x, m, bn, act, name, addend=None):
+        """The acoustic stem's ConvReduce3D (stem.py:179-192): a (kt,1,1) and a (1,kh,kw) convolution of one input,
+        summed, as ONE convolution whose kernel is the sum of both embedded in their common (kt,kh,kw) box (exact;
+        the network input can also feed only one window-mode stem convolution)."""
+        if m.reduction_method != "sum":
+            raise NotImplementedError("%s: ConvReduce3D(cat) in a stem is unsupported" % name)
+        convs = list(m.convs)
+        for c in convs:
+            if type(c) is not nn.Conv3d or isinstance(c.padding, str) or c.padding_mode != "zeros":
+                raise NotImplementedError("%s: ConvReduce3D branches must be zero-padded Conv3d" % name)
+        if len({c.groups for c in convs}) != 1:
+            raise NotImplementedError("%s: ConvReduce3D branches with different groups" % name)
+        kernel, stride, padding, dilation, places = _union_taps(convs, name)
+        c0 = convs[0]
+        w = torch.zeros((c0.out_channels, c0.in_channels // c0.groups) + kernel, dtype=torch.float64)
+        for c, sl in zip(convs, places):
+            w[(slice(None), slice(None)) + sl] += c.weight.detach().double().cpu()
+        biases = [c.bias for c in convs if c.bias is not None]
+        bias = sum(b.detach().double().cpu() for b in biases).float() if biases else None
+        if bn is not None and not _is_bn(bn):
+            raise NotImplementedError("%s: norm %s unsupported (BatchNorm only)" % (name, type(bn).__name__))
+        return self.p.emit_conv(x, w.float(), bias, bn, stride, padding, dilation, c0.groups, _act_code(act), None,
+                                name, addend=addend)
+
+    def lower_ResStage(self, m, x, name, addend=None):
+        n = len(m.res_blocks)
         for i, blk in enumerate(m.res_blocks):
-            x = self.lower(blk, x, "%s.res_blocks.%d" % (name, i))
+            bname = "%s.res_blocks.%d" % (name, i)
+            if addend is not None and i == n - 1:
+                if type(blk).__name__ != "ResBlock":
+                    raise NotImplementedError("%s: an audio fusion needs a ResBlock at the end of the stage" % bname)
+                x = self.lower_ResBlock(blk, x, bname, addend)
+            else:
+                x = self.lower(blk, x, bname)
         return x
 
     def _fusable_bottleneck(self, m, x):
@@ -222,9 +306,10 @@ class Lowering:
                                     m.branch1_conv is not None, act)
         return bool(p.lib.pv_bottleneck_fused_supported(C_.byref(d)))
 
-    def lower_ResBlock(self, m, x, name):
-        # models/resnet.py:1179-1189; branch_fusion is x + y for every builder in scope.
-        if self._fusable_bottleneck(m, x):
+    def lower_ResBlock(self, m, x, name, addend=None):
+        # models/resnet.py:1179-1189; branch_fusion is x + y for every builder in scope.  The fused narrow-block
+        # kernel has no addend: a block that takes one runs as separate convolutions.
+        if addend is None and self._fusable_bottleneck(m, x):
             b = m.branch2
             act = L.ACT_RELU if (m.activation is not None and type(m.activation).__name__ == "ReLU") else L.ACT_NONE
             return self.p.emit_bottleneck_fused(x, b.conv_a, b.norm_a, b.conv_b, b.norm_b, b.conv_c, b.norm_c,
@@ -233,13 +318,17 @@ class Lowering:
             shortcut = self.conv(x, m.branch1_conv, getattr(m, "branch1_norm", None), None, None, name + ".branch1")
         else:
             shortcut = x
-        return self.bottleneck(m.branch2, x, shortcut, m.activation, name + ".branch2")
+        return self.bottleneck(m.branch2, x, shortcut, m.activation, name + ".branch2", addend)
 
     def lower_BottleneckBlock(self, m, x, name):
         return self.bottleneck(m, x, None, None, name)
 
-    def bottleneck(self, m, x, shortcut, final_act, name):
+    lower_SeparableBottleneckBlock = lower_BottleneckBlock
+
+    def bottleneck(self, m, x, shortcut, final_act, name, addend=None):
         # models/resnet.py:1345-1365 with the block's residual add + activation fused into conv_c
+        if type(m).__name__ == "SeparableBottleneckBlock":
+            return self.separable_bottleneck(m, x, shortcut, final_act, name, addend)
         if type(m).__name__ != "BottleneckBlock":
             raise NotImplementedError("branch2 module %s unsupported" % type(m).__name__)
         h = self.conv(x, m.conv_a, m.norm_a, m.act_a, None, name + ".conv_a")
@@ -259,7 +348,52 @@ class Lowering:
                 raise NotImplementedError("SqueezeExcitation variant unsupported")
             h = self.p.emit_se_scale_act(h, blk[0].weight, blk[0].bias, blk[2].weight, blk[2].bias,
                                          _act_code(m.act_b), name + ".se")
-        return self.conv(h, m.conv_c, m.norm_c, final_act, shortcut, name + ".conv_c")
+        return self.conv(h, m.conv_c, m.norm_c, final_act, shortcut, name + ".conv_c", addend=addend)
+
+    def separable_bottleneck(self, m, x, shortcut, final_act, name, addend=None):
+        """SeparableBottleneckBlock (models/resnet.py:1257-1285).  Both conv_b branches run as ONE convolution over
+        the union of their taps (zero where a branch has none), output channels [branch 0 | branch 1], each with its
+        own folded norm; "cat" is that output, "sum" feeds conv_c with its weight repeated along C_in,
+        conv_c(a + b) = [W_c | W_c] . [a ; b], so the sum is never materialised."""
+        h = x
+        if m.conv_a is not None:
+            h = self.conv(x, m.conv_a, m.norm_a, m.act_a, None, name + ".conv_a")
+        convs, norms, acts = list(m.conv_b), list(m.norm_b), list(m.act_b)
+        for c in convs:
+            if type(c) is not nn.Conv3d or isinstance(c.padding, str) or c.padding_mode != "zeros":
+                raise NotImplementedError("%s.conv_b: branches must be zero-padded Conv3d" % name)
+            if c.in_channels != h.C:
+                raise RuntimeError("conv %s.conv_b expects %d input channels, got %d" % (name, c.in_channels, h.C))
+        for n_ in norms:
+            if n_ is not None and not _is_bn(n_):
+                raise NotImplementedError("%s.norm_b: norm %s unsupported (BatchNorm only)" % (name, type(n_).__name__))
+        act_names = {None if a is None else type(a).__name__ for a in acts}
+        if len(act_names) != 1:
+            raise NotImplementedError("%s.act_b: branches with different activations %s" % (name, sorted(map(str, act_names))))
+        kernel, stride, padding, dilation, places = _union_taps(convs, name + ".conv_b")
+        dense = [PK.expand_grouped_dense(c.weight, c.groups) if c.groups != 1 else c.weight.detach().cpu() for c in convs]
+        rows = [c.out_channels for c in convs]
+        w = torch.zeros((sum(rows), h.C) + kernel, dtype=dense[0].dtype)
+        o = 0
+        for wd, r, sl in zip(dense, rows, places):
+            w[(slice(o, o + r), slice(None)) + sl] = wd
+            o += r
+        folded = [PK.fold_bn(c.bias, n_, c.out_channels, c.out_channels) for c, n_ in zip(convs, norms)]
+        folded = (torch.cat([f[0] for f in folded]), torch.cat([f[1] for f in folded]))
+        h = self.p.emit_conv(h, w, None, None, stride, padding, dilation, 1, _act_code(acts[0]), None,
+                             name + ".conv_b", folded=folded)
+        cc = m.conv_c
+        if m.reduce_method == "sum":
+            if len(set(rows)) != 1:
+                raise RuntimeError("%s: summed conv_b branches need equal widths, got %s" % (name, rows))
+            if type(cc) is not nn.Conv3d or cc.groups != 1:
+                raise NotImplementedError("%s.conv_c: Conv3d with groups 1 expected" % name)
+            if cc.in_channels != rows[0]:
+                raise RuntimeError("conv %s.conv_c expects %d input channels, got %d" % (name, cc.in_channels, rows[0]))
+            wc = torch.cat([cc.weight.detach().cpu()] * len(rows), 1)
+            return self.p.emit_conv(h, wc, cc.bias, m.norm_c, _t3(cc.stride), _t3(cc.padding), _t3(cc.dilation), 1,
+                                    _act_code(final_act), shortcut, name + ".conv_c", addend=addend)
+        return self.conv(h, cc, m.norm_c, final_act, shortcut, name + ".conv_c", addend=addend)
 
     # head widths of the Non-local attention core (csrc/pv_attention.cu routing): softmax also runs on the MViT
     # kernels' 32 / 96, the linear ("dot_product") mode only on the widths of csrc/pv_attention_wide.cu
@@ -316,6 +450,8 @@ class Lowering:
     def lower_MultiPathWayWithFuse(self, m, x, name):
         # models/net.py:107-122
         assert isinstance(x, list), "input for MultiPathWayWithFuse needs to be a list of tensors"
+        if type(m.multipathway_fusion).__name__ == "FuseAudioToFastSlow":
+            return self.audio_fused_stage(m, x, name)
         out = list(x)
         # the pathways are independent until the fusion: each gets its own lane (CUDA stream / graph branch)
         for i, blk in enumerate(m.multipathway_blocks):
@@ -334,6 +470,70 @@ class Lowering:
         fuse = self.conv(x_f, m.conv_fast_to_slow, m.norm, m.activation, None, name + ".conv_fast_to_slow")
         self.p.lane = 0        # waits for it where the next Slow stage reads the concat buffer
         return [self.p.concat_channels([x_s, fuse]), x_f]
+
+    def audio_fused_stage(self, m, x, name):
+        """One AVSlowFast stage: the pathways, then FuseAudioToFastSlow (models/audio_visual_slowfast.py:406-418),
+        [fuse_a + cat(x_s, conv_f2s(x_f)), x_f, x_a].  Both writers of the concat buffer - the Slow pathway's last
+        convolution and the Fast->Slow convolution - add fuse_a in their epilogues, so neither the concat nor the add
+        is a pass of its own.  Emission order: the audio pathway and the fuse_a chain (lane 2) come first, so every
+        op that takes fuse_a is emitted after its writer and waits for it across lanes (Plan._schedule)."""
+        if len(x) != 3:
+            raise RuntimeError("FuseAudioToFastSlow takes [slow, fast, audio] pathways, got %d" % len(x))
+        p = self.p
+        blocks, fusion = m.multipathway_blocks, m.multipathway_fusion
+        bname = "%s.multipathway_blocks.%%d" % name
+        fname = name + ".multipathway_fusion"
+        out = list(x)
+        p.lane = 2
+        if blocks[2] is not None:
+            out[2] = self.lower(blocks[2], x[2], bname % 2)
+        xa = out[2]
+        a = p.emit_pool(xa, L.POOL_AVG, (1, 1, xa.W), (1, 1, xa.W), (0, 0, 0), fname + ".mean")   # mean over F
+        a = self.conv_chain(fusion.block_audio_to_fastslow, a, fname + ".block_audio_to_fastslow")
+        p.lane = 0
+        slow = blocks[0]
+        sn = type(slow).__name__
+        if sn == "ResStage":
+            out[0] = self.lower_ResStage(slow, x[0], bname % 0, addend=(a, 0))
+        elif sn == "ResNetBasicStem":
+            out[0] = self.lower_ResNetBasicStem(slow, x[0], bname % 0, addend=(a, 0))
+        else:
+            raise NotImplementedError("%s: Slow pathway block %s cannot take the audio fusion" % (name, sn))
+        p.lane = 1
+        if blocks[1] is not None:
+            out[1] = self.lower(blocks[1], x[1], bname % 1)
+        x_s = out[0]
+        f2s = list(fusion.block_fast_to_slow)
+        c_fuse = f2s[0].out_channels if f2s and isinstance(f2s[0], nn.Conv3d) else 0
+        if a.C != x_s.C + c_fuse:
+            raise RuntimeError("%s: audio fusion has %d channels, the Slow concat %d" % (fname, a.C, x_s.C + c_fuse))
+        if x_s.C != x_s.Cp:
+            raise NotImplementedError("%s: Slow pathway width %d is not a multiple of 8" % (fname, x_s.C))
+        fuse = self.conv_chain(fusion.block_fast_to_slow, out[1], fname + ".block_fast_to_slow", addend=(a, x_s.Cp))
+        p.lane = 0
+        return [p.concat_channels([x_s, fuse]), out[1], out[2]]
+
+    def conv_chain(self, seq, x, name, addend=None):
+        """nn.Sequential of Conv3d [+ BatchNorm] [+ activation] groups (the FuseAudioToFastSlow blocks); the addend
+        goes to the last convolution."""
+        mods = list(seq)
+        groups, i = [], 0
+        while i < len(mods):
+            c = mods[i]
+            if not isinstance(c, nn.Conv3d):
+                raise NotImplementedError("%s.%d: %s unsupported here (Conv3d expected)" % (name, i, type(c).__name__))
+            j, bn, act = i + 1, None, None
+            if j < len(mods) and _is_bn(mods[j]):
+                bn, j = mods[j], j + 1
+            if j < len(mods) and not isinstance(mods[j], nn.Conv3d) and not _is_bn(mods[j]):
+                act, j = mods[j], j + 1
+            groups.append((i, c, bn, act))
+            i = j
+        if not groups:
+            raise NotImplementedError("%s: empty convolution chain" % name)
+        for g, (i, c, bn, act) in enumerate(groups):
+            x = self.conv(x, c, bn, act, None, "%s.%d" % (name, i), addend=addend if g == len(groups) - 1 else None)
+        return x
 
     def lower_PoolConcatPathway(self, m, x, name):
         # models/slowfast.py:608-620

@@ -295,10 +295,13 @@ class Plan:
         return x
 
     def emit_conv(self, x, weight, conv_bias, bn, stride, padding, dilation, groups, act=L.ACT_NONE,
-                  residual=None, name="conv", force_algo=None, se_sums=False):
-        """Conv3d (+folded BN/bias) (+residual) (+activation).  weight: [Co, Ci/g, kt, kh, kw].
+                  residual=None, name="conv", force_algo=None, se_sums=False, addend=None, folded=None):
+        """Conv3d (+folded BN/bias) (+residual) (+activation) (+addend).  weight: [Co, Ci/g, kt, kh, kw].
         se_sums (depthwise only): also accumulate the per-(sample, channel) sums of the output inside
-        the conv kernel (Squeeze-Excitation statistics); the buffer is attached as ``y.se_sums``."""
+        the conv kernel (Squeeze-Excitation statistics); the buffer is attached as ``y.se_sums``.
+        addend: (a, c_off) - a (N, T' in {To, 1}, 1, 1, C) tensor added after the activation, output channel c taking
+        a's channel c_off + c (pv_conv3d_desc.addend).  folded: precomputed (scale, bias) of length Co instead of
+        conv_bias / bn."""
         co, cig, kt, kh, kw = weight.shape
         ci = cig * groups
         if ci != x.C:
@@ -311,7 +314,18 @@ class Plan:
         if min(To, Ho, Wo) <= 0:
             raise RuntimeError("conv %s: kernel larger than (padded) input" % name)
         co_pad = PK.pad8(co)
+        if addend is not None:
+            a, a_off = addend
+            # torch broadcasting of a (N, C, T', 1, 1) tensor against the (N, C, To, Ho, Wo) output
+            if a.N != x.N or a.H != 1 or a.W != 1 or a.T not in (To, 1):
+                raise RuntimeError("conv %s: addend of shape %s does not broadcast to the output %s" % (
+                    name, a.shape5(), (x.N, co, To, Ho, Wo)))
+            if a_off + co_pad > a.Cp:
+                raise RuntimeError("conv %s: addend has %d channels, the output needs %d from channel %d" % (
+                    name, a.C, co, a_off))
         depthwise = groups != 1 and groups == ci == co
+        if depthwise and addend is not None:
+            raise NotImplementedError("conv %s: depthwise convolutions take no addend" % name)
         span = None
         if groups != 1 and not depthwise:
             # grouped conv (ResNeXt-style group counts, CSN with several channels per group): the grouped mode of the
@@ -320,17 +334,21 @@ class Plan:
             if self.use_tcgen05 and force_algo in (None, L.ALGO_TCGEN05) and x.Cp == ci and co_pad == co:
                 probe = self._conv_desc(x, (To, Ho, Wo), co_pad, (kt, kh, kw), stride, padding, dilation, groups, act,
                                         residual, co_pad, 0)
+                if addend is not None:
+                    probe.addend, probe.add_n_stride = 256, a.T * a.row_stride      # layout probe, see below
+                    probe.add_t_stride, probe.add_ch_off = (a.row_stride if a.T == To > 1 else 0), a_off
                 taken, span_g, span_k, _ = L.group_span(probe)
                 span = (span_g, span_k) if taken else None
             if span is None:
                 return self.emit_conv(x, PK.expand_grouped_dense(weight, groups), conv_bias, bn, stride, padding,
-                                      dilation, 1, act, residual, name, force_algo=force_algo, se_sums=se_sums)
+                                      dilation, 1, act, residual, name, force_algo=force_algo, se_sums=se_sums,
+                                      addend=addend, folded=folded)
         if residual is not None:
             self.materialize_input(residual)
         # ---- narrow stems with a temporal extent: factor (kt,kh,kw) -> (1,kh,kw) with kt*Co channels
         #      (all temporal taps in one tensor-core pass) + a temporal tap sum, see pv_temporal_tap_sum
         if (x.lazy_src is not None and self.use_tcgen05 and force_algo in (None, L.ALGO_TCGEN05) and groups == 1
-                and x.Cp == 4 and kt > 1 and residual is None and co_pad * kt <= 256 and dlw == 1
+                and x.Cp == 4 and kt > 1 and residual is None and addend is None and co_pad * kt <= 256 and dlw == 1
                 and (sw * x.Cp * 2) % 16 == 0 and kw * x.Cp <= 64 and pw > 0 and sh <= 8):
             w2 = torch.zeros(kt * co_pad, cig, 1, kh, kw, dtype=weight.dtype)
             wsrc = weight.detach().cpu()
@@ -368,7 +386,10 @@ class Plan:
         elif x.padw is not None:
             raise RuntimeError("W-padded stem input can only feed one window-mode convolution")
         y = self.new_tensor(x.N, To, Ho, Wo, co, Cp=co_pad)
-        scale, bias = PK.fold_bn(conv_bias, bn, co, co_pad)
+        if folded is None:
+            scale, bias = PK.fold_bn(conv_bias, bn, co, co_pad)
+        else:
+            scale, bias = (torch.cat([t.float(), torch.zeros(co_pad - co)]) for t in folded)
         scale_d, bias_d = self.const(scale), self.const(bias)
         tdt = _TORCH_DT[self.dt]
         ci_pad = x.Cp
@@ -379,6 +400,19 @@ class Plan:
         d = self._conv_desc(x, (To, Ho, Wo), co_pad, (kt, kh, kw), stride, padding, dilation,
                             ci_pad if depthwise else (groups if span is not None else 1), act, residual, y.row_stride,
                             ci_pad64)
+        if addend is not None:
+            d.add_n_stride = a.T * a.row_stride
+            d.add_t_stride = a.row_stride if a.T == To > 1 else 0
+            d.add_ch_off = a_off
+            # the buffer is allocated at finalize(): until then an aligned placeholder, so that the routing probes
+            # below check the addend's layout rules as the launch will (a.ptr() is 16-byte aligned: own buffer)
+            d.addend = 256
+
+            def set_addend():
+                d.addend = a.ptr()
+        else:
+            def set_addend():
+                pass
         if window:
             d.x_w_pad, d.x_w_phys = x.padw
             w_lead = PK.window_lead(x.padw[0], pw, x.Cp)
@@ -430,12 +464,14 @@ class Plan:
 
         def fn_stem(stream):
             d.x_row_stride, d.y_row_stride = x.row_stride, y.row_stride
+            set_addend()
             L.check(lib.pv_conv3d_stem_rows_fwd(C.byref(d), x.ptr(), w_d.data_ptr(), scale_d.data_ptr(), bias_d.data_ptr(),
                                                 zero_row.data_ptr(), y.ptr(), stream), "pv_conv3d_stem_rows_fwd(%s)" % name)
 
         def fn(stream):
             d.x_row_stride, d.y_row_stride = x.row_stride, y.row_stride   # may have been retargeted
             d.res_row_stride = residual.row_stride if residual is not None else 0
+            set_addend()
             L.check(lib.pv_conv3d_fwd(C.byref(d), algo, x.ptr(), w_d.data_ptr(), scale_d.data_ptr(),
                                       bias_d.data_ptr(), residual.ptr() if residual is not None else None,
                                       y.ptr(), stream), "pv_conv3d_fwd(%s)" % name)
@@ -446,7 +482,10 @@ class Plan:
         if stem_rows:
             self.stats["stem_rows"] = self.stats.get("stem_rows", 0) + 1
         self.add(name, fn_stem if stem_rows else (fn_dw if (depthwise and residual is None) else fn), kind, flops, nbytes,
-                 reads=(x,) + ((residual,) if residual is not None else ()), writes=(y,) + ((sums,) if sums is not None else ()))
+                 reads=(x,) + ((residual,) if residual is not None else ()) + ((a,) if addend is not None else ()),
+                 writes=(y,) + ((sums,) if sums is not None else ()))
+        if addend is not None:
+            self.meta[-1]["addend"] = (a.buf, a_off)
         return y
 
     def _conv_desc(self, x, out_thw, co_pad, kernel, stride, padding, dilation, groups, act, residual, y_row_stride,

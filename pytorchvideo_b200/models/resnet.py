@@ -11,7 +11,7 @@ from ..layers.utils import set_attributes
 from ..module import B200Module
 from .head import create_res_basic_head
 from .net import Net
-from .stem import create_res_basic_stem
+from .stem import create_acoustic_res_basic_stem, create_res_basic_stem
 
 _MODEL_STAGE_DEPTH = {50: (3, 4, 6, 3), 101: (3, 4, 23, 3), 152: (3, 8, 36, 3)}
 
@@ -24,6 +24,20 @@ class BottleneckBlock(B200Module):
         super().__init__()
         set_attributes(self, locals())
         assert all(op is not None for op in (self.conv_a, self.conv_b, self.conv_c))
+        if self.norm_c is not None:
+            self.norm_c.block_final_bn = True   # read by init_net_weights
+
+
+class SeparableBottleneckBlock(B200Module):
+    """conv_a/norm_a/act_a -> parallel conv_b[i]/norm_b[i]/act_b[i] reduced by "sum" or "cat" -> conv_c/norm_c
+    (resnet.py:1192-1285).  On device both conv_b branches run as one convolution over their union of taps."""
+
+    def __init__(self, *, conv_a, norm_a, act_a, conv_b, norm_b, act_b, conv_c, norm_c, reduce_method="sum"):
+        super().__init__()
+        set_attributes(self, locals())
+        assert all(op is not None for op in (self.conv_b, self.conv_c)), (
+            f"{self.conv_a}, {self.conv_b}, {self.conv_c} has None")
+        assert reduce_method in ["sum", "cat"]
         if self.norm_c is not None:
             self.norm_c.block_final_bn = True   # read by init_net_weights
 
@@ -64,6 +78,39 @@ def create_bottleneck_block(*, dim_in, dim_inner, dim_out, conv_a_kernel_size=(3
                       dilation=conv_b_dilation),
         norm_b=_norm(norm, dim_inner, norm_eps, norm_momentum),
         act_b=act(),
+        conv_c=conv_c(in_channels=dim_inner, out_channels=dim_out, kernel_size=(1, 1, 1), bias=False),
+        norm_c=_norm(norm, dim_out, norm_eps, norm_momentum),
+    )
+
+
+def create_acoustic_bottleneck_block(*, dim_in, dim_inner, dim_out, conv_a_kernel_size=(3, 1, 1),
+                                     conv_a_stride=(2, 1, 1), conv_a_padding=(1, 0, 0), conv_a=nn.Conv3d,
+                                     conv_b_kernel_size=(1, 1, 1), conv_b_stride=(1, 1, 1), conv_b_padding=(0, 0, 0),
+                                     conv_b_num_groups=1, conv_b_dilation=(1, 1, 1), conv_b=nn.Conv3d,
+                                     conv_c=nn.Conv3d, norm=nn.BatchNorm3d, norm_eps=1e-5, norm_momentum=0.1,
+                                     activation=nn.ReLU):
+    """Bottleneck whose conv_b is a (kt,1,1) temporal and a (1,kh,kw) spatial convolution in parallel, summed
+    (resnet.py:151-316).  ``conv_b`` / ``norm_b`` / ``act_b`` hold the spatial branch first, the temporal second."""
+    act = (lambda: None) if activation is None else activation
+    branch_t = dict(kernel_size=[conv_b_kernel_size[0], 1, 1], padding=[conv_b_padding[0], 0, 0],
+                    dilation=[conv_b_dilation[0], 1, 1])
+    branch_s = dict(kernel_size=[1, conv_b_kernel_size[1], conv_b_kernel_size[2]],
+                    padding=[0, conv_b_padding[1], conv_b_padding[2]],
+                    dilation=[1, conv_b_dilation[1], conv_b_dilation[2]])
+    conv_b_1, conv_b_2 = (conv_b(in_channels=dim_inner, out_channels=dim_inner, stride=conv_b_stride, bias=False,
+                                 groups=conv_b_num_groups, **kw) for kw in (branch_t, branch_s))
+    norm_b_1 = _norm(norm, dim_inner, norm_eps, norm_momentum)
+    act_b_1 = act()
+    norm_b_2 = _norm(norm, dim_inner, norm_eps, norm_momentum)
+    act_b_2 = act()
+    return SeparableBottleneckBlock(
+        conv_a=conv_a(in_channels=dim_in, out_channels=dim_inner, kernel_size=conv_a_kernel_size,
+                      stride=conv_a_stride, padding=conv_a_padding, bias=False),
+        norm_a=_norm(norm, dim_inner, norm_eps, norm_momentum),
+        act_a=act(),
+        conv_b=nn.ModuleList([conv_b_2, conv_b_1]),
+        norm_b=nn.ModuleList([norm_b_2, norm_b_1]),
+        act_b=nn.ModuleList([act_b_2, act_b_1]),
         conv_c=conv_c(in_channels=dim_inner, out_channels=dim_out, kernel_size=(1, 1, 1), bias=False),
         norm_c=_norm(norm, dim_out, norm_eps, norm_momentum),
     )
@@ -186,6 +233,22 @@ def create_resnet(*, input_channel=3, model_depth=50, model_num_class=400, dropo
                            dropout_rate=dropout_rate, activation=head_activation,
                            output_with_global_average=head_output_with_global_average))
     return Net(blocks=nn.ModuleList(blocks))
+
+
+def create_acoustic_resnet(*, input_channel=1, model_depth=50, model_num_class=400, dropout_rate=0.5,
+                           norm=nn.BatchNorm3d, activation=nn.ReLU, stem_dim_out=64, stem_conv_kernel_size=(9, 1, 9),
+                           stem_conv_stride=(1, 1, 3), stem_pool=None, stem_pool_kernel_size=(3, 1, 3),
+                           stem_pool_stride=(2, 1, 2), stem=create_acoustic_res_basic_stem, stage1_pool=None,
+                           stage1_pool_kernel_size=(2, 1, 1), stage_conv_a_kernel_size=(3, 1, 1),
+                           stage_conv_b_kernel_size=(3, 1, 3), stage_conv_b_num_groups=(1, 1, 1, 1),
+                           stage_conv_b_dilation=(1, 1, 1), stage_spatial_h_stride=(1, 1, 1, 1),
+                           stage_spatial_w_stride=(1, 2, 2, 2), stage_temporal_stride=(1, 2, 2, 2),
+                           bottleneck=(create_acoustic_bottleneck_block, create_acoustic_bottleneck_block,
+                                       create_bottleneck_block, create_bottleneck_block),
+                           head_pool=nn.AvgPool3d, head_pool_kernel_size=(4, 1, 2),
+                           head_output_size=(1, 1, 1), head_activation=None, head_output_with_global_average=True):
+    """ResNet over a log-mel spectrogram (B, C, T, 1, F) (reference resnet.py:1022-1134)."""
+    return create_resnet(**locals())
 
 
 def create_resnet_with_roi_head(*, input_channel=3, model_depth=50, model_num_class=80, dropout_rate=0.5,

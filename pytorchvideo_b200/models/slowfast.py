@@ -53,6 +53,8 @@ class FastToSlowFusionBuilder:
 
 
 _BB = create_bottleneck_block
+# slowfast.py:14-19: SlowFast also builds at depth 18 (create_resnet does not)
+_SLOWFAST_STAGE_DEPTH = {18: (1, 1, 1, 1), **_MODEL_STAGE_DEPTH}
 
 
 def create_slowfast(*, slowfast_channel_reduction_ratio=(8,), slowfast_conv_channel_fusion_ratio=2,
@@ -76,8 +78,8 @@ def create_slowfast(*, slowfast_channel_reduction_ratio=(8,), slowfast_conv_chan
     """SlowFast network builder (reference slowfast.py:22-361); input is ``[slow_clip, fast_clip]``."""
     torch._C._log_api_usage_once("PYTORCHVIDEO.model.create_slowfast")
     n_path = len(input_channels)
-    assert model_depth in _MODEL_STAGE_DEPTH, f"{model_depth} is not in {_MODEL_STAGE_DEPTH.keys()}"
-    depths = _MODEL_STAGE_DEPTH[model_depth]
+    assert model_depth in _SLOWFAST_STAGE_DEPTH, f"{model_depth} is not in {_SLOWFAST_STAGE_DEPTH.keys()}"
+    depths = _SLOWFAST_STAGE_DEPTH[model_depth]
     if isinstance(slowfast_channel_reduction_ratio, int):
         slowfast_channel_reduction_ratio = (slowfast_channel_reduction_ratio,)
     if isinstance(stem_pool, Callable):

@@ -28,6 +28,25 @@ def create_res_basic_stem(*, in_channels, out_channels, conv_kernel_size=(3, 7, 
     )
 
 
+def create_acoustic_res_basic_stem(*, in_channels, out_channels, conv_kernel_size=(3, 7, 7), conv_stride=(1, 1, 1),
+                                   conv_padding=(1, 3, 3), conv_bias=False, pool=nn.MaxPool3d,
+                                   pool_kernel_size=(1, 3, 3), pool_stride=(1, 2, 2), pool_padding=(0, 1, 1),
+                                   norm=nn.BatchNorm3d, norm_eps=1e-5, norm_momentum=0.1, activation=nn.ReLU):
+    """Stem whose conv is a (kt,1,1) temporal and a (1,kh,kw) spatial convolution, summed (stem.py:110-212).
+    On device the two branches run as one (kt,kh,kw) convolution."""
+    from ..layers.convolutions import ConvReduce3D
+    return ResNetBasicStem(
+        conv=ConvReduce3D(in_channels=in_channels, out_channels=out_channels,
+                          kernel_size=((conv_kernel_size[0], 1, 1), (1, conv_kernel_size[1], conv_kernel_size[2])),
+                          stride=(conv_stride, conv_stride),
+                          padding=((conv_padding[0], 0, 0), (0, conv_padding[1], conv_padding[2])),
+                          bias=(conv_bias, conv_bias), reduction_method="sum"),
+        norm=None if norm is None else norm(num_features=out_channels, eps=norm_eps, momentum=norm_momentum),
+        activation=None if activation is None else activation(),
+        pool=None if pool is None else pool(kernel_size=pool_kernel_size, stride=pool_stride, padding=pool_padding),
+    )
+
+
 class PatchEmbed(B200Module):
     """Patchifying conv; on device its NDHWC output already IS the (B, THW, C) token layout, so the
     reference's flatten(2).transpose(1, 2) (stem.py:289-292) costs nothing."""

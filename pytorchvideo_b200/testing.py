@@ -383,3 +383,61 @@ def build_nonlocal_case(name, create_nonlocal, seed=91):
     g = torch.Generator(device="cpu")
     g.manual_seed(seed + 1)
     return m, f16_exact(torch.randn(shape, generator=g))
+
+
+# ---- audio model / layer cases (tests/golden/audio.pt): name -> (builder, kwargs, inputs) ----------------------------
+# inputs: ("avsf", B, T_fast, crop, (T_audio, F)) - slow / fast clips via slowfast_inputs (alpha 4) and a (B, 1, T, 1, F)
+# spectrogram; ("audio", B, T, F); ("layer", shape) - one tensor.
+AUDIO_CASES = {
+    "avsf_r50": ("create_audio_visual_slowfast", {}, ("avsf", 2, 32, 224, (128, 80))),
+    # the benchmarked shape, weights and inputs on the f16 grid (AUDIO_F16_GRID)
+    "avsf_r50_b8_f16grid": ("create_audio_visual_slowfast", {}, ("avsf", 8, 32, 224, (128, 80))),
+    "avsf_r18_norm_none": ("create_audio_visual_slowfast",
+                           dict(model_depth=18, norm=None, head_pool_kernel_sizes=((8, 2, 2), (32, 2, 2), (16, 1, 10))),
+                           ("avsf", 1, 32, 64, (128, 80))),
+    "avsf_r18_sigmoid": ("create_audio_visual_slowfast",
+                         dict(model_depth=18, activation=nn.Sigmoid,
+                              head_pool_kernel_sizes=((8, 2, 2), (32, 2, 2), (16, 1, 10))),
+                         ("avsf", 1, 32, 64, (128, 80))),
+    "acoustic_r50": ("create_acoustic_resnet", {}, ("audio", 2, 128, 80)),
+    # the reference test's arguments: kernel 3 stem, stride-2 stage 1, softmax head
+    "acoustic_r50_k3": ("create_acoustic_resnet",
+                        dict(stem_conv_kernel_size=(3, 1, 3), stage_temporal_stride=(2, 2, 2, 2),
+                             head_pool_kernel_size=(2, 1, 2), head_activation=nn.Softmax),
+                        ("audio", 2, 32, 32)),
+    # SeparableBottleneckBlock alone: W-only stride (1,1,2) on an H = 1 input
+    "separable_sum": ("create_acoustic_bottleneck_block",
+                      dict(dim_in=32, dim_inner=16, dim_out=64, conv_a_stride=(1, 1, 1), conv_b_kernel_size=(3, 1, 3),
+                           conv_b_stride=(1, 1, 2), conv_b_padding=(1, 0, 1)), ("layer", (2, 32, 6, 1, 20))),
+    "separable_cat": ("create_acoustic_bottleneck_block",
+                      dict(dim_in=32, dim_inner=16, dim_out=64, conv_a_stride=(1, 1, 1), conv_b_kernel_size=(3, 1, 3),
+                           conv_b_stride=(1, 1, 2), conv_b_padding=(1, 0, 1)), ("layer", (2, 32, 6, 1, 20))),
+}
+
+
+AUDIO_F16_GRID = ("avsf_r50_b8_f16grid",)
+
+
+def build_audio_case(name, builders, seed=2024):
+    """(module, inputs) of an AUDIO_CASES entry built from ``builders`` (a module exposing the builder functions:
+    this package's ``models`` or the reference's).  Weights from randomize_model (fresh init zeroes norm_c)."""
+    fn, kw, spec = AUDIO_CASES[name]
+    torch.manual_seed(seed)
+    m = getattr(builders, fn)(**kw)
+    if name == "separable_cat":
+        m.reduce_method = "cat"
+        m.conv_c = nn.Conv3d(2 * kw["dim_inner"], kw["dim_out"], kernel_size=(1, 1, 1), bias=False)
+    grid = name in AUDIO_F16_GRID
+    m = randomize_model(m, seed=seed, f16_weights=grid).eval()
+    if spec[0] == "avsf":
+        _, B, T, crop, (ta, f) = spec
+        x = slowfast_inputs(synthetic_clip(B, T, crop, crop, seed=seed + 1, f16_values=grid)) + \
+            [synthetic_clip(B, ta, 1, f, seed=seed + 2, channels=1, f16_values=grid)]
+    elif spec[0] == "audio":
+        _, B, ta, f = spec
+        x = synthetic_clip(B, ta, 1, f, seed=seed + 2, channels=1, f16_values=grid)
+    else:
+        g = torch.Generator(device="cpu")
+        g.manual_seed(seed + 3)
+        x = torch.randn(spec[1], generator=g)
+    return m, x
