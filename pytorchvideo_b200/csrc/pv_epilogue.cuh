@@ -2,11 +2,19 @@
 //
 // Two consumer warpgroups (256 threads) hold a 128-row x BN tile of fp32 accumulators in wgmma fragments
 // (warpgroup g: rows [64 g, 64 g + 64)) -> y = act(acc*scale+bias (+residual)) (+ addend[n][t][c]) -> f16 -> 128B-swizzled shared
-// staging -> TMA tensor store.  The residual tile is brought in by a TMA tensor load into the SAME staging buffer
-// (requested before the tile's main loop, so its latency hides behind the MMAs) and updated in place, so both the
-// residual read and the output write are full-line bulk transfers issued by one thread, with the tile-edge and
-// channel-tail clipping done by the TMA unit.  Staging is 32 KiB = two [128 rows x 64 f16] swizzled sub-tiles
-// (BN <= 128).
+// staging -> TMA tensor store.  The residual tile is brought in by a TMA tensor load into the staging buffer and
+// updated in place, so both the residual read and the output write are full-line bulk transfers, with the tile-edge
+// and channel-tail clipping done by the TMA unit.  One staging buffer is 32 KiB = two [128 rows x 64 f16] swizzled
+// sub-tiles (BN <= 128).
+//
+// Pipelining: a CTA's k-th tile uses staging buffer S[k % nbuf] (nbuf = 2, or 1 where shared memory allows only
+// one).  The consumers never touch the bulk-copy machinery; one elected lane of the epilogue DMA warp
+// (epilogue_dma) issues every residual load and output store, and two mbarriers per buffer hand it back and forth:
+//   epi_ready[b]  buffer free and its residual landed: the DMA warp's arrive (with expect_tx of the residual bytes)
+//   epi_full[b]   tile staged: one arrive per consumer warp, after every thread's fence.proxy.async
+// Per tile the DMA warp waits epi_full, stores, waits until the store has read the buffer out, then loads the
+// residual of the tile nbuf further on into it.  So the store of tile k drains while the consumers compute tile
+// k + 1, and each residual load is issued a whole tile ahead of its use.
 #pragma once
 #include "pv_common.cuh"
 #include "pv_sm90.cuh"
@@ -14,15 +22,21 @@
 namespace pv {
 namespace sm90 {
 
-constexpr int EPI_STAGING_BYTES = 2 * 128 * 128;
+constexpr int EPI_STAGING_BYTES = 2 * 128 * 128;   // one staging buffer
+constexpr int EPI_MAX_BUFS = 2;
+constexpr int EPI_BARS = 2 * EPI_MAX_BUFS;         // epi_ready[2], epi_full[2]
 constexpr int EPI_THREADS = 256;       // two consumer warpgroups
 constexpr int EPI_BAR_ID = 1;          // named barrier of the consumer warpgroups (0 is __syncthreads)
 constexpr int MAX_BN = 128;
+
+// Host: shared-memory bytes of the epilogue with `nbuf` staging buffers and its barriers.
+constexpr int epi_smem_bytes(int nbuf) { return nbuf * EPI_STAGING_BYTES + 8 * EPI_BARS; }
 
 struct EpiParams {
   CUtensorMap y_map;    // output  [Co, d1, d2, d3, d4], box [64, b1, b2, b3, b4], SWIZZLE_128B
   CUtensorMap r_map;    // residual, same geometry
   int block_n, Co, rows, act, has_residual;
+  int nbuf;             // staging buffers (1 or 2)
   // post-activation addend (pv_conv3d_desc.addend; nullptr = none): a[n * add_n + t * add_t + add_off + c]
   const __half* addend;
   long long add_n, add_t;
@@ -66,17 +80,61 @@ __device__ __forceinline__ float act_t(float x) {
   return apply_act(x, ACT);
 }
 
-// Tile start (consumer thread 0 only): the staging buffer is free once the previous tile's bulk store has read it;
-// then the residual tile of THIS tile is requested into it.  The named barrier in epilogue_tile publishes both.
-__device__ __forceinline__ void epilogue_begin(const EpiParams& E, uint32_t staging, uint32_t res_bar, int n0, int c1,
-                                               int c2, int c3, int c4) {
-  tma_store_wait_read0();
-  if (E.has_residual) {
-    const int nsub = (E.block_n + 63) >> 6;
-    mbar_arrive_expect_tx(res_bar, (uint32_t)(nsub * E.rows * 128));
-    for (int s = 0; s < nsub; ++s)
-      tma_load_5d(staging + (uint32_t)s * 16384u, &E.r_map, res_bar, n0 + s * 64, c1, c2, c3, c4);
+// Staging buffers S[b] (1024-aligned, EPI_STAGING_BYTES apart) and the epilogue's mbarriers in shared memory.
+struct EpiSmem {
+  uint32_t staging;       // S[0]
+  uint8_t* staging_gen;   // S[0], generic address
+  uint32_t bars;          // epi_ready[0..1], epi_full[0..1]
+  __device__ __forceinline__ uint32_t buf(int b) const { return staging + (uint32_t)b * EPI_STAGING_BYTES; }
+  __device__ __forceinline__ uint8_t* buf_gen(int b) const { return staging_gen + b * EPI_STAGING_BYTES; }
+  __device__ __forceinline__ uint32_t ready(int b) const { return bars + 8u * b; }
+  __device__ __forceinline__ uint32_t full(int b) const { return bars + 8u * (EPI_MAX_BUFS + b); }
+  __device__ __forceinline__ void init() const {   // one thread, before the kernel's fence_mbar_init
+    for (int b = 0; b < EPI_MAX_BUFS; ++b) {
+      mbar_init(ready(b), 1);                  // the DMA warp's (expect_tx) arrive
+      mbar_init(full(b), EPI_THREADS / 32);    // one arrive per consumer warp
+    }
   }
+};
+
+// The epilogue DMA warp: called by the whole warp after the kernel's griddepcontrol.wait (the residual may be
+// written by the previous kernel).  coords(tile, n0, c) gives a tile's first output channel and its origin in the
+// outer dims of the store / residual maps; the CTA's tiles are blockIdx.x, blockIdx.x + gridDim.x, ...
+template <class Coords>
+__device__ __forceinline__ void epilogue_dma(const EpiParams& E, const EpiSmem& S, int total_tiles, Coords coords) {
+  if (!elect_one()) return;
+  const int nbuf = E.nbuf;
+  const int nsub = (E.block_n + 63) >> 6;
+  auto fill = [&](int tile, int b) {   // buffer b is free: bring in the tile's residual (if any) and hand it over
+    if (E.has_residual) {
+      int n0, c[4];
+      coords(tile, n0, c);
+      mbar_arrive_expect_tx(S.ready(b), (uint32_t)(nsub * E.rows * 128));
+      for (int s = 0; s < nsub; ++s)
+        tma_load_5d(S.buf(b) + (uint32_t)s * 16384u, &E.r_map, S.ready(b), n0 + s * 64, c[0], c[1], c[2], c[3]);
+    } else {
+      mbar_arrive(S.ready(b));
+    }
+  };
+  for (int b = 0; b < nbuf; ++b) {
+    const int tile = (int)blockIdx.x + b * (int)gridDim.x;
+    if (tile < total_tiles) fill(tile, b);
+  }
+  int b = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    mbar_wait(S.full(b), phase);
+    int n0, c[4];
+    coords(tile, n0, c);
+    for (int s = 0; s < nsub; ++s)
+      tma_store_5d(&E.y_map, S.buf(b) + (uint32_t)s * 16384u, n0 + s * 64, c[0], c[1], c[2], c[3]);
+    tma_store_commit();
+    tma_store_wait_read0();   // the store has read S[b]: it may be refilled while the write drains to HBM
+    const long long next = (long long)tile + (long long)nbuf * gridDim.x;
+    if (next < total_tiles) fill((int)next, b);
+    if (++b == nbuf) { b = 0; phase ^= 1u; }
+  }
+  tma_store_wait_all();       // smem must outlive the bulk stores
 }
 
 // wgmma m64nBN fragment of consumer thread `ctid` (0..255): register 4 j + 2 i + e holds row
@@ -161,16 +219,14 @@ __device__ __forceinline__ void epi_addend(const EpiParams& E, uint8_t* stg, int
 
 // Called by the 256 consumer threads once the accumulators of the tile are complete (wgmma_wait<0>).
 // (c1..c4): tile origin in the store tensor map's outer dims; n0: first output channel of the tile.
+// (buf, phase): the tile's staging buffer and the parity of its barriers, both start at 0 and are advanced here.
 template <int BN>
-__device__ __forceinline__ void epilogue_tile(const EpiParams& E, const float* __restrict__ scale,
-                                              const float* __restrict__ bias, const float (&d)[BN / 2],
-                                              uint32_t staging, uint8_t* staging_gen, uint32_t res_bar,
-                                              uint32_t& res_phase, int ctid, int n0, int c1, int c2, int c3, int c4) {
-  epi_bar_sync(EPI_BAR_ID, EPI_THREADS);     // staging free (thread 0 waited for the previous store's read)
-  if (E.has_residual) {
-    mbar_wait(res_bar, res_phase);
-    res_phase ^= 1u;
-  }
+__device__ __forceinline__ void epilogue_tile(const EpiParams& E, const EpiSmem& S, int& buf, uint32_t& phase,
+                                              const float* __restrict__ scale, const float* __restrict__ bias,
+                                              const float (&d)[BN / 2], int ctid, int n0, int c1, int c2, int c3,
+                                              int c4) {
+  mbar_wait(S.ready(buf), phase);            // buffer free, residual landed
+  uint8_t* staging_gen = S.buf_gen(buf);
   switch (E.act) {
     case PV_ACT_RELU: epi_math_res<BN, PV_ACT_RELU>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid); break;
     case PV_ACT_NONE: epi_math_res<BN, PV_ACT_NONE>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid); break;
@@ -182,14 +238,11 @@ __device__ __forceinline__ void epilogue_tile(const EpiParams& E, const float* _
     epi_bar_sync(EPI_BAR_ID, EPI_THREADS);   // the cells of a row were written by other threads
     epi_addend<BN>(E, staging_gen, ctid, n0, c1, c2, c3, c4);
   }
-  // publish the staged tile to the async proxy and store it
+  // publish the staged tile to the async proxy and hand it to the DMA warp
   fence_proxy_async_smem();
-  epi_bar_sync(EPI_BAR_ID, EPI_THREADS);
-  if (ctid == 0) {
-    const int nsub = (E.block_n + 63) >> 6;
-    for (int s = 0; s < nsub; ++s) tma_store_5d(&E.y_map, staging + (uint32_t)s * 16384u, n0 + s * 64, c1, c2, c3, c4);
-    tma_store_commit();
-  }
+  __syncwarp();
+  mbar_arrive_if(S.full(buf), (ctid & 31) == 0);
+  if (++buf == E.nbuf) { buf = 0; phase ^= 1u; }
 }
 
 // Tile widths with a wgmma instantiation; the host rounds the channel count up to one of them.

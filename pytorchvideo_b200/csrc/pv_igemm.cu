@@ -12,10 +12,11 @@
 //   features are relied on.
 // * B operand (packed weights, K-major rows of taps*ci_pad64) is a 2-D TMA load [64, BLOCK_N].
 // * Both land in swizzled shared memory and feed wgmma (m64nBNk16) via shared-memory descriptors.
-// * Warp-specialised persistent kernel: one producer warpgroup (TMA, k-blocks dealt to up to 4 warps) and two
-//   consumer warpgroups; consumer warpgroup g issues the wgmma of tile rows [64 g, 64 g + 64), keeps their fp32
-//   accumulators in registers and runs the fused epilogue on them.  smem ring of `stages` {A,B} slots with
-//   full/empty mbarriers; one wgmma group stays in flight while the previous stage is released.
+// * Warp-specialised persistent kernel: one producer warpgroup (TMA loads of the k-blocks dealt to up to 3 warps,
+//   warp 11 the epilogue DMA warp) and two consumer warpgroups; consumer warpgroup g issues the wgmma of tile rows
+//   [64 g, 64 g + 64), keeps their fp32 accumulators in registers and runs the fused epilogue on them.  smem ring of
+//   `stages` {A,B} slots with full/empty mbarriers; one wgmma group stays in flight while the previous stage is
+//   released.
 #include "pv_common.cuh"
 #include "pv_sm90.cuh"
 #include "pv_epilogue.cuh"
@@ -31,9 +32,10 @@ using namespace sm90;
 constexpr int IG_BM = 128;        // two consumer warpgroups x wgmma M = 64
 constexpr int IG_MAX_TAPS = 64;
 constexpr int IG_MAX_MAPS = 8;
-constexpr int IG_PROD_WARPS = 4;   // TMA producer warps (one elected lane each, k-blocks round-robin)
+constexpr int IG_PROD_WARPS = 4;   // warps 8..10: TMA loads (one elected lane each, k-blocks round-robin); 11: epilogue DMA
 constexpr int IG_CONS_WARPS = 8;   // warps 0..7: two consumer warpgroups
 constexpr int IG_THREADS = (IG_CONS_WARPS + IG_PROD_WARPS) * 32;   // 384
+constexpr int IG_DMA_WARP = IG_CONS_WARPS + IG_PROD_WARPS - 1;
 
 struct IgemmParams {
   CUtensorMap a_maps[IG_MAX_MAPS];
@@ -50,7 +52,7 @@ struct IgemmParams {
   int kbytes;      // bytes of K per smem row and pipeline stage: 128 (64 ch, SW128) | 64 | 32 (window mode)
   int stages;
   int G, cpt;       // k-blocks per pipeline stage (chunk, 128 / kbytes: 64 K elements), chunks per tile
-  int split_ab;     // producer warps that share the loads of a chunk (1, 2 or 4)
+  int split_ab;     // producer warps that share the loads of a chunk (2 or 3)
   EpiParams epi;
   signed char tap_q[IG_MAX_TAPS][4];
   unsigned char tap_map[IG_MAX_TAPS];
@@ -78,13 +80,13 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& P, const float* __
   const uint32_t b_bytes = (uint32_t)BN * KB;
   const uint32_t stage_bytes = (uint32_t)G * (a_bytes + b_bytes);   // [G x A k-block][G x B k-block]
   constexpr int k_elems = KB / 2;
-  // epilogue staging (1024-aligned) and the barriers live after the tile ring
+  // epilogue staging buffers (1024-aligned) and the barriers live after the tile ring
   const uint32_t staging_off = (uint32_t)((stages * stage_bytes + 1023u) & ~1023u);
   const uint32_t staging = smem_base + staging_off;
-  const uint32_t bar_base = staging + (uint32_t)EPI_STAGING_BYTES;
+  const uint32_t bar_base = staging + (uint32_t)(P.epi.nbuf * EPI_STAGING_BYTES);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (stages + s); };
-  const uint32_t res_bar = bar_base + 8u * (2 * stages);
+  const EpiSmem epi{staging, smem_gen + staging_off, bar_base + 8u * (2 * stages)};
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -97,7 +99,7 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& P, const float* __
       mbar_init(full_bar(s), 1);                // producer warp 0's expect_tx arrive
       mbar_init(empty_bar(s), IG_CONS_WARPS);   // one arrive per consumer warp
     }
-    mbar_init(res_bar, 1);
+    epi.init();
     fence_mbar_init();
   }
   __syncthreads();
@@ -116,7 +118,13 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& P, const float* __
     for (int i = 0; i < 4; ++i) { o[i] = (mt % P.nt[i]) * P.box[i]; mt /= P.nt[i]; }
   };
 
-  if (warp >= IG_CONS_WARPS) {
+  if (warp == IG_DMA_WARP) {
+    epilogue_dma(P.epi, epi, total_tiles, [&](int tile, int& n0, int (&c)[4]) {
+      int n_tile;
+      tile_coords(tile, n_tile, c);
+      n0 = n_tile * BN;
+    });
+  } else if (warp >= IG_CONS_WARPS) {
     // ================================ TMA producers =========================================
     // The loads of a chunk (2 per k-block: A and B) are dealt round-robin to `nsplit` producer warps: one
     // issuing thread sustains only a limited rate of bulk-tensor loads.  Warp 0 of the group alone arrives on
@@ -169,15 +177,14 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& P, const float* __
     const int ctid = threadIdx.x;
     const uint32_t a_row_off = (uint32_t)(ctid >> 7) * 64u * (uint32_t)KB;   // this warpgroup's 64 rows
     const int cpt = P.cpt;
-    int stage = 0;
-    uint32_t phase = 0, res_phase = 0;
+    int stage = 0, epi_buf = 0;
+    uint32_t phase = 0, epi_phase = 0;
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       int n_tile, o[4];
       tile_coords(tile, n_tile, o);
-      if (ctid == 0) epilogue_begin(P.epi, staging, res_bar, n_tile * BN, o[0], o[1], o[2], o[3]);
       int prev = -1;
       for (int ch = 0; ch < cpt; ++ch) {
         mbar_wait(full_bar(stage), phase);
@@ -204,10 +211,8 @@ __device__ __forceinline__ void igemm_body(const IgemmParams& P, const float* __
       wgmma_wait<0>();
       acc_fence(acc);
       mbar_arrive_if(empty_bar(prev < 0 ? stage : prev), prev >= 0 && lane == 0);
-      epilogue_tile<BN>(P.epi, scale, bias, acc, staging, smem_gen + staging_off, res_bar, res_phase, ctid, n_tile * BN,
-                        o[0], o[1], o[2], o[3]);
+      epilogue_tile<BN>(P.epi, epi, epi_buf, epi_phase, scale, bias, acc, ctid, n_tile * BN, o[0], o[1], o[2], o[3]);
     }
-    if (ctid == 0) tma_store_wait_all();   // smem must outlive the bulk stores
   }
 }
 
@@ -476,20 +481,21 @@ int conv3d_tcgen05_launch(const pv_conv3d_desc* d, const void* x, const void* w,
   P.epi.rows = P.rows;
   P.epi.act = d->act;
   P.epi.has_residual = d->has_residual;
+  P.epi.nbuf = EPI_MAX_BUFS;
   epi_set_addend(P.epi, d);
   // k-blocks per pipeline stage: 64 K elements (the kernel's compile-time wgmma sequence, see conv3d_igemm_kernel)
   const int kb_bytes = (IG_BM + P.block_n) * P.kbytes;
-  const size_t smem_fixed = 2048 /*align*/ + EPI_STAGING_BYTES + 16;
+  const size_t smem_fixed = 2048 /*align*/ + epi_smem_bytes(P.epi.nbuf) + 16;
   {
     const int num_kb = P.taps * P.num_kc;
     const int G = 128 / P.kbytes;
-    const int budget = (int)(227 * 1024 - smem_fixed) - 8 * (2 * 24 + 1);   // barriers of up to 24 stages
+    const int budget = (int)(227 * 1024 - smem_fixed) - 8 * (2 * 24);   // barriers of up to 24 stages
     int st = budget / (G * kb_bytes);
     if (st > 24 / G) st = 24 / G > 2 ? 24 / G : 2;
     if (st < 2) st = 2;
     P.G = G;
-    // 2 producer warps (A / B) for one k-block per stage, 4 for chunked stages (window / narrow modes: up to 8 loads)
-    P.split_ab = G >= 2 ? 4 : 2;
+    // 2 producer warps (A / B) for one k-block per stage, 3 for chunked stages (window / narrow modes: up to 8 loads)
+    P.split_ab = G >= 2 ? 3 : 2;
     P.cpt = (num_kb + G - 1) / G;
     P.stages = st;
     // a padding k-block would load channel num_kc * 64 of the span, i.e. the next span's first channels
@@ -500,7 +506,7 @@ int conv3d_tcgen05_launch(const pv_conv3d_desc* d, const void* x, const void* w,
     }
   }
   const int stage_bytes = P.G * kb_bytes;
-  const size_t smem_bytes = (size_t)P.stages * stage_bytes + smem_fixed + 8 * (2 * P.stages + 1);
+  const size_t smem_bytes = (size_t)P.stages * stage_bytes + smem_fixed + 8 * (2 * P.stages);
 
   // ---- taps -> (parity map, coordinate shift); original dims order: tap index = (kt, kh, kw)
   // merged dims never merge a dim that has taps, so each non-trivial original dim maps to one

@@ -3,7 +3,7 @@
 //
 // With few input channels one filter tap is only 8..64 bytes of K, so a 64-channel TMA box per tap
 // would be mostly zero fill.  Here the GEMM K axis is the flattened (tap, ci) index and the A tile
-// (128 output positions x 64 K-elements, 128B-swizzled K-major) is assembled by 4 producer warps
+// (128 output positions x 64 K-elements, 128B-swizzled K-major) is assembled by up to 3 producer warps
 // with coalesced 8/16-byte global loads (im2col gather, zero fill for padding) written straight to
 // the swizzled shared-memory layout the wgmma descriptor expects; weights still arrive by TMA.
 // The two consumer warpgroups (wgmma, register accumulators, fused epilogue) are those of pv_igemm.cu.
@@ -24,8 +24,9 @@ constexpr int GG_BK = 64;
 constexpr int GG_A_BYTES = GG_BM * GG_BK * 2;
 constexpr int GG_MAX_UNITS = 256;
 constexpr int GG_CONS_WARPS = 8;          // warps 0..7: two consumer warpgroups
-constexpr int GG_PROD_WARPS = 4;          // warps 8..11: gather producers
-constexpr int GG_THREADS = (GG_CONS_WARPS + GG_PROD_WARPS) * 32;   // 384
+constexpr int GG_PROD_WARPS = 3;          // warps 8..10: gather producers
+constexpr int GG_THREADS = (GG_CONS_WARPS + GG_PROD_WARPS + 1) * 32;   // 384, warp 11: epilogue DMA
+constexpr int GG_DMA_WARP = GG_CONS_WARPS + GG_PROD_WARPS;
 
 struct GatherParams {
   CUtensorMap b_map;
@@ -39,7 +40,7 @@ struct GatherParams {
   long long x_row_stride;
   long long M;
   int m_tiles, n_tiles, block_n, Co, stages;
-  int nprod;   // active producer warps; stages is a multiple of nprod so every smem slot has ONE owner warp
+  int nprod;   // active producer warps, <= stages (see the slot-ownership note in the kernel)
   int depth;   // k-blocks of cp.async a producer warp keeps in flight: 2 when it owns >= 2 slots, else 1
   EpiParams epi;
   int unit_off[GG_MAX_UNITS];        // element offset of the unit relative to the row's (t0,h0,w0) corner
@@ -58,10 +59,10 @@ conv3d_igemm_gather_kernel(const __grid_constant__ GatherParams P, const __half*
   const uint32_t stage_bytes = GG_A_BYTES + b_bytes;
   const uint32_t staging_off = (uint32_t)((stages * stage_bytes + 1023u) & ~1023u);
   const uint32_t staging = smem_base + staging_off;
-  const uint32_t bar_base = staging + (uint32_t)EPI_STAGING_BYTES;
+  const uint32_t bar_base = staging + (uint32_t)(P.epi.nbuf * EPI_STAGING_BYTES);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (stages + s); };
-  const uint32_t res_bar = bar_base + 8u * (2 * stages);
+  const EpiSmem epi{staging, smem_gen + staging_off, bar_base + 8u * (2 * stages)};
 
   __shared__ int s_off[GG_MAX_UNITS];
   __shared__ unsigned s_d[GG_MAX_UNITS];
@@ -77,7 +78,7 @@ conv3d_igemm_gather_kernel(const __grid_constant__ GatherParams P, const __half*
       mbar_init(full_bar(s), 2);               // the owning producer warp's arrive + its expect_tx arrive
       mbar_init(empty_bar(s), GG_CONS_WARPS);  // one arrive per consumer warp
     }
-    mbar_init(res_bar, 1);
+    epi.init();
     fence_mbar_init();
   }
   __syncthreads();
@@ -88,7 +89,13 @@ conv3d_igemm_gather_kernel(const __grid_constant__ GatherParams P, const __half*
 
   const int total_tiles = P.n_tiles * P.m_tiles;
 
-  if (warp >= PROD_WARP0) {
+  if (warp == GG_DMA_WARP) {
+    epilogue_dma(P.epi, epi, total_tiles, [&](int tile, int& n0, int (&c)[4]) {
+      n0 = (tile % P.n_tiles) * BN;
+      c[0] = (tile / P.n_tiles) * GG_BM;
+      c[1] = c[2] = c[3] = 0;
+    });
+  } else if (warp >= PROD_WARP0) {
     // ================================ gather producers =======================================
     // Warp-per-k-block im2col gather.  Producer warp w owns k-blocks g = w, w+nprod, ... of this CTA's
     // (tile, k-block) sequence and fills the whole 128 x 64 A tile of that k-block alone: lane l
@@ -107,9 +114,11 @@ conv3d_igemm_gather_kernel(const __grid_constant__ GatherParams P, const __half*
     const unsigned Ti = (unsigned)P.Ti, Hi = (unsigned)P.Hi, Wi = (unsigned)P.Wi;
     const uint32_t rsw = (uint32_t)(lane & 7);           // (lane + 32q) & 7
     const uint32_t row_off = (uint32_t)lane * 128u;
-    // Slot ownership: stages % nprod == 0, so slot s is only ever filled by warp s % nprod, in order;
-    // a parity wait can then never alias a completion two phases back (it could with free-running
-    // warps sharing slots).
+    // Slot ownership: k-block g goes to slot g % stages and warp g % nprod, so when stages is not a multiple of
+    // nprod consecutive fills of a slot come from different warps.  A parity wait must then not alias a completion
+    // two phases back: the fill of g waits for the consumers to release g - stages, and the same warp's previous
+    // fill, g - nprod, already waited for g - nprod - stages >= g - 2 stages (nprod <= stages) to be released, and
+    // the consumers release in order.
     // ncu source view: the producers wait on their own cp.async data and on the empty barrier about equally.
     // Optional depth 2 (PVB200_GATHER_DEPTH2): with >= 2 slots per warp a k-block is published one iteration
     // later (cp.async groups), i.e. two k-blocks of copies in flight per warp - measured no faster, off by default.
@@ -228,15 +237,14 @@ conv3d_igemm_gather_kernel(const __grid_constant__ GatherParams P, const __half*
     const int ctid = threadIdx.x;
     const uint32_t a_row_off = (uint32_t)(ctid >> 7) * 64u * 128u;   // this warpgroup's 64 rows
     const int num_kb = P.num_kb;
-    int stage = 0;
-    uint32_t phase = 0, res_phase = 0;
+    int stage = 0, epi_buf = 0;
+    uint32_t phase = 0, epi_phase = 0;
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int n_tile = tile % P.n_tiles;
       const int m_tile = tile / P.n_tiles;
-      if (ctid == 0) epilogue_begin(P.epi, staging, res_bar, n_tile * BN, m_tile * GG_BM, 0, 0, 0);
       int prev = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(full_bar(stage), phase);
@@ -258,10 +266,8 @@ conv3d_igemm_gather_kernel(const __grid_constant__ GatherParams P, const __half*
       wgmma_wait<0>();
       acc_fence(acc);
       mbar_arrive_if(empty_bar(prev < 0 ? stage : prev), prev >= 0 && lane == 0);
-      epilogue_tile<BN>(P.epi, scale, bias, acc, staging, smem_gen + staging_off, res_bar, res_phase, ctid, n_tile * BN,
-                        m_tile * GG_BM, 0, 0, 0);
+      epilogue_tile<BN>(P.epi, epi, epi_buf, epi_phase, scale, bias, acc, ctid, n_tile * BN, m_tile * GG_BM, 0, 0, 0);
     }
-    if (ctid == 0) tma_store_wait_all();   // smem must outlive the bulk stores
   }
 }
 
@@ -342,6 +348,7 @@ int conv3d_gather_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   P.epi.rows = GG_BM;
   P.epi.act = d->act;
   P.epi.has_residual = d->has_residual;
+  P.epi.nbuf = EPI_MAX_BUFS;
   epi_set_addend(P.epi, d);
   for (int m = 0; m < 4; ++m) {      // output as [Co, M, 1, 1, 1]: a row's position is its GEMM row
     P.epi.o_ext[m] = m == 0 ? (int)P.M : 1;
@@ -350,17 +357,16 @@ int conv3d_gather_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   }
   const int stage_bytes = GG_A_BYTES + P.block_n * GG_BK * 2;
   {
-    int st = (227 * 1024 - 2048 - 2048 /*static tables*/ - EPI_STAGING_BYTES - 512) / stage_bytes;
+    int st = (227 * 1024 - 2048 - 2048 /*static tables*/ - epi_smem_bytes(P.epi.nbuf) - 512) / stage_bytes;
     if (st > 16) st = 16;
     if (st < 2) { set_error("gather: not enough smem stages"); return PV_ERR_UNSUPPORTED; }
     static const bool shallow = getenv("PVB200_GATHER_DEPTH2") == nullptr;   // opt-in only
-    // prefer two slots per producer warp (two k-blocks of copies in flight) over more warps with one slot
     P.nprod = st < GG_PROD_WARPS ? st : GG_PROD_WARPS;
-    if (!shallow && st >= 8 && st / 2 < P.nprod) P.nprod = st / 2;
-    P.stages = (st / P.nprod) * P.nprod;
+    P.stages = st;
+    // two k-blocks of copies in flight per warp need two slots per warp
     P.depth = (!shallow && P.stages >= 2 * P.nprod) ? 2 : 1;
   }
-  const size_t smem_bytes = (size_t)P.stages * stage_bytes + 2048 + EPI_STAGING_BYTES + 8 * (2 * P.stages + 1) + 16;
+  const size_t smem_bytes = (size_t)P.stages * stage_bytes + 2048 + epi_smem_bytes(P.epi.nbuf) + 8 * (2 * P.stages) + 16;
   for (int pass = 0; pass < 2; ++pass) {     // output / residual as [Co, M, 1, 1, 1]
     if (pass == 1 && !d->has_residual) break;
     const long long rs = pass == 0 ? d->y_row_stride : d->res_row_stride;

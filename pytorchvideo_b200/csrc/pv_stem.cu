@@ -31,8 +31,9 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 EncodeTiledFn get_encode_fn();   // pv_igemm.cu
 
 constexpr int ST_CONS_WARPS = 8;                                     // warps 0..7: two consumer warpgroups
-constexpr int ST_PROD_WARPS = 4;                                     // warps 8..11: bulk-copy producers
-constexpr int ST_THREADS = (ST_CONS_WARPS + ST_PROD_WARPS) * 32;     // 384
+constexpr int ST_PROD_WARPS = 3;                                     // warps 8..10: bulk-copy producers
+constexpr int ST_THREADS = (ST_CONS_WARPS + ST_PROD_WARPS + 1) * 32; // 384, warp 11: epilogue DMA
+constexpr int ST_DMA_WARP = ST_CONS_WARPS + ST_PROD_WARPS;
 constexpr int ST_MAX_ROWS = 64;                                      // kt * kh filter rows per tile
 
 struct StemParams {
@@ -70,16 +71,16 @@ conv3d_stem_rows_kernel(const __grid_constant__ StemParams P, const unsigned cha
   const uint32_t stage_bytes = (uint32_t)P.rows * P.seg_bytes + 2048u;       // + slack: the last windows read past a row
   const uint32_t staging_off = (ring_off + (uint32_t)stages * stage_bytes + 1023u) & ~1023u;
   const uint32_t staging = smem_base + staging_off;
-  const uint32_t bar_base = staging + (uint32_t)EPI_STAGING_BYTES;
+  const uint32_t bar_base = staging + (uint32_t)(P.epi.nbuf * EPI_STAGING_BYTES);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (stages + s); };
-  const uint32_t res_bar = bar_base + 8u * (2 * stages);
-  const uint32_t w_bar = res_bar + 8u;
+  const EpiSmem epi{staging, smem_gen + staging_off, bar_base + 8u * (2 * stages)};
+  const uint32_t w_bar = epi.bars + 8u * EPI_BARS;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int s = 0; s < stages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), ST_CONS_WARPS); }
-    mbar_init(res_bar, 1);
+    epi.init();
     mbar_init(w_bar, 1);
     prefetch_tmap(&P.epi.y_map);
     fence_mbar_init();
@@ -95,7 +96,13 @@ conv3d_stem_rows_kernel(const __grid_constant__ StemParams P, const unsigned cha
     to = tile % P.To; n = tile / P.To;
   };
 
-  if (warp >= ST_CONS_WARPS) {
+  if (warp == ST_DMA_WARP) {
+    epilogue_dma(P.epi, epi, total_tiles, [&](int tile, int& n0, int (&c)[4]) {
+      n0 = 0;
+      tile_coords(tile, c[0], c[1], c[2], c[3]);
+      c[0] *= 128;
+    });
+  } else if (warp >= ST_CONS_WARPS) {
     // ================================ producers: one bulk copy per input row ================================
     const int pw = warp - ST_CONS_WARPS;
     if (pw == 0 && elect_one()) {          // the packed weights, once
@@ -137,8 +144,8 @@ conv3d_stem_rows_kernel(const __grid_constant__ StemParams P, const unsigned cha
     const int ctid = threadIdx.x;
     const uint32_t a_row_off = (uint32_t)(ctid >> 7) * 64u * 16u;
     const uint32_t b_lbo = (uint32_t)P.n16 * 16u;          // weights: [K / 8][n16][8] - all N rows of a K chunk contiguous
-    int stage = 0;
-    uint32_t phase = 0, res_phase = 0;
+    int stage = 0, epi_buf = 0;
+    uint32_t phase = 0, epi_phase = 0;
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -146,7 +153,6 @@ conv3d_stem_rows_kernel(const __grid_constant__ StemParams P, const unsigned cha
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       int wt, ho, to, n;
       tile_coords(tile, wt, ho, to, n);
-      if (ctid == 0) epilogue_begin(P.epi, staging, res_bar, 0, wt * 128, ho, to, n);
       mbar_wait(full_bar(stage), phase);
       const uint32_t st_base = smem_base + ring_off + (uint32_t)stage * stage_bytes;
 #pragma unroll 1
@@ -169,10 +175,8 @@ conv3d_stem_rows_kernel(const __grid_constant__ StemParams P, const unsigned cha
       acc_fence(acc);
       mbar_arrive_if(empty_bar(stage), lane == 0);
       if (++stage == stages) { stage = 0; phase ^= 1u; }
-      epilogue_tile<BN>(P.epi, scale, bias, acc, staging, smem_gen + staging_off, res_bar, res_phase, ctid, 0, wt * 128, ho,
-                        to, n);
+      epilogue_tile<BN>(P.epi, epi, epi_buf, epi_phase, scale, bias, acc, ctid, 0, wt * 128, ho, to, n);
     }
-    if (ctid == 0) tma_store_wait_all();
   }
 }
 
@@ -227,9 +231,18 @@ extern "C" int pv_conv3d_stem_rows_fwd(const pv_conv3d_desc* d, const void* x, c
   P.base_off = (long long)(d->x_w_pad - d->pw - stem_window_lead(d)) * 8;
   P.w_bytes = (unsigned)((long long)P.rows * P.win * P.n16 * 2);
   P.seg_bytes = (unsigned)((127 * 16 + P.win * 2 + 127) & ~127);
-  // everything but the stage ring: alignment slack, resident weights, ring alignment, staging, barriers (8 stages max)
-  const size_t smem_fixed = 2048 + ((P.w_bytes + 1023) & ~1023u) + 1024 + EPI_STAGING_BYTES + 8 * (2 * 8 + 2) + 16;
+  // everything but the stage ring: alignment slack, resident weights, ring alignment, epilogue staging and barriers,
+  // ring and weight barriers (8 stages max).  With seg_bytes = 2176 for every window length, two staging buffers and
+  // two ring stages fit when align1024(w_bytes) + 4352 * rows + 4096 <= 163656: every accepted shape with
+  // kt * kh <= 9 filter rows (the ResNet, SlowFast, R(2+1)D and X3D stems have 3 or 7), and fewer as rows and weights
+  // grow.  Otherwise one staging buffer, which fits wherever the single-buffered epilogue of earlier versions did.
   const unsigned stage_bytes = (unsigned)P.rows * P.seg_bytes + 2048u;
+  size_t smem_fixed = 0;
+  for (int nbuf = EPI_MAX_BUFS; nbuf >= 1; --nbuf) {
+    P.epi.nbuf = nbuf;
+    smem_fixed = 2048 + ((P.w_bytes + 1023) & ~1023u) + 1024 + epi_smem_bytes(nbuf) + 8 * (2 * 8 + 1) + 16;
+    if (227 * 1024 - (long long)smem_fixed >= 2ll * stage_bytes) break;
+  }
   {
     const long long budget = 227 * 1024 - (long long)smem_fixed;
     long long st = budget / stage_bytes;
