@@ -497,6 +497,50 @@ typedef enum pv_attention_kernel {
   PV_ATTN_WIDE = 4      /* f16 wgmma + TMA kernel for wide heads / the linear mode */
 } pv_attention_kernel;
 int pv_attention_kernel_for(const pv_attention_desc* d, const void* q, const void* k, const void* v, const void* o);
+/* Key-masked softmax attention (models/masked_multistream.py:137-151, nn.MultiheadAttention with a key_padding_mask):
+ * pv_attention_fwd with key j of sample b taking part only where key_valid[b * Nk + j] != 0 (u8 [B][Nk]).  A row whose
+ * keys are all masked gets o = 0 and lse = -inf.  lse_out (optional, fp32 [B][H][Nq]) receives the log-sum-exp of the
+ * scaled scores, max + log(sum), for pv_attention_weights.  Same routing as pv_attention_fwd (pv_attention_kernel_for
+ * answers for both), head dims 32 / 64 / 96 / 128, softmax mode only (normalize = 1 or a q residual: PV_ERR_INVALID,
+ * other head dims: PV_ERR_UNSUPPORTED).  The masked instances are their own kernels; the unmasked ones are unchanged.
+ * pv_attention_weights: the head-averaged softmax nn.MultiheadAttention returns with need_weights=True,
+ *   w[b][i][j] = mean_h exp(scale * q_bhi . k_bhj - lse[b][h][i])  for valid keys, 0 for masked ones (fp32 [B][Nq][Nk]),
+ * recomputed from q / k and the lse of the forward (CUDA cores, fp32 maths).                                           */
+int pv_attention_masked_fwd(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
+                            const unsigned char* key_valid, float* lse_out, void* stream);
+int pv_attention_weights(const pv_attention_desc* d, const void* q, const void* k, const unsigned char* key_valid,
+                         const float* lse, float* w, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Masked sequence ops (models/masked_multistream.py, layers/fusion.py).  x: token rows [B][T][C] (row stride
+ * x_row_stride, C % 8 == 0), mask: u8 [B][T] (non-zero = valid) or NULL = every step valid.
+ * pv_masked_pool     : MaskedTemporalPooling (:35-93), fp32 accumulation, y [B][C]:
+ *                      mode 0 max  (invalid steps -inf; a row with no valid step gives 0),
+ *                      mode 1 avg  (masked sum / max(valid count, 1)), mode 2 sum (masked sum).
+ * pv_masked_default  : LearnMaskedDefault (:170-190): y = x * any + def * (1 - any) in fp32, any = any(mask[b]);
+ *                      x, y [B][C], def fp32 [C].
+ * pv_mask_force_first: dst = src with column 0 set (mask[:, 0] = True of :137-141 / :309-313), u8 [B][T].
+ * pv_reduce_fusion   : ReduceFusion (layers/fusion.py:104-141) y = max | sum | prod (op 0 | 1 | 2) over P <= 8
+ *                      same-shaped row sets xs[p] (row strides x_row_strides[p]), fp32 maths, `rows` rows of C.
+ * ------------------------------------------------------------------------------------------- */
+int pv_masked_pool(const void* x, int dtype, long long x_row_stride, int B, int T, int C, const unsigned char* mask,
+                   int mode, void* y, long long y_row_stride, void* stream);
+int pv_masked_default(const void* x, int dtype, long long x_row_stride, int B, int C, const unsigned char* mask, int T,
+                      const float* def, void* y, long long y_row_stride, void* stream);
+int pv_mask_force_first(const unsigned char* src, unsigned char* dst, int B, int T, void* stream);
+int pv_reduce_fusion(const void* const* xs, const long long* x_row_strides, int P, int dtype, long long rows, int C,
+                     int op, void* y, long long y_row_stride, void* stream);
+/* Masked LSTM recurrence (models/masked_multistream.py:193-256), all T steps of ndir (1 | 2) directions in one launch.
+ * G: gate pre-activations x W_ih^T + b_ih + b_hh, [B][T] rows of g_row_stride elements, direction d at columns
+ * d * 4H + gate * H + j (gate order i, f, g, o); w_hh_t: W_hh^T per direction, fp32 [ndir][H][4H]; mask: u8 [B][T] or
+ * NULL.  Row b runs its first len_b = clamp(popcount(mask[b]), 1, T) steps (the reverse direction from len_b - 1 down
+ * to 0) from h = c = 0 and writes y[b][d * H + j] = h_n; gates and c in fp32.  H <= 512, else PV_ERR_UNSUPPORTED.
+ * f16 with H a multiple of 32: one thread-block cluster per (direction, 32-row batch slice), W_hh resident in shared
+ * memory as f16 and a wgmma product per step with h as the f16 B operand (cluster size: the smallest S <= 16 with H / S
+ * a multiple of 32, at most 128, and 8 H^2 / S bytes of weights within 128 KiB); other H and f32 read W_hh from global
+ * memory every step and multiply on the CUDA cores.                                                               */
+int pv_lstm_recurrence(const void* G, int dtype, long long g_row_stride, const float* w_hh_t, const unsigned char* mask,
+                       int B, int T, int H, int ndir, void* y, long long y_row_stride, void* stream);
 
 #ifdef __cplusplus
 }

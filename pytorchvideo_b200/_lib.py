@@ -12,6 +12,8 @@ PV_F16, PV_F32, PV_U8 = 0, 1, 2
 ACT_NONE, ACT_RELU, ACT_SWISH, ACT_GELU, ACT_SIGMOID = 0, 1, 2, 3, 4
 ALGO_AUTO, ALGO_DIRECT, ALGO_TCGEN05 = 0, 1, 2
 POOL_MAX, POOL_AVG = 0, 1
+MPOOL_MAX, MPOOL_AVG, MPOOL_SUM = 0, 1, 2          # pv_masked_pool modes
+REDUCE_MAX, REDUCE_SUM, REDUCE_PROD = 0, 1, 2     # pv_reduce_fusion ops
 ATTN_WGMMA, ATTN_MMA, ATTN_SIMT, ATTN_WIDE = 1, 2, 3, 4
 
 c_ll = C.c_longlong
@@ -163,6 +165,14 @@ SIGNATURES = {
                                    C.c_float, c_vp]),
     "pv_attention_fwd": (C.c_int, [C.POINTER(AttentionDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_attention_kernel_for": (C.c_int, [C.POINTER(AttentionDesc), c_vp, c_vp, c_vp, c_vp]),
+    "pv_attention_masked_fwd": (C.c_int, [C.POINTER(AttentionDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_attention_weights": (C.c_int, [C.POINTER(AttentionDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_masked_pool": (C.c_int, [c_vp, C.c_int, c_ll, C.c_int, C.c_int, C.c_int, c_vp, C.c_int, c_vp, c_ll, c_vp]),
+    "pv_masked_default": (C.c_int, [c_vp, C.c_int, c_ll, C.c_int, C.c_int, c_vp, C.c_int, c_vp, c_vp, c_ll, c_vp]),
+    "pv_mask_force_first": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, c_vp]),
+    "pv_reduce_fusion": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, c_ll, C.c_int, C.c_int, c_vp, c_ll, c_vp]),
+    "pv_lstm_recurrence": (C.c_int, [c_vp, C.c_int, c_ll, c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_ll,
+                                     c_vp]),
 }
 
 _lib = None

@@ -14,10 +14,12 @@ constexpr int ATT_QPW = 4;                     // queries per warp
 constexpr int ATT_BQ = ATT_WARPS * ATT_QPW;    // 32 queries per CTA
 constexpr int ATT_BK = 32;                     // keys per tile
 
-template <typename T, int D>
+// MASKED: key j of sample b counts only where kv_valid[b * Nk + j] != 0; lse (optional) receives max + log(sum) per row.
+template <typename T, int D, bool MASKED = false>
 __global__ void __launch_bounds__(ATT_WARPS * 32)
 attention_kernel(pv_attention_desc d, const T* __restrict__ q, const T* __restrict__ k,
-                 const T* __restrict__ v, T* __restrict__ o) {
+                 const T* __restrict__ v, T* __restrict__ o,
+                 const unsigned char* __restrict__ kv_valid = nullptr, float* __restrict__ lse = nullptr) {
   constexpr int DS = D + 1;            // padded smem row stride (floats)
   constexpr int NC = D / 32;           // output columns per lane
   extern __shared__ float sh[];
@@ -65,7 +67,8 @@ attention_kernel(pv_attention_desc d, const T* __restrict__ q, const T* __restri
       Vs[r * DS + c] = vv;
     }
     __syncthreads();
-    const bool key_ok = (k0 + lane) < d.Nk;
+    bool key_ok = (k0 + lane) < d.Nk;
+    if constexpr (MASKED) key_ok = key_ok && kv_valid[(long long)b * d.Nk + k0 + lane] != 0;
 #pragma unroll
     for (int i = 0; i < ATT_QPW; ++i) {
       const float* qrow = Qs + (warp * ATT_QPW + i) * DS;
@@ -76,7 +79,7 @@ attention_kernel(pv_attention_desc d, const T* __restrict__ q, const T* __restri
       s = key_ok ? s : -INFINITY;
       float mx = s;
       for (int off = 16; off; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
-      const float m_new = fmaxf(m[i], mx);
+      const float m_new = fmaxf(m[i], mx);     // masked: -inf while no valid key was seen; p stays 0 then
       const float p = key_ok ? __expf(s - m_new) : 0.f;
       float ps = p;
       for (int off = 16; off; off >>= 1) ps += __shfl_xor_sync(0xffffffffu, ps, off);
@@ -102,7 +105,11 @@ attention_kernel(pv_attention_desc d, const T* __restrict__ q, const T* __restri
   for (int i = 0; i < ATT_QPW; ++i) {
     const int qi = q0 + warp * ATT_QPW + i;
     if (qi >= d.Nq) continue;
-    const float inv = 1.f / l[i];
+    float inv = 1.f / l[i];
+    if constexpr (MASKED) {          // a row without a valid key: o = 0, lse = -inf
+      inv = l[i] > 0.f ? inv : 0.f;
+      if (lse && lane == 0) lse[(long long)bh * d.Nq + qi] = l[i] > 0.f ? m[i] + logf(l[i]) : -INFINITY;
+    }
 #pragma unroll
     for (int c = 0; c < NC; ++c) {
       float val = acc[i][c] * inv;
@@ -112,13 +119,14 @@ attention_kernel(pv_attention_desc d, const T* __restrict__ q, const T* __restri
   }
 }
 
-template <typename T, int D>
+template <typename T, int D, bool MASKED = false>
 static int launch_attention(const pv_attention_desc* d, const void* q, const void* k, const void* v,
-                            void* o, cudaStream_t s, const char* name) {
+                            void* o, cudaStream_t s, const char* name, const unsigned char* kv_valid = nullptr,
+                            float* lse = nullptr) {
   const size_t smem = (size_t)((ATT_BQ + 2 * ATT_BK) * (D + 1) + ATT_WARPS * ATT_QPW * 32) * sizeof(float);
-  PV_OPT_IN_SMEM((attention_kernel<T, D>), smem);
+  PV_OPT_IN_SMEM((attention_kernel<T, D, MASKED>), smem);
   dim3 grid((unsigned)cdiv(d->Nq, ATT_BQ), (unsigned)(d->B * d->H)), block(ATT_WARPS * 32);
-  attention_kernel<T, D><<<grid, block, smem, s>>>(*d, (const T*)q, (const T*)k, (const T*)v, (T*)o);
+  attention_kernel<T, D, MASKED><<<grid, block, smem, s>>>(*d, (const T*)q, (const T*)k, (const T*)v, (T*)o, kv_valid, lse);
   PV_LAUNCH_OK(name);
   return PV_OK;
 }
@@ -131,7 +139,51 @@ int attention_wide_launch(const pv_attention_desc* d, const void* q, const void*
                           cudaStream_t s);   // pv_attention_wide.cu
 int attention_wide_simt_launch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
                                cudaStream_t s);   // pv_attention_wide.cu
+int attention_wgmma_masked_launch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
+                                  const unsigned char* kv_valid, float* lse, cudaStream_t s);   // pv_attention_wgmma.cu
+int attention_mma_masked_launch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
+                                const unsigned char* kv_valid, float* lse, cudaStream_t s);     // pv_attention_mma.cu
 
+// Head-averaged softmax weights of the masked forward: one CTA per (query i, sample b) stages the scaled query row and
+// its lse per head; a thread per key recomputes the scores in fp32 from q / k and normalises them with the lse.  `vec`:
+// 16-byte aligned k rows, read 8 elements at a time.
+template <typename T>
+__global__ void __launch_bounds__(128)
+attention_weights_kernel(pv_attention_desc d, const T* __restrict__ q, const T* __restrict__ k,
+                         const unsigned char* __restrict__ kv_valid, const float* __restrict__ lse,
+                         float* __restrict__ w, int vec) {
+  extern __shared__ float aw_q[];                      // [H * D] scaled query row, then [H] lse
+  const int i = blockIdx.x, b = blockIdx.y;
+  const int HD = d.H * d.D;
+  float* ls = aw_q + HD;
+  const T* qr = q + (long long)b * d.q_batch_stride + (long long)i * d.q_row_stride;
+  for (int e = threadIdx.x; e < HD; e += blockDim.x) aw_q[e] = Elem<T>::ld(qr + e) * d.scale;
+  for (int h = threadIdx.x; h < d.H; h += blockDim.x) ls[h] = lse[((long long)b * d.H + h) * d.Nq + i];
+  __syncthreads();
+  for (int j = threadIdx.x; j < d.Nk; j += blockDim.x) {
+    float acc = 0.f;
+    if (!kv_valid || kv_valid[(long long)b * d.Nk + j]) {
+      const T* kr = k + (long long)b * d.k_batch_stride + (long long)j * d.k_row_stride;
+      for (int h = 0; h < d.H; ++h) {
+        if (ls[h] == -INFINITY) continue;
+        const float* qh = aw_q + h * d.D;
+        float s = 0.f;
+        if (vec) {
+          for (int c = 0; c < d.D; c += 8) {
+            float v[8];
+            ld8<T>(kr + h * d.D + c, v);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) s = fmaf(qh[c + e], v[e], s);
+          }
+        } else {
+          for (int c = 0; c < d.D; ++c) s = fmaf(qh[c], Elem<T>::ld(kr + h * d.D + c), s);
+        }
+        acc += __expf(s - ls[h]);
+      }
+    }
+    w[((long long)b * d.Nq + i) * d.Nk + j] = acc / (float)d.H;
+  }
+}
 // Calls the kernels of pv_attention_wide.cu take: head dims 256 / 512 in either mode, and the linear mode
 // (normalize = 1) at 64 / 128.
 static bool wide_family(const pv_attention_desc* d) {
@@ -203,4 +255,56 @@ extern "C" int pv_attention_fwd(const pv_attention_desc* d, const void* q, const
 #undef PV_ATT
   pv::set_error("internal: attention head dim %d", d->D);
   return PV_ERR_INVALID;
+}
+
+extern "C" int pv_attention_masked_fwd(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
+                                       const unsigned char* key_valid, float* lse_out, void* stream) {
+  PV_CHECK_ARG(key_valid, "null key mask");
+  const int kernel = pv_attention_kernel_for(d, q, k, v, o);
+  if (kernel < 0) return kernel;
+  PV_CHECK_ARG(d->normalize == 0 && d->add_q_residual == 0, "masked attention is softmax only, without a q residual");
+  if (pv::wide_family(d)) {
+    pv::set_error("masked attention head dim %d unsupported (32/64/96/128)", d->D);
+    return PV_ERR_UNSUPPORTED;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  if (kernel == PV_ATTN_WGMMA) return pv::attention_wgmma_masked_launch(d, q, k, v, o, key_valid, lse_out, s);
+  if (kernel == PV_ATTN_MMA) return pv::attention_mma_masked_launch(d, q, k, v, o, key_valid, lse_out, s);
+#define PV_ATTM(DD)                                                                                              \
+  if (d->D == DD)                                                                                                \
+    return d->dtype == PV_F16                                                                                    \
+               ? pv::launch_attention<__half, DD, true>(d, q, k, v, o, s, "attention_masked_kernel<__half," #DD ">", \
+                                                        key_valid, lse_out)                                      \
+               : pv::launch_attention<float, DD, true>(d, q, k, v, o, s, "attention_masked_kernel<float," #DD ">",   \
+                                                       key_valid, lse_out);
+  PV_ATTM(32)
+  PV_ATTM(64)
+  PV_ATTM(96)
+  PV_ATTM(128)
+#undef PV_ATTM
+  pv::set_error("internal: masked attention head dim %d", d->D);
+  return PV_ERR_INVALID;
+}
+
+extern "C" int pv_attention_weights(const pv_attention_desc* d, const void* q, const void* k, const unsigned char* key_valid,
+                                    const float* lse, float* w, void* stream) {
+  PV_CHECK_ARG(d && q && k && lse && w, "null argument");
+  PV_CHECK_ARG(d->dtype == PV_F16 || d->dtype == PV_F32, "attention dtype must be f16|f32");
+  PV_CHECK_ARG(d->B > 0 && d->H > 0 && d->Nq > 0 && d->Nk > 0 && d->D > 0, "empty attention problem");
+  PV_CHECK_ARG(d->B <= 65535 && (long long)d->H * d->D <= 8192, "attention weights: B <= 65535, H * D <= 8192");
+  cudaStream_t s = (cudaStream_t)stream;
+  const dim3 grid((unsigned)d->Nq, (unsigned)d->B);
+  const size_t smem = (size_t)(d->H * d->D + d->H) * sizeof(float);
+  const int vec = d->D % 8 == 0 && d->k_row_stride % 8 == 0 && (d->B == 1 || d->k_batch_stride % 8 == 0) &&
+                  (reinterpret_cast<uintptr_t>(k) & 15) == 0;
+  if (d->dtype == PV_F16) {
+    pv::attention_weights_kernel<__half><<<grid, 128, smem, s>>>(*d, (const __half*)q, (const __half*)k, key_valid, lse, w,
+                                                                 vec);
+    PV_LAUNCH_OK("attention_weights_kernel<__half>");
+  } else {
+    pv::attention_weights_kernel<float><<<grid, 128, smem, s>>>(*d, (const float*)q, (const float*)k, key_valid, lse, w,
+                                                                vec);
+    PV_LAUNCH_OK("attention_weights_kernel<float>");
+  }
+  return PV_OK;
 }

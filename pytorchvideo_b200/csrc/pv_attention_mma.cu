@@ -21,10 +21,12 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-template <int D>
+// MASKED: key j of sample b counts only where kv_valid[b * Nk + j] != 0; lse (optional) receives max + log(sum) per row.
+template <int D, bool MASKED = false>
 __global__ void __launch_bounds__(FA_WARPS * 32)
 attention_mma_kernel(pv_attention_desc d, const __half* __restrict__ q, const __half* __restrict__ k,
-                     const __half* __restrict__ v, __half* __restrict__ o) {
+                     const __half* __restrict__ v, __half* __restrict__ o,
+                     const unsigned char* __restrict__ kv_valid = nullptr, float* __restrict__ lse = nullptr) {
   constexpr int DS = D + 8;                 // padded smem row (halves): conflict-free fragment loads
   constexpr int KS = D / 16;                // k-steps of the QK^T product
   constexpr int ND = D / 8;                 // n-tiles of the PV product
@@ -119,7 +121,8 @@ attention_mma_kernel(pv_attention_desc d, const __half* __restrict__ q, const __
       const int key = kbase + nt * 8;
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const bool ok = (key + (e & 1)) < d.Nk;
+        bool ok = (key + (e & 1)) < d.Nk;
+        if constexpr (MASKED) ok = ok && kv_valid[(long long)b * d.Nk + key + (e & 1)] != 0;
         s[nt][e] = ok ? s[nt][e] * d.scale : -INFINITY;
       }
       mx0 = fmaxf(mx0, fmaxf(s[nt][0], s[nt][1]));
@@ -129,15 +132,17 @@ attention_mma_kernel(pv_attention_desc d, const __half* __restrict__ q, const __
     mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
     mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
     mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);     // finite: every tile has >= 1 valid key
+    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);     // unmasked: finite, every tile has >= 1 valid key
     const float c0 = (m0 == -INFINITY) ? 0.f : __expf(m0 - mn0);
     const float c1 = (m1 == -INFINITY) ? 0.f : __expf(m1 - mn1);
     m0 = mn0; m1 = mn1;
+    // masked: no valid key so far leaves the maximum at -inf; subtract 0 then, never -inf - -inf
+    const float e0 = (MASKED && mn0 == -INFINITY) ? 0.f : mn0, e1 = (MASKED && mn1 == -INFINITY) ? 0.f : mn1;
     float ps0 = 0.f, ps1 = 0.f;
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
-      s[nt][0] = __expf(s[nt][0] - mn0); s[nt][1] = __expf(s[nt][1] - mn0);
-      s[nt][2] = __expf(s[nt][2] - mn1); s[nt][3] = __expf(s[nt][3] - mn1);
+      s[nt][0] = __expf(s[nt][0] - e0); s[nt][1] = __expf(s[nt][1] - e0);
+      s[nt][2] = __expf(s[nt][2] - e1); s[nt][3] = __expf(s[nt][3] - e1);
       ps0 += s[nt][0] + s[nt][1];
       ps1 += s[nt][2] + s[nt][3];
     }
@@ -173,7 +178,16 @@ attention_mma_kernel(pv_attention_desc d, const __half* __restrict__ q, const __
   // ---- finalise: row sums across the 4 lanes of a row, normalise, (+q), store
   l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-  const float i0 = 1.f / l0, i1 = 1.f / l1;
+  float i0 = 1.f / l0, i1 = 1.f / l1;
+  if constexpr (MASKED) {          // a row without a valid key: o = 0, lse = -inf
+    i0 = l0 > 0.f ? i0 : 0.f;
+    i1 = l1 > 0.f ? i1 : 0.f;
+    if (lse && t == 0) {
+      float* lr = lse + (long long)bh * d.Nq;
+      if (qa < d.Nq) lr[qa] = l0 > 0.f ? m0 + logf(l0) : -INFINITY;
+      if (qb8 < d.Nq) lr[qb8] = l1 > 0.f ? m1 + logf(l1) : -INFINITY;
+    }
+  }
 #pragma unroll
   for (int nd = 0; nd < ND; ++nd) {
     const int col = nd * 8 + 2 * t;
@@ -196,13 +210,15 @@ attention_mma_kernel(pv_attention_desc d, const __half* __restrict__ q, const __
   }
 }
 
-template <int D>
+template <int D, bool MASKED = false>
 static int launch_attention_mma(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
-                                cudaStream_t s, const char* name) {
+                                cudaStream_t s, const char* name, const unsigned char* kv_valid = nullptr,
+                                float* lse = nullptr) {
   const size_t smem = (size_t)4 * FA_BK * (D + 8) * sizeof(__half);
-  PV_OPT_IN_SMEM(attention_mma_kernel<D>, smem);
+  PV_OPT_IN_SMEM((attention_mma_kernel<D, MASKED>), smem);
   dim3 grid((unsigned)cdiv(d->Nq, FA_BQ), (unsigned)(d->B * d->H)), block(FA_WARPS * 32);
-  attention_mma_kernel<D><<<grid, block, smem, s>>>(*d, (const __half*)q, (const __half*)k, (const __half*)v, (__half*)o);
+  attention_mma_kernel<D, MASKED><<<grid, block, smem, s>>>(*d, (const __half*)q, (const __half*)k, (const __half*)v,
+                                                           (__half*)o, kv_valid, lse);
   PV_LAUNCH_OK(name);
   return PV_OK;
 }
@@ -217,6 +233,18 @@ int attention_mma_launch(const pv_attention_desc* d, const void* q, const void* 
     default: set_error("internal: mma attention head dim %d", d->D); return PV_ERR_INVALID;
   }
 #undef PV_AM
+}
+
+// Key-masked twin (pv_attention_masked_fwd); same alignment rules.  Only D = 128 is routed here.
+int attention_mma_masked_launch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
+                                const unsigned char* kv_valid, float* lse, cudaStream_t s) {
+#define PV_AMM(DD) \
+  case DD: return launch_attention_mma<DD, true>(d, q, k, v, o, s, "attention_mma_masked_kernel<" #DD ">", kv_valid, lse);
+  switch (d->D) {
+    PV_AMM(128)
+    default: set_error("internal: masked mma attention head dim %d", d->D); return PV_ERR_INVALID;
+  }
+#undef PV_AMM
 }
 
 }  // namespace pv

@@ -33,9 +33,11 @@ __device__ __forceinline__ uint32_t aw_pack_h2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-template <int D>
+// MASKED: key j of sample b counts only where kv_valid[b * Nk + j] != 0; lse (optional) receives max + log(sum) per row.
+template <int D, bool MASKED = false>
 __global__ void __launch_bounds__(128, 1)
-attention_wgmma_kernel(const __grid_constant__ AttnWgParams P, const __half* __restrict__ q, __half* __restrict__ o) {
+attention_wgmma_kernel(const __grid_constant__ AttnWgParams P, const __half* __restrict__ q, __half* __restrict__ o,
+                       const unsigned char* __restrict__ kv_valid = nullptr, float* __restrict__ lse = nullptr) {
   constexpr int NC = D / 32;                          // 32-dim chunks
   constexpr uint32_t TILE = NC * AW_CHUNK;            // one Q / K / V tile
   extern __shared__ uint8_t aw_smem[];
@@ -107,7 +109,8 @@ attention_wgmma_kernel(const __grid_constant__ AttnWgParams P, const __half* __r
       const int key = kbase + nt * 8;
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const bool ok = (key + (e & 1)) < d.Nk;
+        bool ok = (key + (e & 1)) < d.Nk;
+        if constexpr (MASKED) ok = ok && kv_valid[(long long)b * d.Nk + key + (e & 1)] != 0;
         sacc[4 * nt + e] = ok ? sacc[4 * nt + e] * d.scale : -INFINITY;
       }
       mx0 = fmaxf(mx0, fmaxf(sacc[4 * nt], sacc[4 * nt + 1]));
@@ -117,15 +120,17 @@ attention_wgmma_kernel(const __grid_constant__ AttnWgParams P, const __half* __r
     mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
     mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
     mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);     // finite: every tile has >= 1 valid key
+    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);     // unmasked: finite, every tile has >= 1 valid key
     const float c0 = (m0 == -INFINITY) ? 0.f : __expf(m0 - mn0);
     const float c1 = (m1 == -INFINITY) ? 0.f : __expf(m1 - mn1);
     m0 = mn0; m1 = mn1;
+    // masked: no valid key so far leaves the maximum at -inf; subtract 0 then, never -inf - -inf
+    const float e0 = (MASKED && mn0 == -INFINITY) ? 0.f : mn0, e1 = (MASKED && mn1 == -INFINITY) ? 0.f : mn1;
     float ps0 = 0.f, ps1 = 0.f;
 #pragma unroll
     for (int nt = 0; nt < 8; ++nt) {
-      sacc[4 * nt] = __expf(sacc[4 * nt] - mn0); sacc[4 * nt + 1] = __expf(sacc[4 * nt + 1] - mn0);
-      sacc[4 * nt + 2] = __expf(sacc[4 * nt + 2] - mn1); sacc[4 * nt + 3] = __expf(sacc[4 * nt + 3] - mn1);
+      sacc[4 * nt] = __expf(sacc[4 * nt] - e0); sacc[4 * nt + 1] = __expf(sacc[4 * nt + 1] - e0);
+      sacc[4 * nt + 2] = __expf(sacc[4 * nt + 2] - e1); sacc[4 * nt + 3] = __expf(sacc[4 * nt + 3] - e1);
       ps0 += sacc[4 * nt] + sacc[4 * nt + 1];
       ps1 += sacc[4 * nt + 2] + sacc[4 * nt + 3];
     }
@@ -167,8 +172,17 @@ attention_wgmma_kernel(const __grid_constant__ AttnWgParams P, const __half* __r
   // ---- finalise: row sums across the 4 lanes of a row, normalise, (+q), store
   l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-  const float i0 = 1.f / l0, i1 = 1.f / l1;
+  float i0 = 1.f / l0, i1 = 1.f / l1;
   const int qa = q0 + warp * 16 + g, qb8 = qa + 8;
+  if constexpr (MASKED) {          // a row without a valid key: o = 0, lse = -inf
+    i0 = l0 > 0.f ? i0 : 0.f;
+    i1 = l1 > 0.f ? i1 : 0.f;
+    if (lse && t == 0) {
+      float* lr = lse + (long long)bh * d.Nq;
+      if (qa < d.Nq) lr[qa] = l0 > 0.f ? m0 + logf(l0) : -INFINITY;
+      if (qb8 < d.Nq) lr[qb8] = l1 > 0.f ? m1 + logf(l1) : -INFINITY;
+    }
+  }
   const __half* qb = q + (long long)b * d.q_batch_stride + (long long)h * D;
   __half* ob = o + (long long)b * d.o_batch_stride + (long long)h * D;
 #pragma unroll
@@ -205,9 +219,9 @@ static bool aw_encode(EncodeTiledFn encode, CUtensorMap* m, const void* p, const
                 CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int D>
+template <int D, bool MASKED = false>
 static int launch_attention_wgmma(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o, cudaStream_t s,
-                                  const char* name) {
+                                  const char* name, const unsigned char* kv_valid = nullptr, float* lse = nullptr) {
   EncodeTiledFn encode = get_encode_fn();
   if (!encode) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return PV_ERR_CUDA; }
   AttnWgParams P;
@@ -220,9 +234,9 @@ static int launch_attention_wgmma(const pv_attention_desc* d, const void* q, con
     return PV_ERR_CUDA;
   }
   constexpr size_t smem = 1024 + 5 * (size_t)(D / 32) * AW_CHUNK + 64;
-  PV_OPT_IN_SMEM(attention_wgmma_kernel<D>, smem);
+  PV_OPT_IN_SMEM((attention_wgmma_kernel<D, MASKED>), smem);
   dim3 grid((unsigned)cdiv(d->Nq, AW_BQ), (unsigned)(d->B * d->H)), block(128);
-  attention_wgmma_kernel<D><<<grid, block, smem, s>>>(P, (const __half*)q, (__half*)o);
+  attention_wgmma_kernel<D, MASKED><<<grid, block, smem, s>>>(P, (const __half*)q, (__half*)o, kv_valid, lse);
   PV_LAUNCH_OK(name);
   return PV_OK;
 }
@@ -237,6 +251,18 @@ int attention_wgmma_launch(const pv_attention_desc* d, const void* q, const void
     default: set_error("internal: wgmma attention head dim %d", d->D); return PV_ERR_INVALID;
   }
 #undef PV_AW
+}
+
+// Key-masked twin (pv_attention_masked_fwd); same alignment rules and head dims.
+int attention_wgmma_masked_launch(const pv_attention_desc* d, const void* q, const void* k, const void* v, void* o,
+                                  const unsigned char* kv_valid, float* lse, cudaStream_t s) {
+#define PV_AWM(DD) \
+  case DD: return launch_attention_wgmma<DD, true>(d, q, k, v, o, s, "attention_wgmma_masked_kernel<" #DD ">", kv_valid, lse);
+  switch (d->D) {
+    PV_AWM(32) PV_AWM(64) PV_AWM(96)
+    default: set_error("internal: masked wgmma attention head dim %d", d->D); return PV_ERR_INVALID;
+  }
+#undef PV_AWM
 }
 
 }  // namespace pv

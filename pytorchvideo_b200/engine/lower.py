@@ -5,6 +5,8 @@ Dispatch is by class *name* and attribute names, exactly the names the reference
 same lowering accepts this package's own parameter-container modules and - where the reference
 is importable - the reference's modules themselves (state_dict-compatible drop-in, SURVEY 8b).
 """
+import weakref
+
 import torch
 import torch.nn as nn
 
@@ -650,8 +652,9 @@ class CompiledModel:
         multi = isinstance(example_inputs, (list, tuple))
         ins = list(example_inputs) if multi else [example_inputs]
         raw = _raw_inputs(model, ins)
+        self.mask_slots = _mask_slots(ins, extra)
         for i, t in enumerate(ins):
-            if i not in raw and t.dim() not in (2, 3, 5):
+            if i not in raw and i not in self.mask_slots and t.dim() not in (2, 3, 5):
                 raise RuntimeError("expected a 5-D (B, C, T, H, W) clip or a (B, N, C) token tensor, got %s" % (tuple(t.shape),))
         device = ins[0].device
         if device.type != "cuda":
@@ -659,11 +662,13 @@ class CompiledModel:
         dt = {"f16": L.PV_F16, "f32": L.PV_F32}[dtype]
         self.multi = multi
         self.plan = Plan(device, dt, use_tcgen05)
-        self.static_in = [torch.empty(t.shape, dtype=t.dtype if (t.dtype in (torch.float16, torch.float32) and i not in raw)
+        self.static_in = [torch.empty(t.shape, dtype=torch.uint8 if i in self.mask_slots else
+                                      t.dtype if (t.dtype in (torch.float16, torch.float32) and i not in raw)
                                       else torch.float32, device=device) for i, t in enumerate(ins)]
         low = Lowering(self.plan, extra)
-        xs = [self.plan.raw_input(s) if i in raw else _emit_input(self.plan, s) for i, s in enumerate(self.static_in)]
-        out = low.lower(model, xs if multi else xs[0], "")
+        xs = [self.plan.raw_input(s) if i in raw else PL.MaskRef(s.shape[0], s.shape[1], tensor=s) if i in self.mask_slots
+              else _emit_input(self.plan, s) for i, s in enumerate(self.static_in)]
+        out = low.lower(model, _root_input(xs, ins, extra) if _masked_root(extra) else (xs if multi else xs[0]), "")
         out = _emit_output(self.plan, out, tokens=ins[0].dim() != 5)
         self.out_buf, self.out_shape = out
         self.aux = low.aux_out
@@ -701,13 +706,21 @@ class CompiledModel:
         ins = list(inputs) if self.multi else [inputs]
         if len(ins) != len(self.static_in):
             raise RuntimeError("expected %d input tensors, got %d" % (len(self.static_in), len(ins)))
-        for s, t in zip(self.static_in, ins):
+        for i, (s, t) in enumerate(zip(self.static_in, ins)):
             if not torch.is_tensor(t) or tuple(t.shape) != tuple(s.shape):
                 raise RuntimeError("input shape %s differs from the compiled shape %s (compile a plan per shape)" % (
                     tuple(t.shape) if torch.is_tensor(t) else type(t).__name__, tuple(s.shape)))
-            if not (t.is_floating_point() or t.dtype == torch.uint8):
+            if i in self.mask_slots:
+                if t.dtype != torch.bool:
+                    raise RuntimeError("input %d is a mask: expected a bool tensor, got %s" % (i, t.dtype))
+            elif not (t.is_floating_point() or t.dtype == torch.uint8):
                 raise RuntimeError("unsupported input dtype %s" % t.dtype)
         return ins
+
+    def side_outputs(self):
+        """[(module, device tensor, shape)] of the per-module results of the last replay (attention weights)."""
+        outs = [(ref(), b.tensor[:int(torch.tensor(shape).prod())], shape) for ref, b, shape in self.plan.side_outputs]
+        return [o for o in outs if o[0] is not None]
 
     def __call__(self, inputs):
         ins = self.check_inputs(inputs)
@@ -737,10 +750,42 @@ def _raw_inputs(model, ins):
     return set()
 
 
+def _masked_root(extra):
+    return bool(extra) and isinstance(extra[0], tuple) and len(extra[0]) >= 2 and extra[0][0] == "masks"
+
+
+def _mask_slots(ins, extra):
+    """Indices of the bool (B, T) masks of a masked module's inputs.  Masked modules call the engine with a flat list
+    [x0, (mask0), x1, (mask1), ...] and extra[0] = ("masks", multi, has_mask0, has_mask1, ...)."""
+    if not _masked_root(extra):
+        return set()
+    slots, i = set(), 0
+    for has in extra[0][2:]:
+        if has:
+            slots.add(i + 1)
+        i += 2 if has else 1
+    if i != len(ins):
+        raise RuntimeError("masked inputs: %d tensors for the layout %s" % (len(ins), extra[0]))
+    return slots
+
+
+def _root_input(xs, ins, extra):
+    """The (x, mask_ref) pair - or the list of pairs of a MaskedMultiPathWay - a masked root module is lowered on."""
+    pairs, i = [], 0
+    for has in extra[0][2:]:
+        x = xs[i]
+        pairs.append((x, xs[i + 1] if has else None))
+        i += 2 if has else 1
+    return pairs if extra[0][1] else pairs[0]
+
+
 def _emit_input(plan, t):
     if t.dim() == 5:
         return plan.emit_input_ncdhw(t, t.shape[1], 4 if t.shape[1] <= 4 else (t.shape[1] + 7) // 8 * 8)
-    return plan.emit_input_tokens(t)
+    x = plan.emit_input_tokens(t)
+    if t.dim() == 2:
+        x.squeeze = True          # a (batch, feature) input: lowerings that keep its rank hand the mark on
+    return x
 
 
 def _emit_output(plan, out, tokens):
@@ -765,10 +810,12 @@ def lower_only(model, example_inputs, dtype="f16", use_tcgen05=True, extra=()):
     ins = list(example_inputs) if multi else [example_inputs]
     plan = Plan("cpu", {"f16": L.PV_F16, "f32": L.PV_F32}[dtype], use_tcgen05)
     raw = _raw_inputs(model, ins)
+    masks = _mask_slots(ins, extra)
     xs = [plan.raw_input(torch.empty(t.shape, dtype=torch.float32)) if i in raw
+          else PL.MaskRef(t.shape[0], t.shape[1], tensor=torch.empty(t.shape, dtype=torch.uint8)) if i in masks
           else _emit_input(plan, torch.empty(t.shape, dtype=torch.float32)) for i, t in enumerate(ins)]
     low = Lowering(plan, extra)
-    out = low.lower(model, xs if multi else xs[0], "")
+    out = low.lower(model, _root_input(xs, ins, extra) if _masked_root(extra) else (xs if multi else xs[0]), "")
     out = _emit_output(plan, out, tokens=ins[0].dim() != 5)
     plan.aux = low.aux_out
     return plan, out[1]
@@ -1013,3 +1060,337 @@ Lowering.lower_PatchEmbed = _lower_patch_embed_module
 Lowering.lower_VisionTransformerBasicHead = _lower_vit_head_module
 Lowering.lower_SequencePool = _lower_sequence_pool_module
 Lowering.lower_MultiscaleVisionTransformers = _lower_mvit
+
+
+# =============================================================================================
+# Masked multistream lowering (models/masked_multistream.py, layers/fusion.py, layers/positional_encoding.py:11-44).
+# A masked handler takes (x, mask) and returns (y, mask): the attention modules hand the mask with its first column
+# forced valid (:137-141, :309-313) to the modules after them, as the reference's in-place write does.  Token tensors
+# are TRef(B, 1, 1, T, C); ``squeeze`` marks a (batch, feature) tensor, ``retargetable`` a result whose producer
+# resolves its row stride at run time, so that ConcatFusion can move it into a channel slice.
+# =============================================================================================
+_MASK_MODULES = ("MaskedTemporalPooling", "LearnMaskedDefault", "TransposeMultiheadAttention", "LSTM",
+                 "TransposeTransformerEncoder")
+_MASKED_HEAD_DIMS = (32, 64, 96, 128)
+_MPOOL = {"max": L.MPOOL_MAX, "avg": L.MPOOL_AVG, "sum": L.MPOOL_SUM}
+
+
+def _is_mask_module(m):
+    n = type(m).__name__
+    return n in _MASK_MODULES and (n != "LSTM" or hasattr(m, "lstm"))       # a plain nn.LSTM takes no mask
+
+
+def _mark(y, x=None, squeeze=None, retargetable=False):
+    y.squeeze = getattr(x, "squeeze", False) if squeeze is None else squeeze
+    y.retargetable = retargetable
+    return y
+
+
+def _token_input(x, name, what):
+    if not isinstance(x, TRef) or x.T != 1 or x.H != 1 or x.lazy_src is not None:
+        raise NotImplementedError("%s: %s runs on (batch, seq_len, feature) token tensors only" % (name, what))
+
+
+def _check_mask(x, mask, name):
+    if mask is not None and (mask.B != x.N or mask.T != x.npos):
+        raise RuntimeError("%s: mask of shape %s for x with (batch, seq_len) = %s" % (name, (mask.B, mask.T),
+                                                                                      (x.N, x.npos)))
+
+
+def _seq3(x, name):
+    if getattr(x, "squeeze", False):
+        raise RuntimeError("%s: requires x shape (batch_size x seq_len x feature_dim)" % name)
+
+
+def _mha_check(a, name):
+    if not getattr(a, "_qkv_same_embed_dim", True) or a.bias_k is not None or a.add_zero_attn or \
+            getattr(a, "batch_first", False):
+        raise NotImplementedError("%s: MultiheadAttention variant unsupported (kdim / vdim, bias_kv, add_zero_attn, "
+                                  "batch_first)" % name)
+    D = a.embed_dim // a.num_heads
+    if D not in _MASKED_HEAD_DIMS:
+        raise NotImplementedError("%s: head dim %d (embed_dim %d / num_heads %d) has no masked attention kernel "
+                                  "(supported: %s)" % (name, D, a.embed_dim, a.num_heads, _MASKED_HEAD_DIMS))
+    return D
+
+
+def _mha(low, a, x, mask, name, weights):
+    """nn.MultiheadAttention(x, x, x, key_padding_mask=~mask): the in-projection as one GEMM, the key-masked attention,
+    the out-projection.  Returns (in-projection-free attention output o, weights Buf or None)."""
+    p = low.p
+    D = _mha_check(a, name)
+    if x.C != a.embed_dim:
+        raise RuntimeError("%s: embed_dim %d, input has %d features" % (name, a.embed_dim, x.C))
+    qkv = PL.emit_linear(p, x, a.in_proj_weight, a.in_proj_bias, L.ACT_NONE, None, name + ".in_proj")
+    F = a.embed_dim
+    q, k, v = (PL.channel_slice(qkv, i * F, F) for i in range(3))
+    return PL.emit_attention_masked(p, q, k, v, a.num_heads, D ** -0.5, mask, name + ".attention", weights=weights)
+
+
+def _masked_pool(low, m, x, mask, name):
+    _seq3(x, name)
+    _check_mask(x, mask, name)
+    return _mark(PL.emit_masked_pool(low.p, x, mask, _MPOOL[m._method], name), squeeze=True, retargetable=True), mask
+
+
+def _learned_default(low, m, x, mask, name):
+    if mask is not None:
+        if mask.B != x.N:
+            raise RuntimeError("%s: mask batch %d, x batch %d" % (name, mask.B, x.N))
+    return _mark(PL.emit_masked_default(low.p, x, mask, m._learned_defaults, name), x, retargetable=True), mask
+
+
+def _transpose_mha(low, m, x, mask, name):
+    _seq3(x, name)
+    _check_mask(x, mask, name)
+    a = m._attention
+    _mha_check(a, name + "._attention")
+    if mask is not None:
+        mask = PL.emit_mask_force_first(low.p, mask, name + ".mask")
+    o, w = _mha(low, a, x, mask, name + "._attention", weights=True)
+    y = PL.emit_linear(low.p, o, a.out_proj.weight, a.out_proj.bias, L.ACT_NONE, None, name + "._attention.out_proj")
+    # a weak reference: the module holds its compiled plans, and a plan that held the module back would put the plan's
+    # CUDA graph in a reference cycle, freed by the garbage collector at an arbitrary moment - possibly inside another
+    # plan's graph capture, which the graph's destruction would invalidate
+    low.p.side_outputs.append((weakref.ref(m), w, (x.N, x.npos, x.npos)))
+    return _mark(y, x, retargetable=True), mask
+
+
+def _encoder(low, m, x, mask, name):
+    """nn.TransformerEncoder of post-norm layers (torch's slow path, which the reference's batch_first=False layers
+    take): x = norm1(x + out_proj(attn(x))); x = norm2(x + linear2(relu(linear1(x)))); the result is position 0."""
+    _seq3(x, name)
+    _check_mask(x, mask, name)
+    p = low.p
+    enc = m.encoder
+    layers = list(enc.layers)
+    for i, lyr in enumerate(layers):
+        lname = "%s.encoder.layers.%d" % (name, i)
+        if getattr(lyr, "norm_first", False):
+            raise NotImplementedError("%s: norm_first (pre-norm) layers are unsupported" % lname)
+        act = lyr.activation
+        if not (act is torch.nn.functional.relu or type(act).__name__ == "ReLU"):
+            raise NotImplementedError("%s: activation %s unsupported (ReLU only)" % (lname, getattr(act, "__name__", act)))
+        _mha_check(lyr.self_attn, lname + ".self_attn")
+    if mask is not None:
+        mask = PL.emit_mask_force_first(p, mask, name + ".mask")
+    for i, lyr in enumerate(layers):
+        lname = "%s.encoder.layers.%d" % (name, i)
+        a = lyr.self_attn
+        o, _ = _mha(low, a, x, mask, lname + ".self_attn", weights=False)
+        h = PL.emit_linear(p, o, a.out_proj.weight, a.out_proj.bias, L.ACT_NONE, x, lname + ".self_attn.out_proj")
+        x = PL.emit_layernorm(p, h, lyr.norm1, lname + ".norm1")
+        f = PL.emit_linear(p, x, lyr.linear1.weight, lyr.linear1.bias, L.ACT_RELU, None, lname + ".linear1")
+        h = PL.emit_linear(p, f, lyr.linear2.weight, lyr.linear2.bias, L.ACT_NONE, x, lname + ".linear2")
+        x = PL.emit_layernorm(p, h, lyr.norm2, lname + ".norm2")
+    if enc.norm is not None:
+        x = PL.emit_layernorm(p, x, enc.norm, name + ".encoder.norm")
+    first = TRef(x.buf, x.N, 1, 1, 1, x.C, Cp=x.C, ch_off=x.ch_off, row_stride=x.npos * x.row_stride)   # out[:, 0, :]
+    return _mark(first, squeeze=True), mask
+
+
+_LSTM_MAX_HIDDEN = 512       # csrc/pv_lstm.cu: one thread per hidden unit
+
+
+def _lstm(low, m, x, mask, name):
+    """LSTM.forward (:227-256): one token GEMM for the input projection of both directions ([W_ih_fwd; W_ih_rev], bias
+    b_ih + b_hh), then the recurrence of every step and direction in one launch; the output is h_n, [B, ndir * H]."""
+    _seq3(x, name)
+    _check_mask(x, mask, name)
+    r = m.lstm
+    H = r.hidden_size
+    if r.num_layers != 1 or not r.batch_first or getattr(r, "proj_size", 0) or r.mode != "LSTM":
+        raise NotImplementedError("%s: only the single-layer batch_first LSTM of the reference is supported" % name)
+    if H > _LSTM_MAX_HIDDEN:
+        raise NotImplementedError("%s: LSTM hidden_dim=%d has no recurrence kernel (at most %d)" % (
+            name, H, _LSTM_MAX_HIDDEN))
+    if r.input_size != x.C:
+        raise RuntimeError("%s: LSTM dim_in %d, input has %d features" % (name, r.input_size, x.C))
+    p = low.p
+    sfx = ["", "_reverse"][:2 if r.bidirectional else 1]
+    nd = len(sfx)
+
+    def par(n, s_):
+        t = getattr(r, n + "_l0" + s_, None)
+        return None if t is None else t.detach().float().cpu()
+    w_ih = torch.cat([par("weight_ih", s_) for s_ in sfx], 0)
+    bias = None
+    if r.bias:
+        bias = torch.cat([par("bias_ih", s_) + par("bias_hh", s_) for s_ in sfx], 0)
+    g = PL.emit_linear(p, x, w_ih, bias, L.ACT_NONE, None, name + ".lstm.input_proj")
+    w_hh_t = p.const(torch.stack([par("weight_hh", s_).t().contiguous() for s_ in sfx], 0))   # [dir][H][4H]
+    y = PL._tok(p, x.N, 1, nd * H)
+    lib = p.lib
+    B, T = x.N, x.npos
+
+    def fn(stream):
+        L.check(lib.pv_lstm_recurrence(g.ptr(), g.dt, g.row_stride, w_hh_t.data_ptr(), PL._mask_ptr(mask), B, T, H, nd,
+                                       y.ptr(), y.row_stride, stream), "pv_lstm_recurrence(%s)" % name)
+    p.add(name + ".lstm.recurrence", fn, "other", 2.0 * nd * B * T * 4 * H * H, nd * 4 * H * H * 4 * T,
+          reads=(g,) + PL._mask_io(mask), writes=(y,))
+    return _mark(y, squeeze=True, retargetable=True), mask
+
+
+_MASKED_LOWERINGS = {"MaskedTemporalPooling": _masked_pool, "LearnMaskedDefault": _learned_default,
+                     "TransposeMultiheadAttention": _transpose_mha, "TransposeTransformerEncoder": _encoder,
+                     "LSTM": _lstm}
+
+
+def _lower_masked(low, m, x, mask, name):
+    n = type(m).__name__
+    if n == "MaskedSequential":
+        return _masked_sequential(low, m, x, mask, name)
+    if not _is_mask_module(m):
+        raise NotImplementedError("%s: %s takes no mask (a stream must be a MaskedSequential or a mask module)" % (name, n))
+    return _MASKED_LOWERINGS[n](low, m, x, mask, name)
+
+
+def _masked_sequential(low, m, x, mask, name):
+    # models/masked_multistream.py:338-344: mask modules get (input, mask), the others the input alone
+    for i, child in enumerate(m):
+        cname = "%s.%d" % (name, i) if name else str(i)
+        if _is_mask_module(child):
+            x, mask = _lower_masked(low, child, x, mask, cname)
+        else:
+            x = low.lower(child, x, cname)
+    return x, mask
+
+
+def _root_handler(fn):
+    def lower(self, m, x, name):
+        if type(m).__name__ != "MaskedSequential" and not _is_mask_module(m):
+            raise NotImplementedError("no B200 lowering for module %s (%s)" % (type(m).__name__, name))
+        if not isinstance(x, tuple) or len(x) != 2:
+            raise RuntimeError("%s.forward takes (x, mask)" % type(m).__name__)
+        return fn(self, m, x[0], x[1], name or ("" if type(m).__name__ == "MaskedSequential" else type(m).__name__))[0]
+    return lower
+
+
+def _lower_multipathway(self, m, x, name):
+    # models/masked_multistream.py:372-384; every stream runs on its own lane until the fusion
+    if m.multipathway_fusion is None:
+        raise RuntimeError("MaskedMultiPathWay needs a multipathway_fusion to reduce its streams")
+    outs = []
+    for i, (blk, (xi, mi)) in enumerate(zip(m.multipathway_blocks, x)):
+        self.p.lane = i
+        outs.append(_lower_masked(self, blk, xi, mi, "%s.multipathway_blocks.%d" % (name, i) if name
+                                  else "multipathway_blocks.%d" % i)[0])
+    self.p.lane = 0
+    return self.lower(m.multipathway_fusion, outs, (name + "." if name else "") + "multipathway_fusion")
+
+
+def reduce_fusion_op(reduce_fn):
+    """Classify ReduceFusion's opaque reduce_fn on a fixed CPU probe: max gives 3, sum 5, prod 6."""
+    try:
+        with torch.no_grad():
+            r = reduce_fn(torch.tensor([[2.0], [3.0]]))
+        v = float(r.reshape(-1)[0]) if torch.is_tensor(r) and r.numel() == 1 else None
+    except Exception as e:       # noqa: BLE001 - any failure means the function is not one of the three
+        raise NotImplementedError("ReduceFusion: reduce_fn is not max / sum / prod over dim 0 (%s)" % e) from None
+    op = {3.0: L.REDUCE_MAX, 5.0: L.REDUCE_SUM, 6.0: L.REDUCE_PROD}.get(v)
+    if op is None:
+        raise NotImplementedError("ReduceFusion: reduce_fn gives %r on the probe [[2], [3]]; only max (3), sum (5) and "
+                                  "prod (6) over dim 0 have a kernel" % (v,))
+    return op
+
+
+def _fusion_parts(x, name):
+    if not isinstance(x, (list, tuple)) or not x:
+        raise RuntimeError("%s: a fusion layer takes a non-empty list of tensors" % name)
+    for t in x:
+        _token_input(t, name, "fusion")
+    return list(x)
+
+
+def _concat_last(low, parts, name):
+    p0 = parts[0]
+    moved = []
+    for i, t in enumerate(parts):
+        if (t.N, t.npos) != (p0.N, p0.npos) or getattr(t, "squeeze", False) != getattr(p0, "squeeze", False):
+            raise RuntimeError("%s: inputs of different shapes" % name)
+        PL._dense8(t, name)
+        if not getattr(t, "retargetable", False) or any(t is u for u in moved):
+            c = PL._tok(low.p, t.N, t.npos, t.C)
+            PL.emit_copy_tokens(low.p, t, c, 0, "%s.copy%d" % (name, i))
+            t = _mark(c, t, retargetable=True)
+        moved.append(t)
+    return _mark(low.p.concat_channels(moved), p0) if len(moved) > 1 else moved[0]
+
+
+def _lower_concat_fusion(self, m, x, name):
+    # layers/fusion.py:46-74, torch.cat(input_list, dim=-1): the producers write channel slices of one buffer
+    return _concat_last(self, _fusion_parts(x, name or "fusion"), name or "fusion")
+
+
+def _lower_temporal_concat_fusion(self, m, x, name):
+    # layers/fusion.py:77-101, torch.cat(input_list, dim=1): (batch, feature) inputs concatenate their features
+    name = name or "fusion"
+    parts = _fusion_parts(x, name)
+    if all(getattr(t, "squeeze", False) for t in parts):
+        return _concat_last(self, parts, name)
+    p0 = parts[0]
+    for t in parts:
+        if t.N != p0.N or t.C != p0.C or getattr(t, "squeeze", False):
+            raise RuntimeError("%s: inputs of different batch / feature sizes" % name)
+        PL._dense8(t, name)
+    y = PL._tok(self.p, p0.N, sum(t.npos for t in parts), p0.C)
+    row = 0
+    for i, t in enumerate(parts):
+        PL.emit_copy_tokens(self.p, t, y, row, "%s.copy%d" % (name, i))
+        row += t.npos
+    return _mark(y, retargetable=True)
+
+
+def _lower_reduce_fusion(self, m, x, name):
+    # layers/fusion.py:104-141, reduce_fn(torch.stack(input_list)) for max / sum / prod over dim 0
+    name = name or "fusion"
+    op = reduce_fusion_op(m.reduce_fn)
+    parts = _fusion_parts(x, name)
+    for t in parts:
+        if getattr(t, "squeeze", False) != getattr(parts[0], "squeeze", False):
+            raise RuntimeError("%s: inputs of different shapes" % name)
+    return _mark(PL.emit_reduce_fusion(self.p, parts, op, name), parts[0], retargetable=True)
+
+
+def _lower_layernorm(self, m, x, name):
+    name = name or "layernorm"
+    _token_input(x, name, "LayerNorm")
+    if tuple(m.normalized_shape) != (x.C,):
+        raise RuntimeError("%s: normalized_shape %s, input has %d features" % (name, tuple(m.normalized_shape), x.C))
+    if m.weight is None or m.bias is None:
+        raise NotImplementedError("%s: LayerNorm without an elementwise affine weight and bias is unsupported" % name)
+    PL._dense8(x, name)
+    return _mark(PL.emit_layernorm(self.p, x, m, name), x, retargetable=True)
+
+
+def _lower_linear(self, m, x, name):
+    name = name or "linear"
+    _token_input(x, name, "Linear")
+    if m.in_features != x.C:
+        raise RuntimeError("%s: in_features %d, input has %d features" % (name, m.in_features, x.C))
+    return _mark(PL.emit_linear(self.p, x, m.weight, m.bias, L.ACT_NONE, None, name), x, retargetable=True)
+
+
+def _lower_positional_encoding(self, m, x, name):
+    name = name or "positional_encoding"
+    _token_input(x, name, "PositionalEncoding")
+    _seq3(x, name)
+    if m.pe.size(1) < x.npos:
+        raise RuntimeError("Cannot apply position encoding of size %s when input has %d positions" % (
+            tuple(m.pe.size()), x.npos))
+    if m.pe.size(2) != x.C:
+        raise RuntimeError("%s: embed_dim %d, input has %d features" % (name, m.pe.size(2), x.C))
+    PL._dense8(x, name)
+    return _mark(PL.emit_pos_cls(self.p, x, m.pe[0, :x.npos].detach().float().cpu(), False, name), x)
+
+
+for _n, _fn in _MASKED_LOWERINGS.items():
+    setattr(Lowering, "lower_" + _n, _root_handler(_fn))
+Lowering.lower_MaskedSequential = _root_handler(_masked_sequential)
+Lowering.lower_MaskedMultiPathWay = _lower_multipathway
+Lowering.lower_ConcatFusion = _lower_concat_fusion
+Lowering.lower_TemporalConcatFusion = _lower_temporal_concat_fusion
+Lowering.lower_ReduceFusion = _lower_reduce_fusion
+Lowering.lower_LayerNorm = _lower_layernorm
+Lowering.lower_Linear = _lower_linear
+Lowering.lower_PositionalEncoding = _lower_positional_encoding

@@ -15,8 +15,8 @@ import torch
 from .. import _lib as L
 from . import packing as PK
 
-_TORCH_DT = {L.PV_F16: torch.float16, L.PV_F32: torch.float32}
-_ESIZE = {L.PV_F16: 2, L.PV_F32: 4}
+_TORCH_DT = {L.PV_F16: torch.float16, L.PV_F32: torch.float32, L.PV_U8: torch.uint8}
+_ESIZE = {L.PV_F16: 2, L.PV_F32: 4, L.PV_U8: 1}
 
 
 class Buf:
@@ -31,6 +31,20 @@ class RawIn:
 
     def __init__(self, tensor):
         self.tensor = tensor
+
+
+class MaskRef:
+    """A (B, T) u8 mask of a plan (non-zero = valid step): the staged plan input (``tensor``) or a plan buffer."""
+
+    def __init__(self, B, T, tensor=None, buf=None):
+        self.B, self.T = int(B), int(T)
+        self.tensor, self.buf = tensor, buf
+
+    def ptr(self):
+        return (self.tensor if self.tensor is not None else self.buf.tensor).data_ptr()
+
+    def io(self):
+        return (self.buf,) if self.buf is not None else ()
 
 
 class TRef:
@@ -81,6 +95,7 @@ class Plan:
         self.ops = []          # (name, closure(stream_ptr))
         self.meta = []         # per-op {name, kind, flops, bytes} (algorithmic figures for the roofline)
         self.attention_calls = []   # per attention op: its problem (B, H, Nq, Nk, D, scale, normalize, residual)
+        self.side_outputs = []      # (weakref to module, Buf, shape): per-module results besides the output (attention weights)
         self.bufs = []
         self.consts = []       # keep device parameter tensors alive
         self.zero_bufs = []    # f32 accumulators that must be cleared every run (SE sums)
@@ -752,13 +767,13 @@ def emit_layernorm(plan, x, ln, name="ln", rows_stride=None, rows=None):
         def fn32(stream):
             L.check(lib.pv_add_layernorm(x.ptr(), x.dt, xs, None, 0, None, 0, y.ptr(), y.row_stride, n_rows, C,
                                          g.data_ptr(), b.data_ptr(), eps, stream), "pv_add_layernorm(%s)" % name)
-        plan.add(name, fn32, "other", 0.0, n_rows * C * 6)
+        plan.add(name, fn32, "other", 0.0, n_rows * C * 6, reads=(x,), writes=(y,))
         return y
 
     def fn(stream):
         L.check(lib.pv_layernorm(x.ptr(), y.ptr(), x.dt, n_rows, 1, C, xs, y.row_stride, g.data_ptr(), b.data_ptr(),
                                  eps, stream), "pv_layernorm(%s)" % name)
-    plan.add(name, fn, "other", 0.0, n_rows * C * 4)
+    plan.add(name, fn, "other", 0.0, n_rows * C * 4, reads=(x,), writes=(y,))
     return y
 
 
@@ -803,7 +818,7 @@ def emit_pos_cls(plan, x, pos_table, has_cls, name="posenc", out_dt=None):
     def fn(stream):
         L.check(lib.pv_add_pos_cls_to(x.ptr(), x.dt, y.ptr(), y.dt, x.N, n_patch, C, x.row_stride, pos.data_ptr(),
                                       1 if has_cls else 0, stream), "pv_add_pos_cls_to")
-    plan.add(name, fn, "other", 0.0, x.N * n_patch * C * (_ESIZE[x.dt] + _ESIZE[y.dt]))
+    plan.add(name, fn, "other", 0.0, x.N * n_patch * C * (_ESIZE[x.dt] + _ESIZE[y.dt]), reads=(x,), writes=(y,))
     return y
 
 
@@ -963,3 +978,143 @@ def channel_slice(x, off, C):
     """View of C channels starting at `off` (no copy)."""
     t = TRef(x.buf, x.N, x.T, x.H, x.W, C, Cp=C, ch_off=x.ch_off + off, row_stride=x.row_stride)
     return t
+
+
+# =============================================================================================
+# Masked sequence ops (models/masked_multistream.py, layers/fusion.py).  Token tensors [B, T, C] with C % 8 == 0;
+# masks are MaskRefs or None (every step valid).
+# =============================================================================================
+def _mask_ptr(mask):
+    return mask.ptr() if mask is not None else None
+
+
+def _mask_io(mask):
+    return mask.io() if mask is not None else ()
+
+
+def _dense8(x, what):
+    if x.C % 8 or x.Cp != x.C:
+        raise NotImplementedError("%s: feature width %d is not a multiple of 8" % (what, x.C))
+
+
+def emit_mask_force_first(plan, mask, name="mask_force_first"):
+    """mask[:, 0] = True (models/masked_multistream.py:137-141, :309-313) on a copy owned by the plan."""
+    out = MaskRef(mask.B, mask.T, buf=plan.new_buf(mask.B * mask.T, L.PV_U8))
+    lib = plan.lib
+
+    def fn(stream):
+        L.check(lib.pv_mask_force_first(mask.ptr(), out.ptr(), mask.B, mask.T, stream), "pv_mask_force_first(%s)" % name)
+    plan.add(name, fn, "other", 0.0, 2 * mask.B * mask.T, reads=mask.io(), writes=out.io())
+    return out
+
+
+def emit_masked_pool(plan, x, mask, mode, name="masked_pool"):
+    """MaskedTemporalPooling (:35-93): [B, T, C] -> [B, C] (a token tensor of one position)."""
+    _dense8(x, name)
+    y = _tok(plan, x.N, 1, x.C)
+    lib = plan.lib
+    B, T, Cc = x.N, x.npos, x.C
+
+    def fn(stream):
+        L.check(lib.pv_masked_pool(x.ptr(), x.dt, x.row_stride, B, T, Cc, _mask_ptr(mask), mode, y.ptr(), y.row_stride,
+                                   stream), "pv_masked_pool(%s)" % name)
+    plan.add(name, fn, "other", 0.0, (B * T + B) * Cc * _ESIZE[x.dt], reads=(x,) + _mask_io(mask), writes=(y,))
+    return y
+
+
+def emit_masked_default(plan, x, mask, default, name="learned_default"):
+    """LearnMaskedDefault (:170-190) on [B, C]."""
+    _dense8(x, name)
+    if x.npos != 1:
+        raise NotImplementedError("%s: LearnMaskedDefault on a (batch, seq_len, feature) tensor is unsupported" % name)
+    if mask is None:
+        raise RuntimeError("%s: LearnMaskedDefault needs a mask" % name)
+    d = plan.const(default.detach().float().cpu().reshape(-1))
+    if d.numel() != x.C:
+        raise RuntimeError("%s: default of %d values for %d features" % (name, d.numel(), x.C))
+    y = _tok(plan, x.N, 1, x.C)
+    lib = plan.lib
+
+    def fn(stream):
+        L.check(lib.pv_masked_default(x.ptr(), x.dt, x.row_stride, x.N, x.C, mask.ptr(), mask.T, d.data_ptr(), y.ptr(),
+                                      y.row_stride, stream), "pv_masked_default(%s)" % name)
+    plan.add(name, fn, "other", 0.0, 2 * x.N * x.C * _ESIZE[x.dt], reads=(x,) + mask.io(), writes=(y,))
+    return y
+
+
+def emit_reduce_fusion(plan, parts, op, name="reduce_fusion"):
+    """ReduceFusion (layers/fusion.py:104-141): elementwise max / sum / prod over P same-shaped token tensors."""
+    p0 = parts[0]
+    if len(parts) > 8:
+        raise NotImplementedError("%s: %d inputs (at most 8)" % (name, len(parts)))
+    for p in parts:
+        _dense8(p, name)
+        if (p.N, p.npos, p.C) != (p0.N, p0.npos, p0.C):
+            raise RuntimeError("%s: inputs of different shapes" % name)
+    y = _tok(plan, p0.N, p0.npos, p0.C)
+    lib = plan.lib
+    P = len(parts)
+    ptrs, strides = (C.c_void_p * P)(), (C.c_longlong * P)()
+
+    def fn(stream):
+        for i, p in enumerate(parts):
+            ptrs[i], strides[i] = p.ptr(), p.row_stride
+        L.check(lib.pv_reduce_fusion(ptrs, strides, P, p0.dt, p0.N * p0.npos, p0.C, op, y.ptr(), y.row_stride, stream),
+                "pv_reduce_fusion(%s)" % name)
+    plan.add(name, fn, "other", 0.0, (P + 1) * p0.N * p0.npos * p0.C * _ESIZE[p0.dt], reads=tuple(parts), writes=(y,))
+    return y
+
+
+def emit_copy_tokens(plan, x, y, row0, name="copy_tokens"):
+    """y[b, row0 + i, :] = x[b, i, :] (the row-slice writes of TemporalConcatFusion)."""
+    lib = plan.lib
+
+    def fn(stream):
+        esz = _ESIZE[x.dt]
+        if x.row_stride == x.C and y.row_stride == y.C:
+            # dense rows: every sample's rows are one contiguous span, one launch for all samples
+            L.check(lib.pv_copy_rows(x.ptr(), y.ptr() + row0 * y.row_stride * esz, x.dt, x.N, x.npos * x.C,
+                                     x.npos * x.C, y.npos * y.C, stream), "pv_copy_rows(%s)" % name)
+            return
+        for b in range(x.N):
+            L.check(lib.pv_copy_rows(x.ptr() + b * x.npos * x.row_stride * esz,
+                                     y.ptr() + (b * y.npos + row0) * y.row_stride * esz, x.dt, x.npos, x.C,
+                                     x.row_stride, y.row_stride, stream), "pv_copy_rows(%s)" % name)
+    plan.add(name, fn, "other", 0.0, 2 * x.N * x.npos * x.C * _ESIZE[x.dt], reads=(x,), writes=(y,))
+
+
+def emit_attention_masked(plan, q, k, v, heads, scale, mask, name="attn", weights=False):
+    """Key-masked softmax attention (pv_attention_masked_fwd) on token tensors; with ``weights`` also the head-averaged
+    fp32 softmax [B, Nq, Nk] (pv_attention_weights).  mask None: every key valid.  Returns (o, weights Buf or None)."""
+    import ctypes as C_
+    B, Nq, Nk, dim = q.N, q.npos, k.npos, q.C
+    assert k.C == dim and v.C == dim and v.npos == Nk and dim % heads == 0
+    if mask is None:
+        mask = MaskRef(B, Nk, tensor=plan.const(torch.ones(B, Nk, dtype=torch.uint8)))
+    o = _tok(plan, B, Nq, dim)
+    d = L.AttentionDesc()
+    d.dtype, d.B, d.H, d.Nq, d.Nk, d.D = plan.dt, B, heads, Nq, Nk, dim // heads
+    d.scale, d.add_q_residual, d.normalize = float(scale), 0, 0
+    lse = plan.new_buf(B * heads * Nq, L.PV_F32) if weights else None
+    w = plan.new_buf(B * Nq * Nk, L.PV_F32) if weights else None
+    lib = plan.lib
+
+    def fn(stream):
+        d.q_row_stride, d.k_row_stride, d.v_row_stride, d.o_row_stride = q.row_stride, k.row_stride, v.row_stride, o.row_stride
+        d.q_batch_stride, d.k_batch_stride = Nq * q.row_stride, Nk * k.row_stride
+        d.v_batch_stride, d.o_batch_stride = Nk * v.row_stride, Nq * o.row_stride
+        L.check(lib.pv_attention_masked_fwd(C_.byref(d), q.ptr(), k.ptr(), v.ptr(), o.ptr(), mask.ptr(),
+                                            lse.tensor.data_ptr() if lse is not None else None, stream),
+                "pv_attention_masked_fwd(%s)" % name)
+    plan.add(name, fn, "attention", 4.0 * B * heads * Nq * Nk * (dim // heads),
+             (B * Nq * dim * 2 + 2 * B * Nk * dim) * _ESIZE[plan.dt], reads=(q, k, v) + mask.io(),
+             writes=(o,) + ((lse,) if lse is not None else ()))
+    plan.attention_calls.append({"name": name, "B": B, "H": heads, "Nq": Nq, "Nk": Nk, "D": dim // heads,
+                                 "scale": d.scale, "normalize": 0, "add_q_residual": 0, "masked": True})
+    if weights:
+        def fn_w(stream):
+            L.check(lib.pv_attention_weights(C_.byref(d), q.ptr(), k.ptr(), mask.ptr(), lse.tensor.data_ptr(),
+                                             w.tensor.data_ptr(), stream), "pv_attention_weights(%s)" % name)
+        plan.add(name + ".weights", fn_w, "other", 2.0 * B * heads * Nq * Nk * (dim // heads), B * Nq * Nk * 4,
+                 reads=(q, k, lse) + mask.io(), writes=(w,))
+    return o, w

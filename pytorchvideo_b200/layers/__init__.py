@@ -5,3 +5,5 @@ from .utils import round_repeats, round_width, set_attributes  # noqa: F401
 from .drop_path import DropPath  # noqa: F401
 from .attention import Mlp, MultiScaleAttention, MultiScaleBlock  # noqa: F401,E402
 from .positional_encoding import SpatioTemporalClsPositionalEncoding  # noqa: F401,E402
+from .positional_encoding import PositionalEncoding  # noqa: F401,E402
+from .fusion import ConcatFusion, ReduceFusion, TemporalConcatFusion, make_fusion_layer  # noqa: F401,E402

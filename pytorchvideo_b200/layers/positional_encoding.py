@@ -1,11 +1,28 @@
-"""cls token + separable spatio-temporal positional encoding container
-(reference layers/positional_encoding.py:47-136)."""
+"""Positional encodings: the sinusoidal ``PositionalEncoding`` (reference layers/positional_encoding.py:11-44) and the
+cls token + separable spatio-temporal positional encoding container (:47-136)."""
+import math
 from typing import Tuple
 
 import torch
 import torch.nn as nn
 
 from ..module import B200Module
+
+
+class PositionalEncoding(B200Module):
+    """x + pe[:, :seq_len, :] on (batch_size, seq_len, embed_dim) tokens, PE(pos, 2i) = sin(pos / 10000^(2i/d)),
+    PE(pos, 2i+1) = cos(...); the ``pe`` buffer is built as the reference builds it.  On device one add launch
+    (pv_add_pos_cls without a cls token)."""
+
+    def __init__(self, embed_dim: int, seq_len: int = 1024) -> None:
+        super().__init__()
+        pe = torch.zeros(seq_len, embed_dim, dtype=torch.float)
+        position = torch.arange(0, seq_len, dtype=torch.float).unsqueeze(1)
+        div_term = torch.exp(torch.arange(0, embed_dim, 2).float() * (-(math.log(10000.0)) / embed_dim))
+        pe[:, 0::2] = torch.sin(position * div_term)
+        pe[:, 1::2] = torch.cos(position * div_term)
+        pe = pe.unsqueeze(0)
+        self.register_buffer("pe", pe)
 
 
 class SpatioTemporalClsPositionalEncoding(B200Module):

@@ -14,3 +14,5 @@ from .x3d import (ProjectedPool, create_x3d, create_x3d_bottleneck_block, create
 from .head import SequencePool, VisionTransformerBasicHead, create_vit_basic_head  # noqa: F401,E402
 from .stem import PatchEmbed, create_conv_patch_embed  # noqa: F401,E402
 from .vision_transformers import MultiscaleVisionTransformers, create_multiscale_vision_transformers  # noqa: F401,E402
+from .masked_multistream import (LSTM, LearnMaskedDefault, MaskedMultiPathWay, MaskedSequential,  # noqa: F401,E402
+                                 MaskedTemporalPooling, TransposeMultiheadAttention, TransposeTransformerEncoder)

@@ -441,3 +441,84 @@ def build_audio_case(name, builders, seed=2024):
         g.manual_seed(seed + 3)
         x = torch.randn(spec[1], generator=g)
     return m, x
+
+
+# ---- masked multistream cases (tests/golden/masked.pt): models/masked_multistream.py, layers/fusion.py --------------
+# Every case runs at B = 5 (not a multiple of 8) on MASKED_MASK: ragged prefixes, a full row, a non-prefix pattern and
+# a row with no valid step; "*_t1" cases run T = 1.  Feature widths are multiples of 8 (f16 token rows).
+MASKED_MASK = [[1, 1, 1, 0, 0, 0, 0], [1, 1, 1, 1, 1, 1, 1], [0, 1, 0, 1, 1, 0, 0], [0, 0, 0, 0, 0, 0, 0],
+               [1, 1, 1, 1, 1, 0, 0]]
+MASKED_FUSIONS = ("concat", "temporal_concat", "max", "sum", "prod")
+MASKED_CASES = tuple(["pool_max", "pool_avg", "pool_sum", "pool_avg_nomask", "pool_max_t1", "default", "posenc", "mha",
+                      "mha_nomask", "mha_d32_t1", "mha_d128", "chain", "encoder_1", "encoder_2", "encoder_nomask",
+                      "lstm_uni", "lstm_bi", "lstm_bi_t1", "lstm_nomask"] +
+                     ["multipath_" + f for f in MASKED_FUSIONS])
+
+
+def masked_case_inputs(name, seed=7):
+    """(x, mask or None) of a case; x is (B, T, F), or (B, F) for "default"."""
+    g = torch.Generator().manual_seed(seed)
+    F = {"mha_d32_t1": 32, "mha_d128": 128}.get(name, 64)
+    mask = torch.tensor(MASKED_MASK, dtype=torch.bool)
+    if name.endswith("_t1"):
+        mask = mask[:, :1]
+    B, T = mask.shape
+    x = torch.randn(B, F, generator=g) if name == "default" else torch.randn(B, T, F, generator=g)
+    return x, (None if name.endswith("nomask") or name == "posenc" else mask)
+
+
+def build_masked_case(name, ns, seed=1234):
+    """The case's module tree built from ``ns``, a namespace with the masked_multistream classes, ``PositionalEncoding``
+    and ``make_fusion_layer`` (this package's or the reference's), with seeded parameters; eval mode."""
+    torch.manual_seed(seed)
+    F = {"mha_d32_t1": 32, "mha_d128": 128}.get(name, 64)
+    if name.startswith("pool_"):
+        m = ns.MaskedTemporalPooling(name.split("_")[1])
+    elif name == "default":
+        m = ns.LearnMaskedDefault(F)
+    elif name == "posenc":
+        m = ns.PositionalEncoding(F, seq_len=16)
+    elif name.startswith("mha"):
+        m = ns.TransposeMultiheadAttention(F, {"mha_d32_t1": 1, "mha_d128": 1}.get(name, 2))
+    elif name == "chain":       # the usage example of models/masked_multistream.py:17-32
+        m = ns.MaskedSequential(ns.PositionalEncoding(F), torch.nn.Dropout(p=0.1), ns.TransposeMultiheadAttention(F, 2),
+                                ns.MaskedTemporalPooling(method="avg"), torch.nn.LayerNorm(F), ns.LearnMaskedDefault(F))
+    elif name.startswith("encoder"):
+        m = ns.TransposeTransformerEncoder(F, 2, 2 if name == "encoder_2" else 1)
+    elif name.startswith("lstm"):
+        m = ns.LSTM(F, 48 if name == "lstm_uni" else 32, bidirectional=name != "lstm_uni")
+    elif name.startswith("multipath_"):
+        m = ns.MaskedMultiPathWay(multipathway_blocks=torch.nn.ModuleList([
+            ns.MaskedSequential(ns.TransposeMultiheadAttention(F, 2), ns.MaskedTemporalPooling("avg"),
+                                ns.LearnMaskedDefault(F)),
+            ns.MaskedSequential(torch.nn.Linear(F, F), ns.LSTM(F, F // 2, bidirectional=True), torch.nn.LayerNorm(F))]),
+            multipathway_fusion=ns.make_fusion_layer(name[len("multipath_"):], [F, F]))
+    else:
+        raise KeyError(name)
+    with torch.no_grad():
+        for p in m.parameters():
+            p.copy_(torch.randn(p.shape) * (0.5 / max(1, p.shape[-1]) ** 0.5 if p.dim() > 1 else 0.2))
+    return m.eval()
+
+
+def masked_engine_args(name, x, mask):
+    """(inputs, extra) of a case as the masked modules hand them to the engine (engine/lower.py ``lower_only``)."""
+    if name == "posenc":
+        return x, ()
+    multi = name.startswith("multipath_")
+    has = mask is not None
+    ins = ([x, mask] if has else [x]) * (2 if multi else 1)
+    return ins, (("masks", multi) + (has,) * (2 if multi else 1),)
+
+
+def masked_call(m, x, mask):
+    """The reference's calling convention of a case's root module.  Each stream gets a mask object of its own: the
+    reference's attention modules write mask[:, 0] = True into the object they receive, which would leak into the
+    other streams through a shared one."""
+    if type(m).__name__ == "MaskedMultiPathWay":
+        return m([(x, None if mask is None else mask.clone()), (x, None if mask is None else mask.clone())])
+    if type(m).__name__ == "MaskedSequential":
+        return m(input=x, mask=mask)
+    if type(m).__name__ == "PositionalEncoding":
+        return m(x)
+    return m(x, mask)
