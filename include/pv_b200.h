@@ -340,6 +340,14 @@ int pv_conv3d_stem_rows_supported(const pv_conv3d_desc* d);
 int pv_conv3d_stem_rows_fwd(const pv_conv3d_desc* d, const void* x, const void* w, const float* scale,
                             const float* bias, const void* zero_row, void* y, void* stream);
 
+/* Temporal-streaming stem (the SlowFast Fast stem, csrc/pv_stem_stream.cu): the stem-rows input and descriptor
+ * conventions, with kt = 5 temporal taps at stride / dilation 1 (pt < kt), Co = 8, window 32 and no addend.  One pass
+ * over the input frames: all 5 taps in one wgmma (N = 40) per frame, summed in fp32 registers, rounded to f16 once.
+ * w: f16 [kh * 32 / 8][40][8], column 8 j + c = temporal tap j of output channel c;  zero_row: >= 4 KiB of zeros. */
+int pv_conv3d_stem_stream_supported(const pv_conv3d_desc* d);
+int pv_conv3d_stem_stream_fwd(const pv_conv3d_desc* d, const void* x, const void* w, const float* scale,
+                              const float* bias, const void* zero_row, void* y, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Fused bottleneck block for narrow pathways (SlowFast Fast pathway), ONE launch:
  *   a = relu(bn_a(conv_a(x)))  (kt,1,1) C_in -> C_mid;   b = relu(bn_b(conv_b(a)))  (1,3,3) stride (1,sb,sb), pad 1

@@ -140,6 +140,8 @@ SIGNATURES = {
     "pv_conv3d_group_span": (C.c_int, [C.POINTER(Conv3dDesc), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "pv_conv3d_stem_rows_supported": (C.c_int, [C.POINTER(Conv3dDesc)]),
     "pv_conv3d_stem_rows_fwd": (C.c_int, [C.POINTER(Conv3dDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_conv3d_stem_stream_supported": (C.c_int, [C.POINTER(Conv3dDesc)]),
+    "pv_conv3d_stem_stream_fwd": (C.c_int, [C.POINTER(Conv3dDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_bottleneck_fused_supported": (C.c_int, [C.POINTER(BottleneckDesc)]),
     "pv_bottleneck_fused_fwd": (C.c_int, [C.POINTER(BottleneckDesc)] + [c_vp] * 15),
     "pv_bottleneck_fused_tiling": (C.c_int, [C.POINTER(BottleneckDesc), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),

@@ -87,6 +87,12 @@ __device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
 }
 
 // ---- TMA ------------------------------------------------------------------------------------
+// non-tensor bulk copy of `bytes` (a multiple of 16) from global to shared memory, completing on mbarrier `bar`
+__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
+               "l"(src), "r"(bytes), "r"(bar)
+               : "memory");
+}
 __device__ __forceinline__ void prefetch_tmap(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
 }

@@ -51,11 +51,6 @@ struct StemParams {
   EpiParams epi;
 };
 
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-               "l"(src), "r"(bytes), "r"(bar)
-               : "memory");
-}
 // no-swizzle K-major descriptor: LBO = bytes between 16-byte K chunks, SBO = bytes between 8-row groups
 template <int BN, int KS>   // KS = win / 16: k16 steps per filter row
 __global__ void __launch_bounds__(ST_THREADS, 1)

@@ -30,6 +30,18 @@ template <int TRANS_B> struct Wgmma<32, TRANS_B> {
   }
 };
 
+// N = 40: the five temporal taps x 8 channels of the streaming stem (pv_stem_stream.cu)
+template <int TRANS_B> struct Wgmma<40, TRANS_B> {
+  static constexpr int REGS = 20;
+  static __device__ __forceinline__ void mma(float (&d)[20], uint64_t a, uint64_t b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %22, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n40k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19}, %20, %21, p, 1, 1, 0, %23;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
+        : "l"(a), "l"(b), "r"(accumulate), "n"(TRANS_B));
+  }
+};
+
 template <int TRANS_B> struct Wgmma<64, TRANS_B> {
   static constexpr int REGS = 32;
   static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b, uint32_t accumulate) {

@@ -150,3 +150,18 @@ def pack_stem_rows(w, ci_pad, co_pad, lead=0):
     full = torch.zeros(n16, k, dtype=torch.float16)
     full[:co_pad] = rows
     return full.reshape(n16, k // 8, 8).permute(1, 0, 2).contiguous()
+
+
+def pack_stem_stream(w, ci_pad, co_pad, lead=0):
+    """Temporal-streaming stem (csrc/pv_stem_stream.cu): [Co, Ci, kt, kh, kw] -> f16 [K / 8][kt * co_pad][8] with
+    K = kh * win.  The layout of ``pack_stem_rows`` for the (1, kh, kw) filter of every temporal tap side by side:
+    column j * co_pad + c holds tap j of output channel c (no padding of the kt * co_pad columns to 16)."""
+    co, ci, kt, kh, kw = w.shape
+    n = kt * co_pad
+    taps = torch.zeros(n, ci, 1, kh, kw, dtype=w.dtype)
+    src = w.detach().cpu()
+    for j in range(kt):
+        taps[j * co_pad: j * co_pad + co] = src[:, :, j:j + 1]
+    rows = pack_dense_window(taps, ci_pad, n, lead)               # [n, K]
+    k = rows.shape[1]
+    return rows.reshape(n, k // 8, 8).permute(1, 0, 2).contiguous()

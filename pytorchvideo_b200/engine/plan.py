@@ -17,6 +17,9 @@ from . import packing as PK
 
 _TORCH_DT = {L.PV_F16: torch.float16, L.PV_F32: torch.float32, L.PV_U8: torch.uint8}
 _ESIZE = {L.PV_F16: 2, L.PV_F32: 4, L.PV_U8: 1}
+# SM count of the H100 SXM: routing thresholds that count waves of work.  Lowering runs without a device, so the plan
+# (and the goldens that pin it) must not depend on the GPU it is built on.
+H100_SXM_SMS = 132
 
 
 class Buf:
@@ -360,30 +363,43 @@ class Plan:
                                       addend=addend, folded=folded)
         if residual is not None:
             self.materialize_input(residual)
-        # ---- narrow stems with a temporal extent: factor (kt,kh,kw) -> (1,kh,kw) with kt*Co channels
-        #      (all temporal taps in one tensor-core pass) + a temporal tap sum, see pv_temporal_tap_sum
-        if (x.lazy_src is not None and self.use_tcgen05 and force_algo in (None, L.ALGO_TCGEN05) and groups == 1
-                and x.Cp == 4 and kt > 1 and residual is None and addend is None and co_pad * kt <= 256 and dlw == 1
-                and (sw * x.Cp * 2) % 16 == 0 and kw * x.Cp <= 64 and pw > 0 and sh <= 8):
+        esz = _ESIZE[self.dt]
+        m_out = x.N * To * Ho * Wo
+        flops = 2.0 * m_out * co * cig * kt * kh * kw
+        nbytes = (x.N * x.npos * ci + m_out * co * (2 if residual is not None else 1)) * esz + weight.numel() * esz
+        stem_candidate = (x.lazy_src is not None and self.use_tcgen05 and force_algo in (None, L.ALGO_TCGEN05)
+                          and groups == 1 and x.Cp == 4 and kt > 1 and residual is None and addend is None and dlw == 1
+                          and pw > 0)
+        # Narrow stems with a temporal extent run as two launches, `.taps` (the convolution's tensor-core pass) and
+        # `.tapsum` (pv_temporal_tap_sum: folded BN, activation), on one of two routes:
+        # ---- at least one full wave of output rows: the streaming stem (csrc/pv_stem_stream.cu) walks every output
+        #      row over all input frames and sums the kt temporal taps in fp32 registers, so `.taps` writes the Co
+        #      channels of the pre-BN sum once (rounded to f16 once); `.tapsum` is then the BN / activation pass over
+        #      it (one tap).  With fewer rows than SMs the factored route fills the machine better (its taps pass has
+        #      kt times more tiles).  PVB200_NO_STEMSTREAM: the factored route at every size, for A/B runs.
+        if (stem_candidate and x.N * Ho * -(-Wo // 128) >= H100_SXM_SMS
+                and not os.environ.get("PVB200_NO_STEMSTREAM")):
+            wp, w_phys, lead, win = self._stem_window(x, kw, sw, pw, Wo)
+            d = self._conv_desc(x, (To, Ho, Wo), co_pad, (kt, kh, kw), stride, padding, dilation, 1, L.ACT_NONE, None,
+                                co_pad, win)
+            d.x_w_pad, d.x_w_phys = wp, w_phys
+            if self.lib.pv_conv3d_stem_stream_supported(C.byref(d)):
+                ysum = self._emit_stem_stream(x, d, weight, co, lead, name + ".taps", flops, nbytes)
+                return self._emit_tap_sum(ysum, To, To, co, 1, 1, 0, 1, conv_bias, bn, act, name)
+        # ---- factor (kt,kh,kw) -> (1,kh,kw) with kt*Co channels (all temporal taps in one tensor-core pass, each
+        #      tap's partial rounded to f16 and written out) + the temporal tap sum.  Only below 16 output channels:
+        #      from there the direct convolution is already a full wgmma width and writes no kt-fold intermediate
+        #      (CSN's 3x7x7 3->64 stem at batch 8: 0.96 ms direct, 2.10 ms factored, DESIGN.md).
+        #      PVB200_NO_STEMFACTOR: the direct stem-rows convolution for every shape, for A/B runs.
+        if (stem_candidate and co_pad < 16 and co_pad * kt <= 256 and (sw * x.Cp * 2) % 16 == 0 and kw * x.Cp <= 64 and sh <= 8
+                and not os.environ.get("PVB200_NO_STEMFACTOR")):
             w2 = torch.zeros(kt * co_pad, cig, 1, kh, kw, dtype=weight.dtype)
             wsrc = weight.detach().cpu()
             for j in range(kt):
                 w2[j * co_pad: j * co_pad + co] = wsrc[:, :, j:j + 1]
             yk = self.emit_conv(x, w2, None, None, (1, sh, sw), (0, ph, pw), (1, dlh, dlw), 1, L.ACT_NONE, None,
                                 name + ".taps")
-            y = self.new_tensor(x.N, To, Ho, Wo, co, Cp=co_pad)
-            scale, bias = PK.fold_bn(conv_bias, bn, co, co_pad)
-            scale_d, bias_d = self.const(scale), self.const(bias)
-            lib = self.lib
-            hw = Ho * Wo
-
-            def fn_sum(stream):
-                L.check(lib.pv_temporal_tap_sum(yk.ptr(), y.ptr(), self.dt, x.N, x.T, To, hw, co_pad, kt, st, pt, dlt,
-                                                scale_d.data_ptr(), bias_d.data_ptr(), act, yk.row_stride,
-                                                y.row_stride, stream), "pv_temporal_tap_sum(%s)" % name)
-            self.add(name + ".tapsum", fn_sum, "other", 0.0, (x.N * x.T * hw * kt * co_pad + x.N * To * hw * co_pad) * 2,
-                     reads=(yk,), writes=(y,))
-            return y
+            return self._emit_tap_sum(yk, x.T, To, co, kt, st, pt, dlt, conv_bias, bn, act, name)
         # ---- network input: pick the layout its first consumer wants
         window = False
         if x.lazy_src is not None:
@@ -391,11 +407,8 @@ class Plan:
                       and dlw == 1 and (sw * x.Cp * 2) % 16 == 0 and (kw + 1) * x.Cp <= 64 and kt * kh <= 64
                       and st * sh <= 8 and pw > 0)
             if window:
-                wp = (pw + 3) // 4 * 4          # left pad rounded up: enables the 4-pixel conversion kernel
-                lead = PK.window_lead(wp, pw, x.Cp)
-                win = PK.window_elems(kw, x.Cp, lead)
-                need = wp - pw + max(x.W + 2 * pw, (Wo - 1) * sw + (win + x.Cp - 1) // x.Cp)
-                self.materialize_input(x, w_pad=wp, w_phys=(need + 3) // 4 * 4)
+                wp, w_phys, _, _ = self._stem_window(x, kw, sw, pw, Wo)
+                self.materialize_input(x, w_pad=wp, w_phys=w_phys)
             else:
                 self.materialize_input(x)
         elif x.padw is not None:
@@ -490,10 +503,6 @@ class Plan:
             L.check(lib.pv_conv3d_fwd(C.byref(d), algo, x.ptr(), w_d.data_ptr(), scale_d.data_ptr(),
                                       bias_d.data_ptr(), residual.ptr() if residual is not None else None,
                                       y.ptr(), stream), "pv_conv3d_fwd(%s)" % name)
-        esz = _ESIZE[self.dt]
-        m_out = x.N * To * Ho * Wo
-        flops = 2.0 * m_out * co * cig * kt * kh * kw
-        nbytes = (x.N * x.npos * ci + m_out * co * (2 if residual is not None else 1)) * esz + weight.numel() * esz
         if stem_rows:
             self.stats["stem_rows"] = self.stats.get("stem_rows", 0) + 1
         self.add(name, fn_stem if stem_rows else (fn_dw if (depthwise and residual is None) else fn), kind, flops, nbytes,
@@ -501,6 +510,54 @@ class Plan:
                  writes=(y,) + ((sums,) if sums is not None else ()))
         if addend is not None:
             self.meta[-1]["addend"] = (a.buf, a_off)
+        return y
+
+    @staticmethod
+    def _stem_window(x, kw, sw, pw, Wo):
+        """(w_pad, w_phys, lead, window elements) of the physically W-padded network input a window-mode stem reads;
+        the left pad is rounded up to 4 pixels, which enables the 4-pixel conversion kernel."""
+        wp = (pw + 3) // 4 * 4
+        lead = PK.window_lead(wp, pw, x.Cp)
+        win = PK.window_elems(kw, x.Cp, lead)
+        need = wp - pw + max(x.W + 2 * pw, (Wo - 1) * sw + (win + x.Cp - 1) // x.Cp)
+        return wp, (need + 3) // 4 * 4, lead, win
+
+    def _emit_tap_sum(self, yk, Ti, To, co, kt, st, pt, dlt, conv_bias, bn, act, name):
+        """``name``.tapsum: y = act(scale * sum over the kt channel groups of yk at frames t*st + j*dlt - pt + bias)
+        with the folded BN of the convolution (pv_temporal_tap_sum)."""
+        co_pad = PK.pad8(co)
+        y = self.new_tensor(yk.N, To, yk.H, yk.W, co, Cp=co_pad)
+        scale, bias = PK.fold_bn(conv_bias, bn, co, co_pad)
+        scale_d, bias_d = self.const(scale), self.const(bias)
+        lib = self.lib
+        hw = yk.H * yk.W
+
+        def fn_sum(stream):
+            L.check(lib.pv_temporal_tap_sum(yk.ptr(), y.ptr(), self.dt, yk.N, Ti, To, hw, co_pad, kt, st, pt, dlt,
+                                            scale_d.data_ptr(), bias_d.data_ptr(), act, yk.row_stride,
+                                            y.row_stride, stream), "pv_temporal_tap_sum(%s)" % name)
+        self.add(name + ".tapsum", fn_sum, "other", 0.0, (yk.N * Ti * hw * kt * co_pad + yk.N * To * hw * co_pad) * 2,
+                 reads=(yk,), writes=(y,))
+        return y
+
+    def _emit_stem_stream(self, x, d, weight, co, lead, name, flops, nbytes):
+        """The temporal-streaming stem (csrc/pv_stem_stream.cu) for descriptor ``d``, which the library accepted: the
+        temporal sum of the convolution, without BN (unit scale, zero bias) and activation (d.act = none)."""
+        self.materialize_input(x, w_pad=d.x_w_pad, w_phys=d.x_w_phys)
+        y = self.new_tensor(x.N, d.To, d.Ho, d.Wo, co, Cp=d.Co)
+        scale, bias = PK.fold_bn(None, None, co, d.Co)
+        scale_d, bias_d = self.const(scale), self.const(bias)
+        w_d = self.const(PK.pack_stem_stream(weight, x.Cp, d.Co, lead))
+        zero_row = self.const(torch.zeros(4096, dtype=torch.float16))
+        lib = self.lib
+
+        def fn(stream):
+            d.x_row_stride, d.y_row_stride = x.row_stride, y.row_stride   # y may have been retargeted
+            L.check(lib.pv_conv3d_stem_stream_fwd(C.byref(d), x.ptr(), w_d.data_ptr(), scale_d.data_ptr(),
+                                                  bias_d.data_ptr(), zero_row.data_ptr(), y.ptr(), stream),
+                    "pv_conv3d_stem_stream_fwd(%s)" % name)
+        self.stats["stem_stream"] = self.stats.get("stem_stream", 0) + 1
+        self.add(name, fn, "tcgen05", flops, nbytes, reads=(x,), writes=(y,))
         return y
 
     def _conv_desc(self, x, out_thw, co_pad, kernel, stride, padding, dilation, groups, act, residual, y_row_stride,
