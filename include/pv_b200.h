@@ -42,7 +42,11 @@ typedef enum pv_act {
   PV_ACT_RELU = 1,
   PV_ACT_SWISH = 2,   /* x*sigmoid(x)        reference layers/swish.py:25-28     */
   PV_ACT_GELU = 3,    /* exact erf GELU      reference layers/attention.py:74   */
-  PV_ACT_SIGMOID = 4
+  PV_ACT_SIGMOID = 4,
+  PV_ACT_HSWISH = 5   /* x*clamp(x+3,0,6)/6  torch.nn.Hardswish; the mobile efficient blocks' "hswish"
+                       * Every entry point that takes an activation rejects a code outside 0..5 with
+                       * PV_ERR_INVALID (PV_ERR_UNSUPPORTED where a kernel family implements fewer
+                       * codes), and every *_supported probe answers 0 for it. */
 } pv_act;
 
 typedef enum pv_conv_algo {

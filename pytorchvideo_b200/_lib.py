@@ -9,7 +9,7 @@ import os
 from . import _build
 
 PV_F16, PV_F32, PV_U8 = 0, 1, 2
-ACT_NONE, ACT_RELU, ACT_SWISH, ACT_GELU, ACT_SIGMOID = 0, 1, 2, 3, 4
+ACT_NONE, ACT_RELU, ACT_SWISH, ACT_GELU, ACT_SIGMOID, ACT_HSWISH = 0, 1, 2, 3, 4, 5
 ALGO_AUTO, ALGO_DIRECT, ALGO_TCGEN05 = 0, 1, 2
 POOL_MAX, POOL_AVG = 0, 1
 MPOOL_MAX, MPOOL_AVG, MPOOL_SUM = 0, 1, 2          # pv_masked_pool modes

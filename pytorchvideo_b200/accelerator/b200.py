@@ -10,7 +10,7 @@ from .efficient_block_base import EfficientBlockBase
 from .model_transmuter import EFFICIENT_BLOCK_TRANSMUTER_REGISTRY, transmute_model
 
 _WHOLE_BLOCKS = ("Net", "ResStage", "ResBlock", "BottleneckBlock", "ResNetBasicStem", "ResNetBasicHead",
-                 "MultiPathWayWithFuse", "ProjectedPool", "NonLocal")
+                 "MultiPathWayWithFuse", "ProjectedPool", "NonLocal", "EfficientX3d", "X3dBottleneckBlock")
 
 
 class B200Block(EfficientBlockBase):

@@ -85,7 +85,7 @@ extern "C" int pv_device_info(int* sm_count, int* cc) {
 }
 
 extern "C" int pv_conv3d_tcgen05_supported(const pv_conv3d_desc* d) {
-  if (!d) return 0;
+  if (!d || !pv::act_known(d->act)) return 0;
   if (pv::wants_gather(d)) return pv::conv3d_gather_supported(d);
   return pv::conv3d_tcgen05_supported(d, nullptr, 0);
 }
@@ -96,7 +96,7 @@ extern "C" int pv_conv3d_group_span(const pv_conv3d_desc* d, int* span_groups, i
   if (span_groups) *span_groups = sg;
   if (span_k) *span_k = sk;
   if (span_n) *span_n = sn;
-  if (!known) return 0;
+  if (!known || !pv::act_known(d->act)) return 0;
   pv_conv3d_desc q = *d;
   q.ci_pad64 = sk;             // grouped mode packs the weights at the span width
   return pv::conv3d_tcgen05_supported(&q, nullptr, 0);

@@ -165,14 +165,22 @@ __device__ __forceinline__ float se_sum_get(const float* sums, long long idx) {
   return (float)((double)reinterpret_cast<const long long*>(sums)[idx] * (1.0 / 16777216.0));
 }
 
+// torch.nn.Hardswish in fp32, in torch's order: x * min(max(x + 3, 0), 6) / 6 (a true division, not a multiply by 1/6)
+__device__ __forceinline__ float hswish(float x) { return x * fminf(fmaxf(x + 3.f, 0.f), 6.f) / 6.f; }
+
 __device__ __forceinline__ float apply_act(float x, int act) {
   switch (act) {
     case PV_ACT_RELU: return fmaxf(x, 0.f);
     case PV_ACT_SWISH: return x / (1.f + __expf(-x));
     case PV_ACT_GELU: return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f));
     case PV_ACT_SIGMOID: return 1.f / (1.f + __expf(-x));
+    case PV_ACT_HSWISH: return hswish(x);
     default: return x;
   }
 }
+
+// The activation codes the library implements; entry points reject every other code (pv_b200.h pv_act), so no
+// kernel ever sees one.
+inline bool act_known(int act) { return act >= PV_ACT_NONE && act <= PV_ACT_HSWISH; }
 
 }  // namespace pv

@@ -73,10 +73,16 @@ __device__ __forceinline__ void epi_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// The fragment math has five instances: ReLU, none, Swish, GELU, and EPI_ACT_RARE for the rarely fused sigmoid and
+// HardSwish, which picks between them at run time (act).  A sixth instance pushes the <128, *> kernels past their
+// 168-register cap into spills (DESIGN.md section 1).
+constexpr int EPI_ACT_RARE = -1;
+
 template <int ACT>
-__device__ __forceinline__ float act_t(float x) {
+__device__ __forceinline__ float act_t(float x, int act) {
   if (ACT == PV_ACT_RELU) return fmaxf(x, 0.f);
   if (ACT == PV_ACT_NONE) return x;
+  if (ACT == EPI_ACT_RARE) return act == PV_ACT_HSWISH ? hswish(x) : apply_act(x, PV_ACT_SIGMOID);
   return apply_act(x, ACT);
 }
 
@@ -141,7 +147,7 @@ __device__ __forceinline__ void epilogue_dma(const EpiParams& E, const EpiSmem& 
 // 64 (ctid / 128) + 16 ((ctid / 32) & 3) + (lane / 4) + 8 i, column 8 j + 2 (lane % 4) + e.
 template <int BN, int ACT, bool RES>
 __device__ __forceinline__ void epi_math(const float (&d)[BN / 2], uint8_t* stg, const float* __restrict__ scale,
-                                         const float* __restrict__ bias, int Co, int n0, int ctid) {
+                                         const float* __restrict__ bias, int Co, int n0, int ctid, int act) {
   const int lane = ctid & 31;
   const int row0 = 64 * (ctid >> 7) + 16 * ((ctid >> 5) & 3) + (lane >> 2);
   const int cq = 2 * (lane & 3);
@@ -166,16 +172,16 @@ __device__ __forceinline__ void epi_math(const float (&d)[BN / 2], uint8_t* stg,
         f0 += r.x;
         f1 += r.y;
       }
-      *cell = __floats2half2_rn(act_t<ACT>(f0), act_t<ACT>(f1));
+      *cell = __floats2half2_rn(act_t<ACT>(f0, act), act_t<ACT>(f1, act));
     }
   }
 }
 
 template <int BN, int ACT>
 __device__ __forceinline__ void epi_math_res(bool res, const float (&d)[BN / 2], uint8_t* stg, const float* scale,
-                                             const float* bias, int Co, int n0, int ctid) {
-  if (res) epi_math<BN, ACT, true>(d, stg, scale, bias, Co, n0, ctid);
-  else epi_math<BN, ACT, false>(d, stg, scale, bias, Co, n0, ctid);
+                                             const float* bias, int Co, int n0, int ctid, int act) {
+  if (res) epi_math<BN, ACT, true>(d, stg, scale, bias, Co, n0, ctid, act);
+  else epi_math<BN, ACT, false>(d, stg, scale, bias, Co, n0, ctid, act);
 }
 
 // Post-activation addend on the staged f16 tile: a second pass over the staging buffer once epi_math has written it,
@@ -228,11 +234,12 @@ __device__ __forceinline__ void epilogue_tile(const EpiParams& E, const EpiSmem&
   mbar_wait(S.ready(buf), phase);            // buffer free, residual landed
   uint8_t* staging_gen = S.buf_gen(buf);
   switch (E.act) {
-    case PV_ACT_RELU: epi_math_res<BN, PV_ACT_RELU>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid); break;
-    case PV_ACT_NONE: epi_math_res<BN, PV_ACT_NONE>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid); break;
-    case PV_ACT_SWISH: epi_math_res<BN, PV_ACT_SWISH>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid); break;
-    case PV_ACT_GELU: epi_math_res<BN, PV_ACT_GELU>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid); break;
-    default: epi_math_res<BN, PV_ACT_SIGMOID>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid); break;
+    case PV_ACT_RELU: epi_math_res<BN, PV_ACT_RELU>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid, E.act); break;
+    case PV_ACT_NONE: epi_math_res<BN, PV_ACT_NONE>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid, E.act); break;
+    case PV_ACT_SWISH: epi_math_res<BN, PV_ACT_SWISH>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid, E.act); break;
+    case PV_ACT_GELU: epi_math_res<BN, PV_ACT_GELU>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid, E.act); break;
+    // PV_ACT_SIGMOID, PV_ACT_HSWISH; the entry points reject every other code (act_known)
+    default: epi_math_res<BN, EPI_ACT_RARE>(E.has_residual, d, staging_gen, scale, bias, E.Co, n0, ctid, E.act); break;
   }
   if (E.addend) {
     epi_bar_sync(EPI_BAR_ID, EPI_THREADS);   // the cells of a row were written by other threads

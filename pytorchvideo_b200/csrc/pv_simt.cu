@@ -894,6 +894,7 @@ extern "C" int pv_temporal_tap_sum(const void* yk, void* y, int dtype, int N, in
                                    const float* bias, int act, long long in_row_stride,
                                    long long out_row_stride, void* stream) {
   PV_CHECK_ARG(yk && y && scale && bias, "null pointer");
+  PV_CHECK_ARG(act_known(act), "activation code %d unsupported", act);
   PV_CHECK_ARG(Co % 8 == 0 && in_row_stride % 8 == 0 && out_row_stride % 8 == 0, "Co/strides %% 8");
   PV_CHECK_ARG(in_row_stride >= (long long)kt * Co && out_row_stride >= Co, "row stride too small");
   const long long total = (long long)N * To * hw * (Co / 8);
@@ -1011,6 +1012,7 @@ namespace pv {
 int conv3d_check(const pv_conv3d_desc* d) {
   PV_CHECK_ARG(d, "null descriptor");
   PV_CHECK_ARG(d->dtype == PV_F16 || d->dtype == PV_F32, "conv dtype must be f16|f32");
+  PV_CHECK_ARG(act_known(d->act), "activation code %d unsupported", d->act);
   PV_CHECK_ARG(d->N >= 0 && d->Ci > 0 && d->Co > 0, "bad sizes");
   PV_CHECK_ARG(d->kt > 0 && d->kh > 0 && d->kw > 0 && d->st > 0 && d->sh > 0 && d->sw > 0 &&
                    d->dt > 0 && d->dh > 0 && d->dw > 0, "bad kernel/stride/dilation");
@@ -1177,6 +1179,7 @@ extern "C" int pv_scale_act(const void* x, void* y, int dtype, long long x_row_s
                             long long y_row_stride, int N, long long npos, int C,
                             const float* gate, int act, void* stream) {
   PV_CHECK_ARG(x && y, "null pointer");
+  PV_CHECK_ARG(act_known(act), "activation code %d unsupported", act);
   PV_CHECK_ARG(C % 8 == 0 && x_row_stride % 8 == 0 && y_row_stride % 8 == 0, "C/strides %% 8");
   const long long total = (long long)N * npos * (C / 8);
   if (total == 0) return PV_OK;

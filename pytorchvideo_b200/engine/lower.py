@@ -34,6 +34,8 @@ def _act_code(m):
         return L.ACT_GELU
     if n == "Sigmoid":
         return L.ACT_SIGMOID
+    if n in ("HardSwish", "Hardswish"):      # the mobile blocks' wrapper and torch.nn.Hardswish
+        return L.ACT_HSWISH
     if n == "Identity":
         return L.ACT_NONE
     raise NotImplementedError("activation %s has no B200 kernel" % n)
@@ -147,7 +149,7 @@ class Lowering:
         return self.p.emit_act(x, L.ACT_RELU, name or "relu")
 
     def lower_SqueezeExcitation(self, m, x, name):
-        blk = m.block
+        blk = _se_block(m, name or "se")
         if type(blk[1]).__name__ != "ReLU" or type(blk[3]).__name__ != "Sigmoid":
             raise NotImplementedError("SqueezeExcitation variant unsupported")
         self.p.materialize_input(x)
@@ -1394,3 +1396,145 @@ Lowering.lower_ReduceFusion = _lower_reduce_fusion
 Lowering.lower_LayerNorm = _lower_layernorm
 Lowering.lower_Linear = _lower_linear
 Lowering.lower_PositionalEncoding = _lower_positional_encoding
+
+
+# =============================================================================================
+# Mobile efficient blocks (layers/accelerator/mobile_cpu/, models/accelerator/mobile_cpu/): this package's trees and
+# the reference's original-form trees.  Their class names collide with others (SqueezeExcitation, ReLU, Swish,
+# Identity), so these handlers also check attributes.  The reference's deployable form (convert() applied: Conv2d
+# decompositions, _Reshape, _SkipConnectMul, fused ConvReLU) is refused with the name of the first module met.
+# =============================================================================================
+_MOBILE_ACTS = ("ReLU", "Swish", "HardSwish", "Identity")
+
+
+def _deployable(m, name):
+    from ..module import B200Module
+    if getattr(m, "convert_flag", False) and not isinstance(m, B200Module):
+        raise NotImplementedError("%s: %s is in the reference's deployable (converted) form, which has no B200 lowering; "
+                                  "lower the original form" % (name, type(m).__name__))
+
+
+def _se_block(m, name):
+    """The fvcore-style Sequential(Conv3d, ReLU, Conv3d, Sigmoid) of a SqueezeExcitation: ``.block`` (fvcore / X3D) or
+    ``.se.block`` (the mobile wrapper)."""
+    _deployable(m, name)
+    se = getattr(m, "se", None)
+    blk = getattr(se, "block", None) if se is not None else getattr(m, "block", None)
+    if not isinstance(blk, nn.Sequential) or len(blk) != 4:
+        raise NotImplementedError("%s: SqueezeExcitation variant %s unsupported" % (
+            name, type(se).__name__ if se is not None else "without a block"))
+    return blk
+
+
+def _mobile_parts(m, name):
+    """(conv, bn or None, act wrapper) of a mobile convolution block: kernel = Sequential(conv, [bn], act)."""
+    _deployable(m, name)
+    k = getattr(m, "kernel", None)
+    mods = getattr(k, "_modules", {})
+    if not isinstance(k, nn.Sequential) or list(mods) not in (["conv", "act"], ["conv", "bn", "act"]) \
+            or type(mods["conv"]) is not nn.Conv3d or type(mods["act"]).__name__ not in _MOBILE_ACTS:
+        raise NotImplementedError("%s: %s without its original Sequential(conv, [bn], act) kernel has no B200 lowering"
+                                  % (name, type(m).__name__))
+    return mods["conv"], mods.get("bn"), mods["act"]
+
+
+def _mobile_conv(self, x, m, name, residual=None, act=None):
+    """A mobile convolution block as one convolution; ``act`` (with ``residual``) replaces its own activation, which
+    must then be the identity."""
+    conv, bn, own = _mobile_parts(m, name)
+    if act is not None and type(own).__name__ != "Identity":
+        raise NotImplementedError("%s: activation %s before the block's residual add / activation" % (
+            name, type(own).__name__))
+    return self.conv(x, conv, bn, own if act is None else act, residual, name)
+
+
+def _lower_mobile_conv(self, m, x, name):
+    return _mobile_conv(self, x, m, name or "conv")
+
+
+def _lower_x3d_bottleneck(self, m, x, name):
+    name = name or "block"
+    _deployable(m, name)
+    layers = m.layers
+    keys = [k for k in layers._modules if k != "se"]
+    if keys != ["conv_0", "conv_1", "act_func_1", "conv_2"]:
+        raise NotImplementedError("%s: X3dBottleneckBlock layers %s unsupported" % (name, list(layers._modules)))
+    shortcut = None
+    if m._use_residual:       # the shortcut first, as ResBlock's branch1: the same launch order as models/x3d.py
+        shortcut = x if m._res_proj is None else _mobile_conv(self, x, m._res_proj, name + "._res_proj")
+    h = _mobile_conv(self, x, layers.conv_0, name + ".layers.conv_0")
+    se = layers._modules.get("se")
+    if se is None:
+        h = _mobile_conv(self, h, layers.conv_1, name + ".layers.conv_1", act=layers.act_func_1)
+    else:
+        blk = _se_block(se, name + ".layers.se")
+        if type(blk[1]).__name__ != "ReLU" or type(blk[3]).__name__ != "Sigmoid":
+            raise NotImplementedError("%s.layers.se: SqueezeExcitation variant unsupported" % name)
+        conv, bn, own = _mobile_parts(layers.conv_1, name + ".layers.conv_1")
+        if type(own).__name__ != "Identity":
+            raise NotImplementedError("%s.layers.conv_1: activation %s before the SE" % (name, type(own).__name__))
+        h = self.conv(h, conv, bn, None, None, name + ".layers.conv_1", se_sums=True)
+        h = self.p.emit_se_scale_act(h, blk[0].weight, blk[0].bias, blk[2].weight, blk[2].bias,
+                                     _act_code(layers.act_func_1), name + ".layers.se")
+    return _mobile_conv(self, h, layers.conv_2, name + ".layers.conv_2", residual=shortcut, act=m.final_act)
+
+
+def _lower_efficient_x3d(self, m, x, name):
+    pre = name + "." if name else ""
+    if self.extra != ("head",):          # ("head",): the head alone, on the s5 feature map (EfficientX3d.forward)
+        for s in ("s1", "s2", "s3", "s4", "s5"):
+            for cname, blk in getattr(m, s).named_children():
+                x = self.lower(blk, x, "%s%s.%s" % (pre, s, cname))
+    if not m.enable_head:
+        return x
+    # head (efficient_x3d.py forward): conv_5 -> avg_pool -> lin_5 -> permute -> projection -> act -> mean over the
+    # (1, 1, 1) grid -> view (N, -1); the activation goes into the projection's epilogue
+    head = m.head
+    if list(head._modules) != ["conv_5", "avg_pool", "lin_5"]:
+        raise NotImplementedError("%shead: layers %s unsupported" % (pre, list(head._modules)))
+    x = _mobile_conv(self, x, head.conv_5, pre + "head.conv_5")
+    x = self.lower(head.avg_pool, x, pre + "head.avg_pool")
+    x = _mobile_conv(self, x, head.lin_5, pre + "head.lin_5")
+    _deployable(m.projection, pre + "projection")
+    proj = getattr(m.projection, "model", None)
+    if not isinstance(proj, nn.Linear):
+        raise NotImplementedError("%sprojection: %s unsupported" % (pre, type(proj).__name__))
+    if type(m.act).__name__ not in _MOBILE_ACTS:
+        raise NotImplementedError("%sact: %s unsupported" % (pre, type(m.act).__name__))
+    w = proj.weight.reshape(proj.out_features, proj.in_features, 1, 1, 1)
+    x = self.p.emit_conv(x, w, proj.bias, None, (1, 1, 1), (0, 0, 0), (1, 1, 1), 1, _act_code(m.act), None,
+                         pre + "projection")
+    return self.p.emit_head_reduce(x, False, pre + "mean")
+
+
+def _lower_pool_size1(self, m, x, name):
+    _deployable(m, name or "pool")
+    return self.pool(x, m.pool, name or "pool")
+
+
+def _lower_no_op_convert(self, m, x, name):
+    return self.lower(m.model, x, (name + "." if name else "") + "model")
+
+
+def _lower_hardswish(self, m, x, name):
+    self.p.materialize_input(x)
+    return self.p.emit_act(x, L.ACT_HSWISH, name or "hswish")
+
+
+for _n in ("Conv3dPwBnAct", "Conv3d3x3x3DwBnAct", "Conv3dTemporalKernel1BnAct", "Conv3d3x1x1BnAct", "Conv3d5x1x1BnAct"):
+    setattr(Lowering, "lower_" + _n, _lower_mobile_conv)
+def _lower_adaptive_avg_pool3d(self, m, x, name):
+    # torch.nn.AdaptiveAvgPool3d, or the mobile wrapper of the same name that holds one as ``.model``
+    if isinstance(getattr(m, "model", None), nn.Module):
+        return _lower_no_op_convert(self, m, x, name)
+    return self.pool(x, m, name)
+
+
+Lowering.lower_NoOpConvertBlock = _lower_no_op_convert
+Lowering.lower_FullyConnected = _lower_no_op_convert
+Lowering.lower_AdaptiveAvgPool3d = _lower_adaptive_avg_pool3d
+Lowering.lower_X3dBottleneckBlock = _lower_x3d_bottleneck
+Lowering.lower_EfficientX3d = _lower_efficient_x3d
+Lowering.lower_AdaptiveAvgPool3dOutSize1 = _lower_pool_size1
+Lowering.lower_HardSwish = _lower_hardswish
+Lowering.lower_Hardswish = _lower_hardswish

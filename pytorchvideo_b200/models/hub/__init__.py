@@ -66,6 +66,18 @@ def x3d_l(pretrained=False, progress=True, **kw):
     return _build(create_x3d, pretrained, input_clip_length=16, input_crop_size=312, depth_factor=5.0, **kw)
 
 
+def efficient_x3d_xs(pretrained=False, progress=True, **kw):
+    """X3D-XS in the mobile efficient-block tree (reference hub/efficient_x3d_mobile_cpu.py)."""
+    from ..accelerator.mobile_cpu.efficient_x3d import create_x3d as create_efficient_x3d
+    return _build(create_efficient_x3d, pretrained, expansion="XS", **kw)
+
+
+def efficient_x3d_s(pretrained=False, progress=True, **kw):
+    """X3D-S in the mobile efficient-block tree (reference hub/efficient_x3d_mobile_cpu.py)."""
+    from ..accelerator.mobile_cpu.efficient_x3d import create_x3d as create_efficient_x3d
+    return _build(create_efficient_x3d, pretrained, expansion="S", **kw)
+
+
 def csn_r101(pretrained=False, progress=True, **kw):
     return _build(create_csn, pretrained, model_depth=101, stem_pool=nn.MaxPool3d, head_pool_kernel_size=(4, 7, 7),
                   **kw)

@@ -522,3 +522,125 @@ def masked_call(m, x, mask):
     if type(m).__name__ == "PositionalEncoding":
         return m(x)
     return m(x, mask)
+
+
+# ---- Efficient X3D / mobile efficient-block cases (tests/golden/efficient_x3d.pt) -----------------------------------
+# name: (class in the efficient-block namespace, kwargs, input shape, f16_grid)
+_XS_CLIP = (1, 3, 4, 160, 160)
+EFFICIENT_CASES = {
+    "xs_b2": ("EfficientX3d", {"expansion": "XS"}, (2, 3, 4, 160, 160), False),
+    "xs_b8_f16grid": ("EfficientX3d", {"expansion": "XS"}, (8, 3, 4, 160, 160), True),
+    "s_b1": ("EfficientX3d", {"expansion": "S"}, (1, 3, 13, 160, 160), False),
+    "m_b1": ("EfficientX3d", {"expansion": "M"}, (1, 3, 16, 224, 224), False),
+    "xs_no_head": ("EfficientX3d", {"enable_head": False}, _XS_CLIP, False),
+    "xs_head_relu": ("EfficientX3d", {"head_act": "relu"}, _XS_CLIP, False),
+    "xs_head_swish": ("EfficientX3d", {"head_act": "swish"}, _XS_CLIP, False),
+    "xs_head_hswish": ("EfficientX3d", {"head_act": "hswish"}, _XS_CLIP, False),
+    "block_hswish_se": ("X3dBottleneckBlock", dict(in_channels=24, mid_channels=54, out_channels=48, spatial_stride=2,
+                                                   se_ratio=0.0625, act_functions=("hswish",) * 3), (2, 24, 4, 14, 14),
+                        False),
+    "block_hswish": ("X3dBottleneckBlock", dict(in_channels=24, mid_channels=54, out_channels=48, spatial_stride=2,
+                                                se_ratio=0, act_functions=("hswish",) * 3), (2, 24, 4, 14, 14), False),
+    "block_no_residual": ("X3dBottleneckBlock", dict(in_channels=24, mid_channels=54, out_channels=48, use_residual=False,
+                                                     act_functions=("relu", "swish", "relu")), (2, 24, 4, 10, 10), False),
+    "block_bias_no_bn": ("X3dBottleneckBlock", dict(in_channels=24, mid_channels=54, out_channels=24, bias=(True,) * 3,
+                                                    use_bn=(False,) * 3, act_functions=("relu", "hswish", "hswish")),
+                         (2, 24, 4, 12, 12), False),
+    "conv_pw_hswish": ("Conv3dPwBnAct", dict(in_channels=24, out_channels=40, activation="hswish"), (2, 24, 3, 8, 8),
+                       False),
+    "conv_dw_swish": ("Conv3d3x3x3DwBnAct", dict(in_channels=40, spatial_stride=2, activation="swish"),
+                      (2, 40, 3, 11, 11), False),
+    "conv_t1_relu": ("Conv3dTemporalKernel1BnAct", dict(in_channels=24, out_channels=32, spatial_kernel=3,
+                                                        spatial_stride=2, spatial_padding=1, activation="relu"),
+                     (2, 24, 3, 12, 12), False),
+    "conv_3x1x1_hswish": ("Conv3d3x1x1BnAct", dict(in_channels=24, out_channels=32, activation="hswish"),
+                          (2, 24, 5, 6, 6), False),
+    "conv_5x1x1_dw_hswish": ("Conv3d5x1x1BnAct", dict(in_channels=24, out_channels=24, groups=24, activation="hswish"),
+                             (2, 24, 6, 8, 8), False),
+}
+
+
+def tree_digests_text(text):
+    import hashlib
+    return hashlib.sha256(text.encode()).hexdigest()
+
+
+def tree_digests(model):
+    """(sha256 of ``repr(model)``, sha256 of its ``state_dict`` keys in order): the module tree of a golden case in 128
+    bytes instead of the ~70 kB of text of a whole Efficient X3D."""
+    return tree_digests_text(repr(model)), tree_digests_text("\n".join(model.state_dict().keys()))
+
+
+def efficient_namespace(root="pytorchvideo_b200"):
+    """The efficient-block classes of ``root`` (this package, or "pytorchvideo" for the reference): both keep them at
+    the same module paths."""
+    import importlib
+    import types
+    ns = types.SimpleNamespace()
+    for mod in ("models.accelerator.mobile_cpu.efficient_x3d", "models.accelerator.mobile_cpu.residual_blocks",
+                "layers.accelerator.mobile_cpu.convolutions"):
+        m = importlib.import_module(root + "." + mod)
+        for k in dir(m):
+            if not k.startswith("_"):
+                setattr(ns, k, getattr(m, k))
+    return ns
+
+
+def build_efficient_case(name, ns, seed=31):
+    """(module, input) of an EFFICIENT_CASES entry built from ``ns`` (efficient_namespace), with randomize_model
+    weights (the residual branch's last BatchNorm drawn small, as for models/x3d.py); model inputs are synthetic clips, block inputs standard normal (straddling the HardSwish knees)."""
+    cls, kw, shape, grid = EFFICIENT_CASES[name]
+    torch.manual_seed(seed)
+    m = getattr(ns, cls)(**kw)
+    for blk in m.modules():     # the residual branch's last BatchNorm, as models/resnet.py marks norm_c
+        if type(blk).__name__ == "X3dBottleneckBlock" and "bn" in blk.layers.conv_2.kernel._modules:
+            blk.layers.conv_2.kernel.bn.block_final_bn = True
+    m = randomize_model(m, seed=seed, f16_weights=grid).eval()
+    if cls == "EfficientX3d":
+        B, _, T, H, W = shape
+        return m, synthetic_clip(B, T, H, W, seed=seed + 1, f16_values=grid)
+    g = torch.Generator(device="cpu")
+    g.manual_seed(seed + 1)
+    return m, torch.randn(shape, generator=g)
+
+
+@torch.no_grad()
+def map_x3d_to_efficient(x3d, eff):
+    """Copy the weights of a ``models.x3d.create_x3d`` network (hub x3d_xs / x3d_s) into the EfficientX3d of the same
+    widths: the same network in another module tree.  The one structural difference: a stride-only shortcut
+    projection of create_x3d has no BatchNorm, the efficient block's always has one; it gets the identity statistics
+    (weight 1, bias 0, mean 0, var 1 - eps), which fold to scale 1.0 and bias 0.0 exactly."""
+    def conv_bn(dst, conv, bn):
+        k = dst.kernel
+        k.conv.weight.copy_(conv.weight)
+        if bn is not None:
+            k.bn.load_state_dict(bn.state_dict())
+        elif "bn" in k._modules:
+            k.bn.weight.fill_(1.0)
+            k.bn.bias.zero_()
+            k.bn.running_mean.zero_()
+            k.bn.running_var.fill_(1.0 - k.bn.eps)
+    blocks = list(x3d.blocks)
+    stem = blocks[0]
+    conv_bn(eff.s1.pathway0_stem_conv_xy, stem.conv.conv_t, None)
+    conv_bn(eff.s1.pathway0_stem_conv, stem.conv.conv_xy, stem.norm)
+    for s, stage in enumerate(blocks[1:5]):
+        dst_stage = list(getattr(eff, "s%d" % (s + 2)).children())
+        assert len(dst_stage) == len(stage.res_blocks)
+        for src, dst in zip(stage.res_blocks, dst_stage):
+            b = src.branch2
+            conv_bn(dst.layers.conv_0, b.conv_a, b.norm_a)
+            conv_bn(dst.layers.conv_1, b.conv_b, b.norm_b[0])
+            if "se" in dst.layers._modules:
+                dst.layers.se.se.block.load_state_dict(b.norm_b[1].block.state_dict())
+            else:
+                assert type(b.norm_b[1]).__name__ == "Identity"
+            conv_bn(dst.layers.conv_2, b.conv_c, b.norm_c)
+            assert (src.branch1_conv is None) == (dst._res_proj is None)
+            if src.branch1_conv is not None:
+                conv_bn(dst._res_proj, src.branch1_conv, src.branch1_norm)
+    head = blocks[5]
+    conv_bn(eff.head.conv_5, head.pool.pre_conv, head.pool.pre_norm)
+    conv_bn(eff.head.lin_5, head.pool.post_conv, head.pool.post_norm)
+    eff.projection.model.load_state_dict(head.proj.state_dict())
+    return eff
