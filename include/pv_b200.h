@@ -323,6 +323,17 @@ int pv_conv3d_fwd(const pv_conv3d_desc* d, int algo, const void* x, const void* 
  * (layers/attention.py:364-403).  w: [tap][C]. */
 int pv_dwconv3d_fwd(const pv_conv3d_desc* d, const void* x, const void* w, const float* scale,
                     const float* bias, void* y, float* se_sums, void* stream);
+/* Depthwise 3x3 convolution over a one-frame token plane: the (1,3,3) attention pools of the image MViT
+ * (layers/attention.py:364-403, models/vision_transformers.py use_2d_patch=True).
+ *   y[n][h][w][c] = scale[c] * sum_{i,j} x[n][h*sh + i - ph][w*sw + j - pw][c] * w[i*3 + j][c] + bias[c]
+ * fp32 accumulation, one f16 rounding; no activation.  Takes f16, groups == Ci == Co, Ti == To == 1, kernel (1,3,3),
+ * no temporal stride or padding, sh == sw in {1, 2, 4}, ph, pw <= 2, no dilation, residual or addend, Co and
+ * x_row_stride and x_batch_stride multiples of 8, y_row_stride even, x 16-byte aligned; else PV_ERR_UNSUPPORTED.
+ * x_batch_stride / y_batch_stride step over MViT's cls row as in pv_dwconv3d_fwd.  w: [tap][C].
+ * pv_dwplane_supported answers 1 exactly for the descriptors pv_dwplane_fwd takes (host only, no GPU). */
+int pv_dwplane_supported(const pv_conv3d_desc* d);
+int pv_dwplane_fwd(const pv_conv3d_desc* d, const void* x, const void* w, const float* scale,
+                   const float* bias, void* y, void* stream);
 
 /* 1 if PV_ALGO_TCGEN05 supports this descriptor (pure host-side check, no GPU needed). */
 int pv_conv3d_tcgen05_supported(const pv_conv3d_desc* d);

@@ -134,6 +134,8 @@ SIGNATURES = {
     "pv_conv3d_fwd": (C.c_int, [C.POINTER(Conv3dDesc), C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp,
                                 c_vp, c_vp]),
     "pv_dwconv3d_fwd": (C.c_int, [C.POINTER(Conv3dDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_dwplane_supported": (C.c_int, [C.POINTER(Conv3dDesc)]),
+    "pv_dwplane_fwd": (C.c_int, [C.POINTER(Conv3dDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_temporal_tap_sum": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_ll, C.c_int, C.c_int,
                                       C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, c_ll, c_ll, c_vp]),
     "pv_conv3d_tcgen05_supported": (C.c_int, [C.POINTER(Conv3dDesc)]),

@@ -655,8 +655,9 @@ class CompiledModel:
         ins = list(example_inputs) if multi else [example_inputs]
         raw = _raw_inputs(model, ins)
         self.mask_slots = _mask_slots(ins, extra)
+        image = _image_root(model, ins)
         for i, t in enumerate(ins):
-            if i not in raw and i not in self.mask_slots and t.dim() not in (2, 3, 5):
+            if i not in raw and i not in self.mask_slots and t.dim() not in (2, 3, 5) and not image:
                 raise RuntimeError("expected a 5-D (B, C, T, H, W) clip or a (B, N, C) token tensor, got %s" % (tuple(t.shape),))
         device = ins[0].device
         if device.type != "cuda":
@@ -671,7 +672,7 @@ class CompiledModel:
         xs = [self.plan.raw_input(s) if i in raw else PL.MaskRef(s.shape[0], s.shape[1], tensor=s) if i in self.mask_slots
               else _emit_input(self.plan, s) for i, s in enumerate(self.static_in)]
         out = low.lower(model, _root_input(xs, ins, extra) if _masked_root(extra) else (xs if multi else xs[0]), "")
-        out = _emit_output(self.plan, out, tokens=ins[0].dim() != 5)
+        out = _emit_output(self.plan, out, tokens=ins[0].dim() not in (4, 5))
         self.out_buf, self.out_shape = out
         self.aux = low.aux_out
         self.plan.finalize()
@@ -781,7 +782,24 @@ def _root_input(xs, ins, extra):
     return pairs if extra[0][1] else pairs[0]
 
 
+def _image_root(model, ins):
+    """True when the input is one (B, C, H, W) image batch for an image MViT (``patch_embed.patch_model`` a Conv2d,
+    create_multiscale_vision_transformers(use_2d_patch=True)); it runs as a clip of one frame.  A 4-D input to any
+    other module raises."""
+    if not any(torch.is_tensor(t) and t.dim() == 4 for t in ins):
+        return False
+    pm = getattr(getattr(model, "patch_embed", None), "patch_model", None)
+    if type(model).__name__ != "MultiscaleVisionTransformers" or not isinstance(pm, nn.Conv2d) or len(ins) != 1:
+        raise RuntimeError("a 4-D (B, C, H, W) input is taken only by an image MViT (patch_embed.patch_model a Conv2d); "
+                           "%s expects 5-D (B, C, T, H, W) clips or (B, N, C) tokens" % type(model).__name__)
+    return True
+
+
 def _emit_input(plan, t):
+    if t.dim() == 4:              # an image batch (see _image_root): a one-frame clip over the same storage
+        x = _emit_input(plan, t.unsqueeze(2))
+        x.image = True
+        return x
     if t.dim() == 5:
         return plan.emit_input_ncdhw(t, t.shape[1], 4 if t.shape[1] <= 4 else (t.shape[1] + 7) // 8 * 8)
     x = plan.emit_input_tokens(t)
@@ -813,12 +831,13 @@ def lower_only(model, example_inputs, dtype="f16", use_tcgen05=True, extra=()):
     plan = Plan("cpu", {"f16": L.PV_F16, "f32": L.PV_F32}[dtype], use_tcgen05)
     raw = _raw_inputs(model, ins)
     masks = _mask_slots(ins, extra)
+    _image_root(model, ins)
     xs = [plan.raw_input(torch.empty(t.shape, dtype=torch.float32)) if i in raw
           else PL.MaskRef(t.shape[0], t.shape[1], tensor=torch.empty(t.shape, dtype=torch.uint8)) if i in masks
           else _emit_input(plan, torch.empty(t.shape, dtype=torch.float32)) for i, t in enumerate(ins)]
     low = Lowering(plan, extra)
     out = low.lower(model, _root_input(xs, ins, extra) if _masked_root(extra) else (xs if multi else xs[0]), "")
-    out = _emit_output(plan, out, tokens=ins[0].dim() != 5)
+    out = _emit_output(plan, out, tokens=ins[0].dim() not in (4, 5))
     plan.aux = low.aux_out
     return plan, out[1]
 
@@ -966,7 +985,18 @@ def _lower_mvit(self, m, x, name):
     pe = m.patch_embed
     if type(pe).__name__ != "PatchEmbed":
         raise NotImplementedError("MViT without a conv patch embedding is unsupported")
-    x = self.conv(x, pe.patch_model, None, None, None, "patch_embed.patch_model")
+    pm = pe.patch_model
+    if isinstance(pm, nn.Conv2d):
+        # image MViT (vision_transformers.py use_2d_patch=True): the Conv2d runs as a (1, kh, kw) Conv3d on the
+        # one-frame clip, so a 7x7 / stride 4 embed takes the window-mode tensor-core stem like the video models'
+        if not getattr(x, "image", False):
+            raise RuntimeError("an image MViT (Conv2d patch embedding) takes (B, C, H, W) images")
+        if isinstance(pm.padding, str) or pm.padding_mode != "zeros":
+            raise NotImplementedError("patch_embed.patch_model: string padding / padding_mode unsupported")
+        x = self.p.emit_conv(x, pm.weight.unsqueeze(2), pm.bias, None, (1,) + tuple(pm.stride), (0,) + tuple(pm.padding),
+                             (1,) + tuple(pm.dilation), pm.groups, L.ACT_NONE, None, "patch_embed.patch_model")
+    else:
+        x = self.conv(x, pm, None, None, None, "patch_embed.patch_model")
     enc = m.cls_positional_encoding
     T, H, W = enc.patch_embed_shape()
     if (x.T, x.H, x.W) != (T, H, W):

@@ -951,15 +951,26 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool"):
         d.pt, d.ph, d.pw = p
         d.dt, d.dh, d.dw = dl
         d.groups, d.act, d.has_residual = dim_all, L.ACT_NONE, 0
+        d.x_row_stride, d.y_row_stride = x.row_stride, y.row_stride
+        d.x_batch_stride, d.y_batch_stride = x.npos * x.row_stride, y.npos * y.row_stride
+        # a one-frame token grid (image MViT) pooled by a (1,kh,kw) conv: the plane kernel (csrc/pv_dwplane.cu) when it
+        # takes the shape; every other pool keeps pv_dwconv3d_fwd
+        plane = k[0] == 1 and T == 1 and bool(lib.pv_dwplane_supported(C_.byref(d)))
+        if plane:
+            plan.stats["dwplane"] = plan.stats.get("dwplane", 0) + 1
 
         def fn(stream):
             d.x_row_stride, d.y_row_stride = x.row_stride, y.row_stride
             d.x_batch_stride, d.y_batch_stride = x.npos * x.row_stride, y.npos * y.row_stride
-            # depthwise entry point: lane-per-channel-pair stencil for 3x3x3 in f16, generic stencil otherwise; the
-            # batch strides step over the cls row in front of every sample
-            L.check(lib.pv_dwconv3d_fwd(C_.byref(d), x.ptr() + cls * x.row_stride * esz, w_d.data_ptr(),
-                                        ones.data_ptr(), zeros.data_ptr(), y.ptr() + cls * y.row_stride * esz, None,
-                                        stream), "pv_dwconv3d_fwd(%s)" % name)
+            # the batch strides step over the cls row in front of every sample
+            xp, yp = x.ptr() + cls * x.row_stride * esz, y.ptr() + cls * y.row_stride * esz
+            if plane:
+                L.check(lib.pv_dwplane_fwd(C_.byref(d), xp, w_d.data_ptr(), ones.data_ptr(), zeros.data_ptr(), yp,
+                                           stream), "pv_dwplane_fwd(%s)" % name)
+            else:
+                # depthwise entry point: lane-per-channel-pair stencil for 3x3x3 in f16, generic stencil otherwise
+                L.check(lib.pv_dwconv3d_fwd(C_.byref(d), xp, w_d.data_ptr(), ones.data_ptr(), zeros.data_ptr(), yp,
+                                            None, stream), "pv_dwconv3d_fwd(%s)" % name)
         plan.add(name + ".dwconv", fn, "depthwise", 2.0 * x.N * To * Ho * Wo * dim_all * k[0] * k[1] * k[2],
                  (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz)
     else:

@@ -50,6 +50,16 @@ def slowfast_r101(pretrained=False, progress=True, **kw):
     return _build(create_slowfast, pretrained, model_depth=101, slowfast_fusion_conv_kernel_size=(5, 1, 1), **kw)
 
 
+def slowfast_16x8_r101_50_50(pretrained=False, progress=True, **kw):
+    """SlowFast-R101 16x8 whose res4 has temporal conv_a kernels in its first 6 blocks only (reference
+    hub/slowfast.py:101-147).  Inputs: 16 Slow and 64 Fast frames."""
+    res4 = ((3, 1, 1),) * 6 + ((1, 1, 1),) * (23 - 6)
+    return _build(create_slowfast, pretrained, model_depth=101, slowfast_fusion_conv_kernel_size=(5, 1, 1),
+                  stage_conv_a_kernel_sizes=(((1, 1, 1), (1, 1, 1), res4, (3, 1, 1)),
+                                             ((3, 1, 1), (3, 1, 1), res4, (3, 1, 1))),
+                  head_pool_kernel_sizes=((16, 7, 7), (64, 7, 7)), **kw)
+
+
 def x3d_xs(pretrained=False, progress=True, **kw):
     return _build(create_x3d, pretrained, input_clip_length=4, input_crop_size=160, **kw)
 
@@ -105,5 +115,23 @@ def mvit_base_16x4(pretrained=False, progress=True, **kw):
 def mvit_base_32x3(pretrained=False, progress=True, **kw):
     from ..vision_transformers import create_multiscale_vision_transformers
     cfg = dict(_MVIT_VIDEO_BASE, temporal_size=32)
+    cfg.update(kw)
+    return _build(create_multiscale_vision_transformers, pretrained, **cfg)
+
+
+_MVIT_IMAGE_BASE_16 = {
+    "spatial_size": 224, "temporal_size": 1, "depth": 16,
+    "conv_patch_embed_kernel": [7, 7], "conv_patch_embed_stride": [4, 4], "conv_patch_embed_padding": [3, 3],
+    "use_2d_patch": True,
+    "embed_dim_mul": [[1, 2.0], [3, 2.0], [14, 2.0]], "atten_head_mul": [[1, 2.0], [3, 2.0], [14, 2.0]],
+    "pool_q_stride_size": [[1, 1, 2, 2], [3, 1, 2, 2], [14, 1, 2, 2]], "pool_kv_stride_adaptive": [1, 4, 4],
+    "pool_kvq_kernel": [1, 3, 3],
+}
+
+
+def mvit_base_16(pretrained=False, progress=True, **kw):
+    """Image MViT-B, depth 16 (reference hub/vision_transformers.py:41-54, 127-158): takes (B, 3, 224, 224) images."""
+    from ..vision_transformers import create_multiscale_vision_transformers
+    cfg = dict(_MVIT_IMAGE_BASE_16)
     cfg.update(kw)
     return _build(create_multiscale_vision_transformers, pretrained, **cfg)

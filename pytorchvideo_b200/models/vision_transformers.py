@@ -45,7 +45,7 @@ def create_multiscale_vision_transformers(*, spatial_size, temporal_size, cls_em
                                           head_num_classes=400, create_scriptable_model=False,
                                           multiscale_vit_class=MultiscaleVisionTransformers):
     if use_2d_patch:
-        raise NotImplementedError("2-D (image) patch embedding is outside the video hot path")
+        assert temporal_size == 1, "If use_2d_patch, temporal_size needs to be 1."
     if pool_kv_stride_adaptive is not None:
         assert pool_kv_stride_size is None, "pool_kv_stride_size should be none if pool_kv_stride_adaptive is set."
     if norm != "layernorm":
@@ -56,9 +56,10 @@ def create_multiscale_vision_transformers(*, spatial_size, temporal_size, cls_em
     patch_embed = create_conv_patch_embed(
         in_channels=input_channels, out_channels=patch_embed_dim, conv_kernel_size=conv_patch_embed_kernel,
         conv_stride=conv_patch_embed_stride, conv_padding=conv_patch_embed_padding,
-        conv=nn.Conv3d) if enable_patch_embed else None
+        conv=nn.Conv2d if use_2d_patch else nn.Conv3d) if enable_patch_embed else None
     in_dims = [temporal_size, spatial_size[0], spatial_size[1]]
-    grid = [in_dims[i] // conv_patch_embed_stride[i] for i in range(3)] if enable_patch_embed else in_dims
+    in_stride = (1,) + tuple(conv_patch_embed_stride) if use_2d_patch else conv_patch_embed_stride
+    grid = [in_dims[i] // in_stride[i] for i in range(3)] if enable_patch_embed else in_dims
     pos = SpatioTemporalClsPositionalEncoding(embed_dim=patch_embed_dim, patch_embed_shape=grid,
                                               sep_pos_embed=sep_pos_embed, has_cls=cls_embed_on)
     dpr = [x.item() for x in torch.linspace(0, droppath_rate_block, depth)]

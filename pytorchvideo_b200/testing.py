@@ -147,6 +147,24 @@ def build_case(case, hub_module, weight_seed=1234, input_seed=42):
     return model, (slowfast_inputs(clip) if is_sf else clip), is_sf
 
 
+# The image MViT and SlowFast-16x8-R101-50-50 hub entries -> tests/golden/hub_tail.pt (oracle/gen_golden_hub.py).
+# name: (batch, input shape per sample); the SlowFast input is a 64-frame clip split into 16 Slow + 64 Fast frames.
+HUB_TAIL_CASES = {
+    "mvit_base_16": (2, (3, 224, 224)),
+    "slowfast_16x8_r101_50_50": (1, (3, 64, 224, 224)),
+}
+
+
+def build_hub_tail_case(case, hub_module, weight_seed=1234, input_seed=42):
+    """(model, input) of a HUB_TAIL_CASES entry, built from ``hub_module``: an image batch (B, 3, H, W) for the image
+    MViT, the [slow, fast] pathway list for the SlowFast."""
+    B, shape = HUB_TAIL_CASES[case]
+    model = randomize_model(getattr(hub_module, case)(), seed=weight_seed).eval()
+    if len(shape) == 3:
+        return model, synthetic_clip(B, 1, shape[1], shape[2], seed=input_seed)[:, :, 0].contiguous()
+    return model, slowfast_inputs(synthetic_clip(B, shape[1], shape[2], shape[3], seed=input_seed))
+
+
 # Grouped conv_b (ResNeXt-style group counts, CSN with several channels per group): the builders' own arguments on the
 # hub entries.  Kept apart from MODEL_CASES, whose host lowering test counts every groups > 1 conv as depthwise.
 # name: (hub builder name, kwargs, batch, T, H, W, is_slowfast, f16_grid) -> tests/golden/model_grouped_<name>.pt
