@@ -299,6 +299,17 @@ typedef struct pv_conv3d_desc {
   const void* addend;
   long long add_n_stride, add_t_stride;
   int add_ch_off;
+  /* Pre-activation prologue of the depthwise entry points (the BatchNorm3d + GELU that MViT's attention pools apply
+   * before a depthwise pooling conv, layers/attention.py:189-197):
+   *   y[c] = scale[c] * sum_taps w[tap][c] * u(x_tap) + bias[c],  u(x) = act(pre_act, pre_scale[c] * x + pre_bias[c])
+   * for in-bounds taps and u = 0 for padded taps (normalise, activate, then zero-pad).  fp32 vectors of Co values.  Set
+   * by pre_scale != NULL; pre_bias must then be non-NULL too, and pre_act is a pv_act code applied to every in-bounds
+   * input once.  pv_dwconv3d_fwd and pv_dwplane_fwd honour it on every kernel they dispatch to; pv_conv3d_fwd and the
+   * stem entry points return PV_ERR_UNSUPPORTED when it is set.  NULL = no prologue (a zero-initialised descriptor
+   * behaves as without these fields).                                                                              */
+  const float* pre_scale;
+  const float* pre_bias;
+  int pre_act;
 } pv_conv3d_desc;
 
 /* Temporal tap reduction used to factor a (kt,kh,kw) stem convolution with few output channels into

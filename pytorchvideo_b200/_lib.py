@@ -81,7 +81,8 @@ class Conv3dDesc(C.Structure):
                 ("x_row_stride", c_ll), ("y_row_stride", c_ll), ("res_row_stride", c_ll),
                 ("ci_pad64", C.c_int), ("x_w_pad", C.c_int), ("x_w_phys", C.c_int),
                 ("x_batch_stride", c_ll), ("y_batch_stride", c_ll),
-                ("addend", c_vp), ("add_n_stride", c_ll), ("add_t_stride", c_ll), ("add_ch_off", C.c_int)]
+                ("addend", c_vp), ("add_n_stride", c_ll), ("add_t_stride", c_ll), ("add_ch_off", C.c_int),
+                ("pre_scale", c_vp), ("pre_bias", c_vp), ("pre_act", C.c_int)]
 
 
 class Pool3dDesc(C.Structure):

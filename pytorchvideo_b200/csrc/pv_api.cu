@@ -85,7 +85,7 @@ extern "C" int pv_device_info(int* sm_count, int* cc) {
 }
 
 extern "C" int pv_conv3d_tcgen05_supported(const pv_conv3d_desc* d) {
-  if (!d || !pv::act_known(d->act)) return 0;
+  if (!d || !pv::act_known(d->act) || pv::conv3d_has_prologue(d)) return 0;
   if (pv::wants_gather(d)) return pv::conv3d_gather_supported(d);
   return pv::conv3d_tcgen05_supported(d, nullptr, 0);
 }
@@ -107,6 +107,10 @@ extern "C" int pv_conv3d_fwd(const pv_conv3d_desc* d, int algo, const void* x, c
                              void* stream) {
   int rc = pv::conv3d_check(d);
   if (rc != PV_OK) return rc;
+  if (pv::conv3d_has_prologue(d)) {
+    pv::set_error("pv_conv3d_fwd takes no pre-activation prologue (pv_dwconv3d_fwd / pv_dwplane_fwd do)");
+    return PV_ERR_UNSUPPORTED;
+  }
   PV_CHECK_ARG(x && w && scale && bias && y, "null pointer");
   PV_CHECK_ARG(!d->has_residual || residual, "has_residual set but residual is null");
   cudaStream_t s = (cudaStream_t)stream;

@@ -183,4 +183,43 @@ __device__ __forceinline__ float apply_act(float x, int act) {
 // kernel ever sees one.
 inline bool act_known(int act) { return act >= PV_ACT_NONE && act <= PV_ACT_HSWISH; }
 
+// ---- pre-activation prologue of the depthwise kernels (pv_conv3d_desc.pre_scale / pre_bias / pre_act) -------------
+inline bool conv3d_has_prologue(const pv_conv3d_desc* d) { return d->pre_scale || d->pre_bias || d->pre_act; }
+inline bool conv3d_prologue_ok(const pv_conv3d_desc* d) {
+  return !conv3d_has_prologue(d) || (d->pre_scale && d->pre_bias && act_known(d->pre_act));
+}
+// Launch-ledger name of a kernel instance with / without the prologue: "<base>>" or "<base>,pre>".
+#define PV_PRE_NAME(base, pre) ((pre) ? base ",pre>" : base ">")
+
+__device__ __forceinline__ float pre_u(float x, float s, float b, int act) { return apply_act(fmaf(s, x, b), act); }
+
+// The prologue in place on a landed f16 halo box [outer][tt][hh][ww][cc]: element (t, h, w, c) of every outer slice is
+// input position (t0 + t, h0 + h, w0 + w), channel c0 + c.  Only in-bounds positions of channels < C are transformed:
+// the rest is the TMA zero fill, i.e. the convolution's zero padding, which must stay 0 although u(0) != 0.  A thread
+// keeps one channel pair (its prologue constants in registers) and walks whole halo rows, so the index arithmetic is
+// paid once per row; consecutive threads touch consecutive 4-byte words.  Each element is transformed once and rounded
+// to f16; the caller synchronises the CTA before the stencil reads the box.
+__device__ __forceinline__ void halo_prologue(__half* xs, int outer, int tt, int hh, int ww, int cc, int c0, int C,
+                                              int t0, int h0, int w0, int Ti, int Hi, int Wi,
+                                              const float* __restrict__ ps, const float* __restrict__ pb, int act) {
+  const int cp = cc >> 1;
+  const int nrow = blockDim.x / cp;
+  const int ci = threadIdx.x % cp, r0 = threadIdx.x / cp;
+  const int ch = c0 + 2 * ci;
+  if (r0 >= nrow || ch >= C) return;
+  const float s0 = __ldg(ps + ch), s1 = __ldg(ps + ch + 1), b0 = __ldg(pb + ch), b1 = __ldg(pb + ch + 1);
+  const int wlo = max(0, -w0), whi = min(ww, Wi - w0);
+  __half2* x2 = reinterpret_cast<__half2*>(xs) + ci;
+  const int rows = outer * tt * hh;
+  for (int r = r0; r < rows; r += nrow) {
+    const int h = r % hh, t = (r / hh) % tt;
+    if ((unsigned)(t0 + t) >= (unsigned)Ti || (unsigned)(h0 + h) >= (unsigned)Hi) continue;
+    __half2* row = x2 + r * ww * cp;
+    for (int w = wlo; w < whi; ++w) {
+      const float2 v = __half22float2(row[w * cp]);
+      row[w * cp] = __floats2half2_rn(pre_u(v.x, s0, b0, act), pre_u(v.y, s1, b1, act));
+    }
+  }
+}
+
 }  // namespace pv

@@ -39,9 +39,14 @@ struct DwParams {
   int kt, kh, st, sh, pt, ph, pw, dt, dh;
   int act;
   long long y_row_stride, y_batch_stride;
+  int Ti, Hi, Wi;             // input extent (bounds of the prologue)
+  const float* pre_scale;     // PRE: pre-activation prologue (pv_conv3d_desc.pre_*)
+  const float* pre_bias;
+  int pre_act;
 };
 
-template <int KW, int SW>
+// PRE: the pre-activation prologue runs once over the landed halo box (in-bounds positions only), before the stencil.
+template <int KW, int SW, bool PRE>
 __global__ void __launch_bounds__(256)
 dwconv3d_tile_kernel(const __grid_constant__ DwParams P, const __half* __restrict__ w,
                      const float* __restrict__ scale, const float* __restrict__ bias,
@@ -83,6 +88,11 @@ dwconv3d_tile_kernel(const __grid_constant__ DwParams P, const __half* __restric
   }
   __syncthreads();
   mbar_wait(bar_a, 0);
+  if constexpr (PRE) {
+    halo_prologue(xs, 1, P.tt, P.hh, P.ww, cc, c0, P.C, to0 * P.st - P.pt, ho0 * P.sh - P.ph, wo0 * SW - P.pw, P.Ti,
+                  P.Hi, P.Wi, P.pre_scale, P.pre_bias, P.pre_act);
+    __syncthreads();
+  }
 
   const int G = cc >> 3;
   const int wq_n = (P.bw + WT - 1) / WT;
@@ -240,6 +250,7 @@ dwconv_temporal_kernel(const __half* __restrict__ x, const __half* __restrict__ 
 int dwconv3d_temporal_launch(const pv_conv3d_desc* d, const void* x, const void* w, const float* scale,
                              const float* bias, void* y, float* se_sums, cudaStream_t stream) {
   if (se_sums || d->dtype != PV_F16 || d->groups != d->Ci || d->Ci != d->Co || d->has_residual) return PV_ERR_UNSUPPORTED;
+  if (conv3d_has_prologue(d)) return PV_ERR_UNSUPPORTED;      // the tile kernel and the stencils take the prologue
   if (d->kh != 1 || d->kw != 1 || !(d->kt == 3 || d->kt == 5) || d->st != 1 || d->sh != 1 || d->sw != 1 || d->dt != 1)
     return PV_ERR_UNSUPPORTED;
   if (d->pt != d->kt / 2 || d->ph != 0 || d->pw != 0 || d->Co % 8 || d->x_row_stride % 8 || d->y_row_stride % 8)
@@ -284,6 +295,9 @@ int dwconv3d_tile_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   P.To = d->To; P.Ho = d->Ho; P.Wo = d->Wo;
   P.kt = d->kt; P.kh = d->kh; P.st = d->st; P.sh = d->sh; P.pt = d->pt; P.ph = d->ph; P.pw = d->pw;
   P.dt = d->dt; P.dh = d->dh; P.act = d->act;
+  P.Ti = d->Ti; P.Hi = d->Hi; P.Wi = d->Wi;
+  P.pre_scale = d->pre_scale; P.pre_bias = d->pre_bias; P.pre_act = d->pre_act;
+  const bool pre = d->pre_scale != nullptr;
   P.y_row_stride = d->y_row_stride;
   P.y_batch_stride = d->y_batch_stride ? d->y_batch_stride : (long long)d->To * d->Ho * d->Wo * d->y_row_stride;
   // ---- output box search: maximise outputs per halo byte under a 96 KiB halo budget
@@ -329,17 +343,24 @@ int dwconv3d_tile_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   const int halo_elems = P.tt * P.hh * P.ww * P.cc;
   const size_t smem = (size_t)(((halo_elems + 63) & ~63) + d->kt * d->kh * d->kw * P.cc) * 2 + 128;
   dim3 grid((unsigned)tiles, (unsigned)chunks), block(256);
+#define PV_DWT2(KW_, SW_, PRE_)                                                                               \
+  do {                                                                                                        \
+    PV_OPT_IN_SMEM((dwconv3d_tile_kernel<KW_, SW_, PRE_>), 110 * 1024);                                       \
+    dwconv3d_tile_kernel<KW_, SW_, PRE_><<<grid, block, smem, stream>>>(P, (const __half*)w, scale, bias, (__half*)y, \
+                                                                        se_sums);                             \
+    if (PRE_) PV_LAUNCH_OK("dwconv3d_tile_kernel<" #KW_ "," #SW_ ",pre>");                                    \
+    else PV_LAUNCH_OK("dwconv3d_tile_kernel<" #KW_ "," #SW_ ">");                                             \
+  } while (0)
 #define PV_DWT(KW_, SW_)                                                                                      \
   do {                                                                                                        \
-    PV_OPT_IN_SMEM((dwconv3d_tile_kernel<KW_, SW_>), 110 * 1024);                                             \
-    dwconv3d_tile_kernel<KW_, SW_><<<grid, block, smem, stream>>>(P, (const __half*)w, scale, bias, (__half*)y, se_sums); \
-    PV_LAUNCH_OK("dwconv3d_tile_kernel<" #KW_ "," #SW_ ">");                                                  \
+    if (pre) PV_DWT2(KW_, SW_, true); else PV_DWT2(KW_, SW_, false);                                          \
   } while (0)
   if (d->kw == 3 && d->sw == 1) PV_DWT(3, 1);
   else if (d->kw == 3) PV_DWT(3, 2);
   else if (d->sw == 1) PV_DWT(1, 1);
   else PV_DWT(1, 2);
 #undef PV_DWT
+#undef PV_DWT2
   return PV_OK;
 }
 

@@ -40,6 +40,10 @@ struct DwLaneParams {
   int st, pt, ph, pw;         // temporal stride, paddings
   int act;
   long long y_row_stride, y_batch_stride;
+  int Ti, Hi, Wi;             // input extent (bounds of the prologue)
+  const float* pre_scale;     // PRE: pre-activation prologue (pv_conv3d_desc.pre_*)
+  const float* pre_bias;
+  int pre_act;
 };
 
 
@@ -48,8 +52,9 @@ __device__ __forceinline__ float2 fma_x2(float2 a, float2 b, float2 c) {
   return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
 
-// NW warps per CTA: 8 (two 100 KB CTAs per SM) or 4 (four 50 KB CTAs per SM - more CTAs to stagger the TMA waits)
-template <int S, int PH, int PW, bool X2, int NW>
+// NW warps per CTA: 8 (two 100 KB CTAs per SM) or 4 (four 50 KB CTAs per SM - more CTAs to stagger the TMA waits).
+// PRE: the pre-activation prologue runs once over the landed halo box (in-bounds positions only), before the stencil.
+template <int S, int PH, int PW, bool X2, int NW, bool PRE>
 __global__ void __launch_bounds__(NW * 32, 16 / NW)
 dwconv3d_lane_kernel(const __grid_constant__ DwLaneParams P, const __half* __restrict__ w,
                      const float* __restrict__ scale, const float* __restrict__ bias,
@@ -89,6 +94,11 @@ dwconv3d_lane_kernel(const __grid_constant__ DwLaneParams P, const __half* __res
   const int lane_off = live ? 2 * lane : 0;
   __syncthreads();          // barrier initialised before anyone waits on it
   mbar_wait(bar_a, 0);
+  if constexpr (PRE) {
+    halo_prologue(reinterpret_cast<__half*>(dwl_smem), 1, P.tt, P.hh, P.ww, cc, c0, P.C, to0 * P.st - P.pt,
+                  ho0 * S - P.ph, wo0 * S - P.pw, P.Ti, P.Hi, P.Wi, P.pre_scale, P.pre_bias, P.pre_act);
+    __syncthreads();
+  }
 
   const int npw = P.bw / PW, nph = P.bh / PH;
   const int total = P.bt * nph * npw;
@@ -191,6 +201,9 @@ int dwconv3d_lane_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   P.st = d->st; P.pt = d->pt; P.ph = d->ph; P.pw = d->pw; P.act = d->act;
   P.y_row_stride = d->y_row_stride;
   P.y_batch_stride = d->y_batch_stride ? d->y_batch_stride : (long long)d->To * d->Ho * d->Wo * d->y_row_stride;
+  P.Ti = d->Ti; P.Hi = d->Hi; P.Wi = d->Wi;
+  P.pre_scale = d->pre_scale; P.pre_bias = d->pre_bias; P.pre_act = d->pre_act;
+  const bool pre = d->pre_scale != nullptr;
   // patch shape: 4x4 unless the plane is a multiple of 7 wide but not of 4 (14x14, 7x7 planes): 2x7
   const bool p27 = (d->Wo % 4 != 0) && (d->Wo % 7 == 0);
   const int PH = p27 ? 2 : 4, PW = p27 ? 7 : 4;
@@ -239,12 +252,16 @@ int dwconv3d_lane_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   const size_t smem = (size_t)P.tt * P.hh * P.ww * P.cc * 2 + 256;
   dim3 grid((unsigned)tiles, (unsigned)chunks), block(nw * 32);
   static const bool x2 = [] { const char* e = getenv("PVB200_DW_X2"); return !(e && e[0] == '0'); }();
+#define PV_DWL3(S_, PH_, PW_, X2_, NW_, PRE_)                                                                  \
+  do {                                                                                                        \
+    PV_OPT_IN_SMEM((dwconv3d_lane_kernel<S_, PH_, PW_, X2_, NW_, PRE_>), 110 * 1024);                         \
+    dwconv3d_lane_kernel<S_, PH_, PW_, X2_, NW_, PRE_><<<grid, block, smem, stream>>>(P, (const __half*)w,     \
+                                                                  scale, bias, (__half*)y, se_sums);          \
+    PV_LAUNCH_OK(PV_PRE_NAME("dwconv3d_lane_kernel<" #S_ "," #PH_ "," #PW_ "," #X2_ "," #NW_, PRE_));         \
+  } while (0)
 #define PV_DWL2(S_, PH_, PW_, X2_, NW_)                                                                       \
   do {                                                                                                        \
-    PV_OPT_IN_SMEM((dwconv3d_lane_kernel<S_, PH_, PW_, X2_, NW_>), 110 * 1024);                               \
-    dwconv3d_lane_kernel<S_, PH_, PW_, X2_, NW_><<<grid, block, smem, stream>>>(P, (const __half*)w, scale,   \
-                                                                               bias, (__half*)y, se_sums);    \
-    PV_LAUNCH_OK("dwconv3d_lane_kernel<" #S_ "," #PH_ "," #PW_ "," #X2_ "," #NW_ ">");                       \
+    if (pre) PV_DWL3(S_, PH_, PW_, X2_, NW_, true); else PV_DWL3(S_, PH_, PW_, X2_, NW_, false);              \
   } while (0)
 #define PV_DWL(S_, PH_, PW_)                                                                                  \
   do {                                                                                                        \
@@ -257,6 +274,7 @@ int dwconv3d_lane_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   else PV_DWL(2, 2, 7);
 #undef PV_DWL
 #undef PV_DWL2
+#undef PV_DWL3
   return PV_OK;
 }
 

@@ -38,11 +38,16 @@ struct DwPlaneParams {
   const __half* x;            // stride 4 only: x read straight from global memory
   int Hi, Wi;
   long long x_row_stride, x_batch_stride;
+  const float* pre_scale;     // PRE: pre-activation prologue (pv_conv3d_desc.pre_*)
+  const float* pre_bias;
+  int pre_act;
 };
 
 constexpr int kPlaneWarps = 4;
 
-template <int S, int PH, int PW>
+// PRE: the pre-activation prologue, once per input element: over the landed halo box (in-bounds positions only), or at
+// stride 4, where every input position feeds at most one output, on each tap as it is loaded.
+template <int S, int PH, int PW, bool PRE>
 __global__ void __launch_bounds__(kPlaneWarps * 32, 4)
 dwconv_plane_kernel(const __grid_constant__ DwPlaneParams P, const __half* __restrict__ w,
                     const float* __restrict__ scale, const float* __restrict__ bias, __half* __restrict__ y) {
@@ -80,6 +85,16 @@ dwconv_plane_kernel(const __grid_constant__ DwPlaneParams P, const __half* __res
   if constexpr (S != 4) {
     __syncthreads();          // barrier initialised before anyone waits on it
     mbar_wait(bar_a, 0);
+    if constexpr (PRE) {
+      halo_prologue(reinterpret_cast<__half*>(dwp_smem), P.bn, 1, P.hh, P.ww, cc, c0, P.C, 0, ho0 * S - P.ph,
+                    wo0 * S - P.pw, 1, P.Hi, P.Wi, P.pre_scale, P.pre_bias, P.pre_act);
+      __syncthreads();
+    }
+  }
+  float2 pps = make_float2(1.f, 1.f), ppb = make_float2(0.f, 0.f);
+  if (PRE && S == 4 && live) {
+    pps = make_float2(__ldg(P.pre_scale + ch), __ldg(P.pre_scale + ch + 1));
+    ppb = make_float2(__ldg(P.pre_bias + ch), __ldg(P.pre_bias + ch + 1));
   }
 
   const int npw = P.bw / PW, nph = P.bh / PH;
@@ -112,8 +127,12 @@ dwconv_plane_kernel(const __grid_constant__ DwPlaneParams P, const __half* __res
               for (int kw = 0; kw < 3; ++kw) {
                 const int wi = (wo0 + pwi * PW + b) * 4 - P.pw + kw;
                 if (wi < 0 || wi >= P.Wi) continue;
-                const float2 xv = __half22float2(
+                float2 xv = __half22float2(
                     __ldg(reinterpret_cast<const __half2*>(xn + ((long long)h * P.Wi + wi) * P.x_row_stride)));
+                if constexpr (PRE) {
+                  xv.x = pre_u(xv.x, pps.x, ppb.x, P.pre_act);
+                  xv.y = pre_u(xv.y, pps.y, ppb.y, P.pre_act);
+                }
                 acc[a][b].x = fmaf(xv.x, wr[kh * 3 + kw].x, acc[a][b].x);
                 acc[a][b].y = fmaf(xv.y, wr[kh * 3 + kw].y, acc[a][b].y);
               }
@@ -188,6 +207,7 @@ extern "C" int pv_dwplane_fwd(const pv_conv3d_desc* d, const void* x, const void
   PV_CHECK_ARG(d && x && w && scale && bias && y, "null pointer");
   PV_CHECK_ARG(((uintptr_t)x & 15) == 0 && ((uintptr_t)y & 3) == 0 && ((uintptr_t)w & 3) == 0,
                "pv_dwplane_fwd: x must be 16-byte and y, w 4-byte aligned");
+  PV_CHECK_ARG(conv3d_prologue_ok(d), "prologue: pre_scale and pre_bias both set, pre_act a known activation code");
   if (!dwplane_takes(d)) {
     set_error("pv_dwplane_fwd: f16 depthwise (1,3,3) on a one-frame plane, sh == sw in {1, 2, 4}, padding <= 2, "
               "no activation, channels and row / batch strides multiples of 8 (got k=(%d,%d,%d) s=(%d,%d,%d) T=%d)",
@@ -210,6 +230,8 @@ extern "C" int pv_dwplane_fwd(const pv_conv3d_desc* d, const void* x, const void
   P.x = (const __half*)x; P.Hi = d->Hi; P.Wi = d->Wi;
   P.x_row_stride = d->x_row_stride;
   P.x_batch_stride = d->x_batch_stride ? d->x_batch_stride : (long long)d->Hi * d->Wi * d->x_row_stride;
+  P.pre_scale = d->pre_scale; P.pre_bias = d->pre_bias; P.pre_act = d->pre_act;
+  const bool pre = d->pre_scale != nullptr;
   // patch shape: 4x4 unless the plane is a multiple of 7 wide but not of 4 (14x14, 7x7 planes): 2x7
   // stride 4 (loads straight from global memory): 1x2 patches, so enough warps are in flight to hide the latency
   const bool p27 = (d->Wo % 4 != 0) && (d->Wo % 7 == 0);
@@ -258,11 +280,17 @@ extern "C" int pv_dwplane_fwd(const pv_conv3d_desc* d, const void* x, const void
   const size_t smem = S == 4 ? 256 : (size_t)P.bn * P.hh * P.ww * P.cc * 2 + 256;
   dim3 grid((unsigned)tiles, (unsigned)chunks), block(kPlaneWarps * 32);
   cudaStream_t s = (cudaStream_t)stream;
+#define PV_DWP2(S_, PH_, PW_, PRE_)                                                                           \
+  do {                                                                                                        \
+    PV_OPT_IN_SMEM((dwconv_plane_kernel<S_, PH_, PW_, PRE_>), 52 * 1024);                                     \
+    dwconv_plane_kernel<S_, PH_, PW_, PRE_><<<grid, block, smem, s>>>(P, (const __half*)w, scale, bias,        \
+                                                                      (__half*)y);                            \
+    if (PRE_) PV_LAUNCH_OK("dwconv_plane_kernel<" #S_ "," #PH_ "," #PW_ ",pre>");                             \
+    else PV_LAUNCH_OK("dwconv_plane_kernel<" #S_ "," #PH_ "," #PW_ ">");                                      \
+  } while (0)
 #define PV_DWP(S_, PH_, PW_)                                                                                  \
   do {                                                                                                        \
-    PV_OPT_IN_SMEM((dwconv_plane_kernel<S_, PH_, PW_>), 52 * 1024);                                           \
-    dwconv_plane_kernel<S_, PH_, PW_><<<grid, block, smem, s>>>(P, (const __half*)w, scale, bias, (__half*)y); \
-    PV_LAUNCH_OK("dwconv_plane_kernel<" #S_ "," #PH_ "," #PW_ ">");                                           \
+    if (pre) PV_DWP2(S_, PH_, PW_, true); else PV_DWP2(S_, PH_, PW_, false);                                  \
   } while (0)
   if (S == 1 && !p27) PV_DWP(1, 4, 4);
   else if (S == 1) PV_DWP(1, 2, 7);
@@ -270,5 +298,6 @@ extern "C" int pv_dwplane_fwd(const pv_conv3d_desc* d, const void* x, const void
   else if (S == 2) PV_DWP(2, 2, 7);
   else PV_DWP(4, 1, 2);
 #undef PV_DWP
+#undef PV_DWP2
   return PV_OK;
 }

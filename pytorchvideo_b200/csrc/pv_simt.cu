@@ -221,7 +221,8 @@ conv3d_direct_kernel(pv_conv3d_desc d, const T* __restrict__ x, const T* __restr
 // consecutive lanes walk the channel groups of a position, then the next position, so every
 // warp-level load is a run of consecutive 16-byte vectors (coalesced in NDHWC).
 // =============================================================================================
-template <typename T>
+// PRE: pv_conv3d_desc's pre-activation prologue on every in-bounds input value as it is loaded (kept in fp32).
+template <typename T, bool PRE>
 __global__ void __launch_bounds__(256)
 dwconv3d_kernel(pv_conv3d_desc d, const T* __restrict__ x, const T* __restrict__ w,
                 const float* __restrict__ scale, const float* __restrict__ bias,
@@ -240,9 +241,13 @@ dwconv3d_kernel(pv_conv3d_desc d, const T* __restrict__ x, const T* __restrict__
   const long long ybs = d.y_batch_stride ? d.y_batch_stride : (long long)d.To * d.Ho * d.Wo * d.y_row_stride;
   const long long mo = (((long long)to) * d.Ho + ho) * d.Wo + wo;   // position inside the sample
 
-  float acc[8];
+  float acc[8], ps[8], pb[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+  for (int i = 0; i < 8; ++i) {
+    acc[i] = 0.f;
+    ps[i] = PRE ? __ldg(d.pre_scale + c + i) : 1.f;
+    pb[i] = PRE ? __ldg(d.pre_bias + c + i) : 0.f;
+  }
 
   for (int kt_ = 0; kt_ < d.kt; ++kt_) {
     const int ti = t0 + kt_ * d.dt;
@@ -258,6 +263,10 @@ dwconv3d_kernel(pv_conv3d_desc d, const T* __restrict__ x, const T* __restrict__
         float xv[8], wv[8];
         ld8<T>(row + (long long)wi * d.x_row_stride, xv);
         ld8<T>(wrow + (long long)kw_ * d.Co, wv);
+        if constexpr (PRE) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) xv[i] = pre_u(xv[i], ps[i], pb[i], d.pre_act);
+        }
 #pragma unroll
         for (int i = 0; i < 8; ++i) acc[i] = fmaf(xv[i], wv[i], acc[i]);
       }
@@ -281,7 +290,9 @@ dwconv3d_kernel(pv_conv3d_desc d, const T* __restrict__ x, const T* __restrict__
 // (kt,kh) filter row the KW weight vectors are converted once and every input column is loaded and
 // converted once and used by all outputs it feeds - 2.7x fewer loads and half the instructions of the
 // one-output-per-thread kernel for the 3x3x3 / stride-1 case (X3D, CSN, MViT pooling).
-template <typename T, int KW, int SW>
+// PRE: the pre-activation prologue on every in-bounds input column as it is loaded (once per column and filter row,
+// kept in fp32).
+template <typename T, int KW, int SW, bool PRE>
 __global__ void __launch_bounds__(128)
 dwconv3d_w4_kernel(pv_conv3d_desc d, const T* __restrict__ x, const T* __restrict__ w,
                    const float* __restrict__ scale, const float* __restrict__ bias, T* __restrict__ y,
@@ -300,11 +311,16 @@ dwconv3d_w4_kernel(pv_conv3d_desc d, const T* __restrict__ x, const T* __restric
   const int t0 = to * d.st - d.pt, h0 = ho * d.sh - d.ph, w0 = wo0 * SW - d.pw;
   const long long xbs = d.x_batch_stride ? d.x_batch_stride : (long long)d.Ti * d.Hi * d.Wi * d.x_row_stride;
   const long long ybs = d.y_batch_stride ? d.y_batch_stride : (long long)d.To * d.Ho * d.Wo * d.y_row_stride;
-  float acc[WT][8];
+  float acc[WT][8], ps[8], pb[8];
 #pragma unroll
   for (int o = 0; o < WT; ++o)
 #pragma unroll
     for (int i = 0; i < 8; ++i) acc[o][i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    ps[i] = PRE ? __ldg(d.pre_scale + c + i) : 1.f;
+    pb[i] = PRE ? __ldg(d.pre_bias + c + i) : 0.f;
+  }
   for (int kt_ = 0; kt_ < d.kt; ++kt_) {
     const int ti = t0 + kt_ * d.dt;
     if ((unsigned)ti >= (unsigned)d.Ti) continue;
@@ -322,6 +338,10 @@ dwconv3d_w4_kernel(pv_conv3d_desc d, const T* __restrict__ x, const T* __restric
         if ((unsigned)wi >= (unsigned)d.Wi) continue;
         float xv[8];
         ld8<T>(row + (long long)wi * d.x_row_stride, xv);
+        if constexpr (PRE) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) xv[i] = pre_u(xv[i], ps[i], pb[i], d.pre_act);
+        }
 #pragma unroll
         for (int o = 0; o < WT; ++o) {
           const int k = j - o * SW;          // tap index this column has for output o (compile-time)
@@ -1028,6 +1048,7 @@ int conv3d_check(const pv_conv3d_desc* d) {
   PV_CHECK_ARG(!d->has_residual || d->res_row_stride >= d->Co, "residual row stride < Co");
   PV_CHECK_ARG(conv3d_addend_ok(d), "addend: 16-byte aligned pointer and non-negative strides / channel offset that "
                "are multiples of 8 elements required");
+  PV_CHECK_ARG(conv3d_prologue_ok(d), "prologue: pre_scale and pre_bias both set, pre_act a known activation code");
   return PV_OK;
 }
 
@@ -1040,6 +1061,10 @@ int conv3d_direct_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   if (M == 0) return PV_OK;
   const int esz = d->dtype == PV_F16 ? 2 : 4;
   if (d->groups == 1) {
+    if (conv3d_has_prologue(d)) {
+      set_error("the pre-activation prologue is taken by depthwise convolutions only");
+      return PV_ERR_UNSUPPORTED;
+    }
     PV_CHECK_ARG(d->Ci % 4 == 0 && d->Co % 4 == 0, "direct conv needs Ci%%4==0 && Co%%4==0");
     PV_CHECK_ARG((d->x_row_stride * esz) % (4 * esz) == 0 && (d->y_row_stride % 4) == 0,
                  "row strides must be multiples of 4 elements");
@@ -1064,6 +1089,7 @@ int conv3d_direct_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
       return PV_ERR_UNSUPPORTED;
     }
     PV_CHECK_ARG(d->Co % 8 == 0, "depthwise conv needs C%%8==0");
+    const bool pre = d->pre_scale != nullptr;
     PV_CHECK_ARG(d->x_row_stride % 8 == 0 && d->y_row_stride % 8 == 0, "row strides must be multiples of 8");
     // TMA-fed shared-memory stencil (pv_dwconv.cu) whenever it applies
     if (!d->has_residual && d->dtype == PV_F16 && !getenv("PVB200_DW_SIMT")) {
@@ -1075,10 +1101,15 @@ int conv3d_direct_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
       const int wo4 = (d->Wo + 3) / 4;
       const long long tot4 = (long long)d->N * d->To * d->Ho * wo4 * (d->Co / 8);
       dim3 g4((unsigned)cdiv(tot4, 128)), b4(128);
+#define PV_DW2(TT, KW_, SW_, PRE_)                                                                                     \
+  do {                                                                                                                 \
+    dwconv3d_w4_kernel<TT, KW_, SW_, PRE_><<<g4, b4, 0, s>>>(*d, (const TT*)x, (const TT*)w, scale, bias, (TT*)y, tot4, \
+                                                             wo4);                                                     \
+    PV_LAUNCH_OK(PV_PRE_NAME("dwconv3d_w4_kernel<" #TT "," #KW_ "," #SW_, PRE_));                                      \
+  } while (0)
 #define PV_DW(TT, KW_, SW_)                                                                                            \
   do {                                                                                                                 \
-    dwconv3d_w4_kernel<TT, KW_, SW_><<<g4, b4, 0, s>>>(*d, (const TT*)x, (const TT*)w, scale, bias, (TT*)y, tot4, wo4); \
-    PV_LAUNCH_OK("dwconv3d_w4_kernel<" #TT "," #KW_ "," #SW_ ">");                                                     \
+    if (pre) PV_DW2(TT, KW_, SW_, true); else PV_DW2(TT, KW_, SW_, false);                                             \
   } while (0)
       if (d->dtype == PV_F16) {
         if (d->kw == 3 && d->sw == 1) PV_DW(__half, 3, 1); else if (d->kw == 3) PV_DW(__half, 3, 2);
@@ -1088,19 +1119,23 @@ int conv3d_direct_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
         else if (d->sw == 1) PV_DW(float, 1, 1); else PV_DW(float, 1, 2);
       }
 #undef PV_DW
+#undef PV_DW2
       return PV_OK;
     }
     const long long total = M * (d->Co / 8);
     dim3 grid((unsigned)cdiv(total, 256)), block(256);
+#define PV_DWG(TT, PRE_)                                                                                               \
+  do {                                                                                                                 \
+    dwconv3d_kernel<TT, PRE_><<<grid, block, 0, s>>>(*d, (const TT*)x, (const TT*)w, scale, bias, (const TT*)residual, \
+                                                     (TT*)y, total);                                                   \
+    PV_LAUNCH_OK(PV_PRE_NAME("dwconv3d_kernel<" #TT, PRE_));                                                           \
+  } while (0)
     if (d->dtype == PV_F16) {
-      dwconv3d_kernel<__half><<<grid, block, 0, s>>>(*d, (const __half*)x, (const __half*)w, scale, bias,
-                                                  (const __half*)residual, (__half*)y, total);
-      PV_LAUNCH_OK("dwconv3d_kernel<__half>");
+      if (pre) PV_DWG(__half, true); else PV_DWG(__half, false);
     } else {
-      dwconv3d_kernel<float><<<grid, block, 0, s>>>(*d, (const float*)x, (const float*)w, scale, bias,
-                                                 (const float*)residual, (float*)y, total);
-      PV_LAUNCH_OK("dwconv3d_kernel<float>");
+      if (pre) PV_DWG(float, true); else PV_DWG(float, false);
     }
+#undef PV_DWG
   }
   return PV_OK;
 }

@@ -186,6 +186,7 @@ using namespace pv;
 // (x_w_pad, x_w_phys, ci_pad64 = window length) but the weights are packed [K / 8][N16][8] (engine/packing.py).
 extern "C" int pv_conv3d_stem_rows_supported(const pv_conv3d_desc* d) {
   if (!d || d->dtype != PV_F16 || d->groups != 1 || d->has_residual || !act_known(d->act)) return 0;
+  if (conv3d_has_prologue(d)) return 0;
   if (d->Ci != 4 || d->sw != 2 || d->dw != 1 || d->x_w_pad <= 0 || d->x_row_stride != 4) return 0;
   if (d->x_w_pad < d->pw || (d->x_w_phys * 8) % 16) return 0;
   const int lead = stem_window_lead(d);

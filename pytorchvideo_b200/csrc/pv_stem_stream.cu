@@ -242,6 +242,7 @@ using namespace pv;
 // (kw 5..7), and no addend.  Weights f16 [kh * win / 8][40][8] (engine/packing.py pack_stem_stream).
 extern "C" int pv_conv3d_stem_stream_supported(const pv_conv3d_desc* d) {
   if (!d || d->dtype != PV_F16 || d->groups != 1 || d->has_residual || d->addend || !act_known(d->act)) return 0;
+  if (conv3d_has_prologue(d)) return 0;
   if (d->Ci != 4 || d->sw != 2 || d->dw != 1 || d->x_w_pad <= 0 || d->x_row_stride != 4) return 0;
   if (d->x_w_pad < d->pw || (d->x_w_phys * 8) % 16) return 0;
   if (d->Co != SS_CO || d->kt != 5 || d->st != 1 || d->dt != 1 || d->pt < 0 || d->pt >= d->kt) return 0;

@@ -855,12 +855,33 @@ def _check_thw(x, thw, has_cls, name):
     return (T, H, W)
 
 
-def _lower_mvit_attention(low, attn, xn, thw, name, residual=None):
-    """MultiScaleAttention.forward (layers/attention.py:467-544) on normalised tokens ``xn``:
-    returns (proj(attention) [+ residual fused into the GEMM epilogue], pooled q thw)."""
+def _folded(weight, bias, fold):
+    """A Linear that consumes ``s * x + t`` (an eval BatchNorm1d folded away, ``fold = (s, t)``) as one on x:
+    W diag(s), W t + bias."""
+    if fold is None:
+        return weight, bias
+    s, t = fold
+    w = weight.detach().float().cpu()
+    b = w @ t + (bias.detach().float().cpu() if bias is not None else 0.0)
+    return w * s[None, :], b
+
+
+def _attention_pool(attn, branch):
+    """(pool, norm, norm_before_pool) of the _AttentionPool wrapper ``_attention_pool_<branch>`` - what forward calls
+    (after fuse_bn() attn.norm_<branch> is an Identity while the wrapper still holds the BatchNorm3d)."""
+    ap = getattr(attn, "_attention_pool_" + branch)
+    pool = ap.pool if ap.has_pool else None
+    norm = ap.norm if ap.has_norm else None
+    return pool, norm, bool(ap.has_norm and ap.norm_before_pool)
+
+
+def _lower_mvit_attention(low, attn, xn, thw, name, residual=None, fold=None):
+    """MultiScaleAttention.forward (layers/attention.py:501-544) on normalised tokens ``xn`` (or on x with the block's
+    BatchNorm1d ``fold`` = (s, t) folded into the q/k/v projections): returns (proj(attention) [+ residual fused into
+    the GEMM epilogue], pooled q thw)."""
     p = low.p
-    if attn.pool_first:
-        raise NotImplementedError("pool_first=True is not used by any hub MViT and has no B200 lowering")
+    if getattr(attn, "pool_first", False):
+        return _lower_mvit_attention_pool_first(low, attn, xn, thw, name, residual)
     has_cls = attn.has_cls_embed
     heads, dim_att = attn.num_heads, attn.dim_out
     thw = _check_thw(xn, thw, has_cls, name)
@@ -870,71 +891,130 @@ def _lower_mvit_attention(low, attn, xn, thw, name, residual=None):
         b = None if attn.q.bias is None else torch.cat([attn.q.bias, attn.k.bias, attn.v.bias], 0)
     else:
         w, b = attn.qkv.weight, attn.qkv.bias
+    w, b = _folded(w, b, fold)
     qkv = PL.emit_linear(p, xn, w, b, L.ACT_NONE, None, name + ".qkv")
     q, k, v = (PL.channel_slice(qkv, i * dim_att, dim_att) for i in range(3))
     thw_q = thw
-    if getattr(attn, "pool_q", None) is not None:
-        q, thw_q = PL.emit_token_pool(p, q, thw, attn.pool_q, getattr(attn, "norm_q", None), heads, has_cls, name + ".pool_q")
-    pool_k, pool_v = getattr(attn, "pool_k", None), getattr(attn, "pool_v", None)
-    norm_k, norm_v = getattr(attn, "norm_k", None), getattr(attn, "norm_v", None)
-    if pool_k is not None and pool_v is not None and PL.pools_fusable(pool_k, pool_v, norm_k, norm_v):
-        # k | v are adjacent channel slices of the QKV GEMM output: ONE depthwise launch + ONE LayerNorm launch for both
+    pool_q, norm_q, before_q = _attention_pool(attn, "q")
+    if pool_q is not None:
+        q, thw_q = PL.emit_token_pool(p, q, thw, pool_q, norm_q, heads, has_cls, name + ".pool_q", before_q)
+    pool_k, norm_k, before_k = _attention_pool(attn, "k")
+    pool_v, norm_v, before_v = _attention_pool(attn, "v")
+    if pool_k is not None and pool_v is not None and PL.pools_fusable(pool_k, pool_v, norm_k, norm_v, before_k, before_v):
+        # k | v are adjacent channel slices of the QKV GEMM output: ONE depthwise launch (+ ONE LayerNorm launch) for both
         kv, _ = PL.emit_token_pool(p, PL.channel_slice(qkv, dim_att, 2 * dim_att), thw, (pool_k, pool_v), (norm_k, norm_v),
-                                   heads, has_cls, name + ".pool_kv")
+                                   heads, has_cls, name + ".pool_kv", before_k)
         k, v = PL.channel_slice(kv, 0, dim_att), PL.channel_slice(kv, dim_att, dim_att)
     else:
         if pool_k is not None:
-            k, _ = PL.emit_token_pool(p, k, thw, pool_k, norm_k, heads, has_cls, name + ".pool_k")
+            k, _ = PL.emit_token_pool(p, k, thw, pool_k, norm_k, heads, has_cls, name + ".pool_k", before_k)
         if pool_v is not None:
-            v, _ = PL.emit_token_pool(p, v, thw, pool_v, norm_v, heads, has_cls, name + ".pool_v")
+            v, _ = PL.emit_token_pool(p, v, thw, pool_v, norm_v, heads, has_cls, name + ".pool_v", before_v)
     o = PL.emit_attention(p, q, k, v, heads, attn.scale, attn.residual_pool, name + ".core")
     x = PL.emit_linear(p, o, attn.proj.weight, attn.proj.bias, L.ACT_NONE, residual, name + ".proj")
     return x, thw_q
 
 
-def _lower_mlp(low, mlp, xn, name, residual=None):
+def _lower_mvit_attention_pool_first(low, attn, xn, thw, name, residual=None):
+    """pool_first=True (layers/attention.py:511-517): every branch pools the normalised tokens per head (dim // heads
+    channels), then its q / k / v linear runs on the pooled tokens; residual_pool adds the projected pooled q."""
+    p = low.p
+    has_cls = attn.has_cls_embed
+    heads = attn.num_heads
+    thw = _check_thw(xn, thw, has_cls, name)
+    if xn.C % heads:
+        raise RuntimeError("%s: %d channels do not split into %d heads" % (name, xn.C, heads))
+    outs, thw_q = {}, thw
+    for br in ("q", "k", "v"):
+        pool, norm, before = _attention_pool(attn, br)
+        src = xn
+        if pool is not None:
+            src, pthw = PL.emit_token_pool(p, xn, thw, pool, norm, heads, has_cls, name + ".pool_" + br, before)
+            if br == "q":
+                thw_q = pthw
+        lin = getattr(attn, br)
+        outs[br] = PL.emit_linear(p, src, lin.weight, lin.bias, L.ACT_NONE, None, name + "." + br)
+    o = PL.emit_attention(p, outs["q"], outs["k"], outs["v"], heads, attn.scale, attn.residual_pool, name + ".core")
+    x = PL.emit_linear(p, o, attn.proj.weight, attn.proj.bias, L.ACT_NONE, residual, name + ".proj")
+    return x, thw_q
+
+
+def _lower_mlp(low, mlp, xn, name, residual=None, fold=None):
     # layers/attention.py:102-114: fc1 -> act -> fc2 (dropout = identity in eval)
     act = _act_code(mlp.act)
     if act == L.ACT_GELU and getattr(mlp.act, "approximate", "none") != "none":
         raise NotImplementedError("Mlp activation must be the exact (erf) GELU")
-    h = PL.emit_linear(low.p, xn, mlp.fc1.weight, mlp.fc1.bias, act, None, name + ".fc1")
+    w1, b1 = _folded(mlp.fc1.weight, mlp.fc1.bias, fold)
+    h = PL.emit_linear(low.p, xn, w1, b1, act, None, name + ".fc1")
     return PL.emit_linear(low.p, h, mlp.fc2.weight, mlp.fc2.bias, L.ACT_NONE, residual, name + ".fc2")
+
+
+def _norm_kind(m):
+    return type(m).__name__
+
+
+def _block_norms_are_layernorm(blk):
+    return _norm_kind(blk.norm1) == "LayerNorm" and _norm_kind(blk.norm2) == "LayerNorm"
+
+
+def _lower_block_norm(p, x, norm, name, pool_first=False):
+    """(x_norm, fold) for a block norm as forward calls it (layers/attention.py:738-742, 748-752): a LayerNorm launch;
+    an eval BatchNorm1d folded into the linears that consume x_norm (fold = (s, t), x_norm = x), or - when the attention
+    pools x_norm first (zero padding and max / avg do not commute with the affine) - materialised by one launch over
+    every row, cls included; an Identity (after fuse_bn()) is x itself."""
+    kind = _norm_kind(norm)
+    if kind == "LayerNorm":
+        return PL.emit_layernorm(p, x, norm, name), None
+    if kind == "BatchNorm1d":
+        s, t = PL.bn_affine(norm)
+        if s.numel() != x.C:
+            raise RuntimeError("%s: BatchNorm1d has %d channels, the tokens %d" % (name, s.numel(), x.C))
+        if pool_first:
+            return PL.emit_channel_affine(p, x, s, t, name), None
+        return x, (s, t)
+    if kind == "Identity":
+        return x, None
+    raise NotImplementedError("%s: block norm %s unsupported" % (name, kind))
 
 
 def _lower_mvit_block(low, blk, x, thw, name, xn=None, next_ln=None, want_sum=True):
     """MultiScaleBlock.forward (layers/attention.py:729-757); DropPath is the identity in eval.
-    Returns (x, thw', xn_next).  f16 engine with ``plan.trunk32``: the residual stream x is fp32 - the branch outputs
-    (attention proj, fc2) stay f16 and each residual add is fused with the LayerNorm that follows it (norm2; ``next_ln`` =
-    the next block's norm1 / the model's norm_embed, whose f16 output comes back as xn_next; ``xn`` = this block's
-    already normalised input handed over by the previous block)."""
+    Returns (x, thw', xn_next).  f16 engine with ``plan.trunk32`` (LayerNorm blocks only): the residual stream x is
+    fp32 - the branch outputs (attention proj, fc2) stay f16 and each residual add is fused with the LayerNorm that
+    follows it (norm2; ``next_ln`` = the next block's norm1 / the model's norm_embed, whose f16 output comes back as
+    xn_next; ``xn`` = this block's already normalised input handed over by the previous block).  BatchNorm1d / Identity
+    block norms dispatch on the modules themselves (see _lower_block_norm)."""
     p = low.p
     attn = blk.attn
-    if getattr(blk, "norm1_is_batchnorm_1d", False) or getattr(blk, "norm2_is_batchnorm_1d", False):
-        raise NotImplementedError("batchnorm MViT variant unsupported")
     has_cls = attn.has_cls_embed
     thw = _check_thw(x, thw, has_cls, name)
     trunk32 = p.trunk32
+    assert not trunk32 or _block_norms_are_layernorm(blk)
+    fold1 = None
     if xn is None:
-        xn = PL.emit_layernorm(p, x, blk.norm1, name + ".norm1")
+        xn, fold1 = _lower_block_norm(p, x, blk.norm1, name + ".norm1", pool_first=getattr(attn, "pool_first", False))
     widen = blk.dim != blk.dim_out
     if blk.dim_mul_in_att and widen:
-        x = PL.emit_linear(p, xn, blk.proj.weight, blk.proj.bias, L.ACT_NONE, None, name + ".proj")
+        w, b = _folded(blk.proj.weight, blk.proj.bias, fold1)
+        x = PL.emit_linear(p, xn, w, b, L.ACT_NONE, None, name + ".proj")
     x_res = x
     if getattr(blk, "pool_skip", None) is not None:
         x_res, _ = PL.emit_token_pool(p, x, thw, blk.pool_skip, None, 1, has_cls, name + ".pool_skip")
     if trunk32:
         br, thw_q = _lower_mvit_attention(low, attn, xn, thw, name + ".attn", residual=None)
         x, xn2 = PL.emit_add_layernorm(p, x_res, br, blk.norm2, name + ".norm2")
+        fold2 = None
     else:
-        x, thw_q = _lower_mvit_attention(low, attn, xn, thw, name + ".attn", residual=x_res)
-        xn2 = PL.emit_layernorm(p, x, blk.norm2, name + ".norm2")
+        x, thw_q = _lower_mvit_attention(low, attn, xn, thw, name + ".attn", residual=x_res, fold=fold1)
+        xn2, fold2 = _lower_block_norm(p, x, blk.norm2, name + ".norm2")
     if (not blk.dim_mul_in_att) and widen:
-        x = PL.emit_linear(p, xn2, blk.proj.weight, blk.proj.bias, L.ACT_NONE, None, name + ".proj")
+        w, b = _folded(blk.proj.weight, blk.proj.bias, fold2)
+        x = PL.emit_linear(p, xn2, w, b, L.ACT_NONE, None, name + ".proj")
     if trunk32:
         br2 = _lower_mlp(low, blk.mlp, xn2, name + ".mlp", residual=None)
         x, xn_next = PL.emit_add_layernorm(p, x, br2, next_ln, name + ".add", want_sum=want_sum or next_ln is None)
         return x, thw_q, xn_next
-    x = _lower_mlp(low, blk.mlp, xn2, name + ".mlp", residual=x)
+    x = _lower_mlp(low, blk.mlp, xn2, name + ".mlp", residual=x, fold=fold2)
     return x, thw_q, None
 
 
@@ -983,10 +1063,25 @@ def _lower_vit_head(low, head, x, name="head"):
 def _lower_mvit(self, m, x, name):
     p = self.p
     pe = m.patch_embed
-    if type(pe).__name__ != "PatchEmbed":
-        raise NotImplementedError("MViT without a conv patch embedding is unsupported")
-    pm = pe.patch_model
-    if isinstance(pm, nn.Conv2d):
+    enc = m.cls_positional_encoding
+    T, H, W = enc.patch_embed_shape()
+    pos, has_cls = _pos_table(enc)
+    if type(pe).__name__ == "Identity":
+        # enable_patch_embed=False: the input already is the (B, T*H*W, C) patch-token tensor, C the width of the
+        # positional table (cls_token is a 0-d placeholder when cls_embed_on=False)
+        if x.T != 1 or x.H != 1:
+            raise RuntimeError("an MViT without a patch embedding takes (B, T*H*W, C) tokens")
+        if x.npos != T * H * W or x.C != pos.shape[1]:
+            raise RuntimeError("expected (B, %d, %d) tokens for the %s patch grid, got (B, %d, %d)" % (
+                T * H * W, pos.shape[1], (T, H, W), x.npos, x.C))
+        pm = None
+    elif type(pe).__name__ != "PatchEmbed":
+        raise NotImplementedError("MViT patch embedding %s unsupported" % type(pe).__name__)
+    else:
+        pm = pe.patch_model
+    if pm is None:
+        pass
+    elif isinstance(pm, nn.Conv2d):
         # image MViT (vision_transformers.py use_2d_patch=True): the Conv2d runs as a (1, kh, kw) Conv3d on the
         # one-frame clip, so a 7x7 / stride 4 embed takes the window-mode tensor-core stem like the video models'
         if not getattr(x, "image", False):
@@ -997,15 +1092,14 @@ def _lower_mvit(self, m, x, name):
                              (1,) + tuple(pm.dilation), pm.groups, L.ACT_NONE, None, "patch_embed.patch_model")
     else:
         x = self.conv(x, pm, None, None, None, "patch_embed.patch_model")
-    enc = m.cls_positional_encoding
-    T, H, W = enc.patch_embed_shape()
-    if (x.T, x.H, x.W) != (T, H, W):
+    if pm is not None and (x.T, x.H, x.W) != (T, H, W):
         raise RuntimeError("input clip gives a %s patch grid but the model was built for %s" % ((x.T, x.H, x.W), (T, H, W)))
-    pos, has_cls = _pos_table(enc)
     ne = m.norm_embed
     ne_is_ln = type(ne).__name__ == "LayerNorm"
-    if p.trunk32 and not ne_is_ln:
-        p.trunk32 = False            # the head's GEMM needs f16 tokens: without a final LayerNorm keep the f16 stream
+    if p.trunk32 and not (ne_is_ln and all(_block_norms_are_layernorm(b) for b in m.blocks)):
+        # the head's GEMM needs f16 tokens: without a final LayerNorm keep the f16 stream; the fp32 trunk also fuses
+        # every residual add with a LayerNorm, so BatchNorm / Identity block norms keep it too
+        p.trunk32 = False
     x = PL.emit_pos_cls(p, x, pos, has_cls, "cls_positional_encoding", out_dt=L.PV_F32 if p.trunk32 else None)
     thw = (T, H, W)
     xn = None
@@ -1016,7 +1110,14 @@ def _lower_mvit(self, m, x, name):
         x, thw, xn = _lower_mvit_block(self, blk, x, thw, "blocks.%d" % i, xn=xn, next_ln=nxt, want_sum=not last)
     head = m.head
     if type(head).__name__ == "Identity":
-        raise NotImplementedError("headless MViT output is unsupported")
+        # head=None: the (B, N, C) tokens after norm_embed
+        if p.trunk32:
+            x = xn             # norm_embed was fused into the last block's residual add
+        elif ne_is_ln:
+            x = PL.emit_layernorm(p, x, ne, "norm_embed")
+        elif type(ne).__name__ != "Identity":
+            raise NotImplementedError("MViT norm_embed %s unsupported" % type(ne).__name__)
+        return _tok_out(x)
     if type(head).__name__ != "VisionTransformerBasicHead":
         raise NotImplementedError("MViT head %s unsupported" % type(head).__name__)
     mode = head.sequence_pool.mode if head.sequence_pool is not None else None
@@ -1040,6 +1141,8 @@ def _tok_out(x, squeeze=False):
 def _lower_block_module(self, m, x, name):
     if len(self.extra) != 1:
         raise RuntimeError("MultiScaleBlock.forward(x, thw_shape): thw_shape is required")
+    if not _block_norms_are_layernorm(m):
+        self.p.trunk32 = False      # the fp32 trunk fuses the residual adds with LayerNorms (see _lower_mvit)
     y, thw, _ = _lower_mvit_block(self, m, x, self.extra[0], name or "block")
     self.aux_out = list(thw)
     return _tok_out(y)

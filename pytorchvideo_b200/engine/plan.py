@@ -884,32 +884,65 @@ def _pool_geometry(pool):
     if kind == "Conv3d":
         k, s, p, dl = [tuple(int(v) for v in t) for t in (pool.kernel_size, pool.stride, pool.padding, pool.dilation)]
         return kind, k, s, p, dl, int(pool.in_channels)
-    if kind == "MaxPool3d":
+    if kind in ("MaxPool3d", "AvgPool3d"):
+        if kind == "AvgPool3d" and (pool.ceil_mode or not pool.count_include_pad or pool.divisor_override is not None):
+            raise NotImplementedError("AvgPool3d pools take count_include_pad=True, ceil_mode=False and no divisor_override")
         k, s, p = [tuple(int(v) for v in (t if isinstance(t, (tuple, list)) else (t,) * 3))
                    for t in (pool.kernel_size, pool.stride, pool.padding)]
         return kind, k, s, p, (1, 1, 1), 0
     raise NotImplementedError("pool module %s unsupported" % kind)
 
 
-def pools_fusable(pool_a, pool_b, norm_a, norm_b):
-    """True when two _AttentionPool branches (pool_k / pool_v) can run as ONE depthwise launch + ONE LayerNorm launch over
-    adjacent channel slices: same conv geometry, LayerNorms of the same width / eps."""
+def bn_affine(bn):
+    """Eval-mode BatchNorm as a per-channel affine (scale, shift), fp32 CPU tensors."""
+    if bn.running_mean is None or bn.running_var is None:
+        raise NotImplementedError("BatchNorm without running statistics is unsupported")
+    with torch.no_grad():
+        inv = 1.0 / torch.sqrt(bn.running_var.detach().double().cpu() + float(bn.eps))
+        w = bn.weight.detach().double().cpu() if bn.weight is not None else torch.ones_like(inv)
+        b = bn.bias.detach().double().cpu() if bn.bias is not None else torch.zeros_like(inv)
+        s = w * inv
+        return s.float(), (b - bn.running_mean.detach().double().cpu() * s).float()
+
+
+def _prologue_vectors(norm, width):
+    """_AttentionPool with norm_before_pool (layers/attention.py:191-195): GELU(norm(x)) before the pool.  BatchNorm3d
+    (eval) gives its affine, Identity the unit one; (scale, shift) of ``width`` channels."""
+    kind = type(norm).__name__
+    if kind == "BatchNorm3d":
+        s, b = bn_affine(norm)
+        if s.numel() != width:
+            raise RuntimeError("attention-pool BatchNorm3d has %d channels, the pool %d" % (s.numel(), width))
+        return s, b
+    if kind == "Identity":
+        return torch.ones(width), torch.zeros(width)
+    raise NotImplementedError("pre-pool norm %s unsupported" % kind)
+
+
+def pools_fusable(pool_a, pool_b, norm_a, norm_b, before_a=False, before_b=False):
+    """True when two _AttentionPool branches (pool_k / pool_v) can run as ONE depthwise launch over adjacent channel
+    slices: same conv geometry, and either LayerNorms of the same width / eps after the pool (then ONE LayerNorm launch
+    for both) or a pre-pool norm + GELU on both (the prologue vectors are concatenated over the two slices)."""
     if type(pool_a).__name__ != "Conv3d" or type(pool_b).__name__ != "Conv3d":
         return False
     if _pool_geometry(pool_a) != _pool_geometry(pool_b):
         return False
+    if before_a or before_b:
+        return before_a and before_b
     na, nb = type(norm_a).__name__, type(norm_b).__name__
     if na != "LayerNorm" or nb != "LayerNorm":
         return False
     return tuple(norm_a.normalized_shape) == tuple(norm_b.normalized_shape) and float(norm_a.eps) == float(norm_b.eps)
 
 
-def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool"):
+def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool", norm_before_pool=False):
     """_AttentionPool (layers/attention.py:162-212) on a token tensor/slice x [B, cls+THW, dim]:
-    depthwise Conv3d / MaxPool3d over the (T,H,W) grid of the patch tokens (cls row passes through),
+    depthwise Conv3d / MaxPool3d / AvgPool3d over the (T,H,W) grid of the patch tokens (cls row passes through),
     then the per-head LayerNorm over head_dim (cls row included; it is read straight from x by the LayerNorm
-    launch).  ``pool`` / ``norm`` may be tuples (pool_k, pool_v) / (norm_k, norm_v): x then holds the branches as
-    adjacent channel slices and both run in one depthwise + one LayerNorm launch (see pools_fusable).
+    launch).  With ``norm_before_pool`` (BatchNorm3d or Identity norms) the norm and a GELU run instead as the
+    prologue of the depthwise conv, on every in-bounds input before the zero padding, and the cls row is copied raw.
+    ``pool`` / ``norm`` may be tuples (pool_k, pool_v) / (norm_k, norm_v): x then holds the branches as
+    adjacent channel slices and both run in one depthwise (+ one LayerNorm) launch (see pools_fusable).
     Returns (tokens, thw')."""
     import ctypes as C_
     pools = list(pool) if isinstance(pool, (tuple, list)) else [pool]
@@ -930,6 +963,8 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool"):
                 raise NotImplementedError("%s: only depthwise, bias-free pooling convs are supported" % name)
         if dim % pool_ch:
             raise RuntimeError("%s: pool channels do not divide the token width" % name)
+    elif norm_before_pool:
+        raise NotImplementedError("%s: a pre-pool norm needs a pooling conv" % name)
     To = (T + 2 * p[0] - dl[0] * (k[0] - 1) - 1) // s[0] + 1
     Ho = (H + 2 * p[1] - dl[1] * (k[1] - 1) - 1) // s[1] + 1
     Wo = (W + 2 * p[2] - dl[2] * (k[2] - 1) - 1) // s[2] + 1
@@ -953,6 +988,12 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool"):
         d.groups, d.act, d.has_residual = dim_all, L.ACT_NONE, 0
         d.x_row_stride, d.y_row_stride = x.row_stride, y.row_stride
         d.x_batch_stride, d.y_batch_stride = x.npos * x.row_stride, y.npos * y.row_stride
+        if norm_before_pool:
+            vec = [_prologue_vectors(n, pool_ch) for n in norms]
+            pre_s = plan.const(torch.cat([s_.repeat(reps) for s_, _ in vec]).contiguous())
+            pre_b = plan.const(torch.cat([b_.repeat(reps) for _, b_ in vec]).contiguous())
+            d.pre_scale, d.pre_bias, d.pre_act = pre_s.data_ptr(), pre_b.data_ptr(), L.ACT_GELU
+            plan.stats["pool_prologue"] = plan.stats.get("pool_prologue", 0) + 1
         # a one-frame token grid (image MViT) pooled by a (1,kh,kw) conv: the plane kernel (csrc/pv_dwplane.cu) when it
         # takes the shape; every other pool keeps pv_dwconv3d_fwd
         plane = k[0] == 1 and T == 1 and bool(lib.pv_dwplane_supported(C_.byref(d)))
@@ -975,7 +1016,7 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool"):
                  (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz)
     else:
         d = L.Pool3dDesc()
-        d.dtype, d.mode = x.dt, L.POOL_MAX
+        d.dtype, d.mode = x.dt, L.POOL_MAX if kind == "MaxPool3d" else L.POOL_AVG
         d.N, d.Ti, d.Hi, d.Wi, d.C = x.N, T, H, W, dim_all
         d.To, d.Ho, d.Wo = To, Ho, Wo
         d.kt, d.kh, d.kw = k
@@ -987,8 +1028,9 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool"):
             d.x_batch_stride, d.y_batch_stride = x.npos * x.row_stride, y.npos * y.row_stride
             L.check(lib.pv_pool3d_fwd(C_.byref(d), x.ptr() + cls * x.row_stride * esz,
                                       y.ptr() + cls * y.row_stride * esz, stream), "pv_pool3d_fwd(%s)" % name)
-        plan.add(name + ".maxpool", fn, "other", 0.0, (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz)
-    have_norm = [n is not None and type(n).__name__ != "Identity" for n in norms]
+        plan.add(name + (".maxpool" if kind == "MaxPool3d" else ".avgpool"), fn, "other", 0.0,
+                 (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz)
+    have_norm = [n is not None and type(n).__name__ != "Identity" and not norm_before_pool for n in norms]
     if any(have_norm) and not all(have_norm):
         raise NotImplementedError("%s: fused pooling branches need a norm on every branch" % name)
     if not all(have_norm):
@@ -1040,6 +1082,32 @@ def emit_attention(plan, q, k, v, heads, scale, residual_pool, name="attn", norm
     plan.attention_calls.append({"name": name, "B": B, "H": heads, "Nq": Nq, "Nk": Nk, "D": dim // heads,
                                  "scale": d.scale, "normalize": d.normalize, "add_q_residual": d.add_q_residual})
     return o
+
+
+def emit_channel_affine(plan, x, scale, shift, name="affine"):
+    """y = scale[c] * x + shift[c] on every token row (eval BatchNorm1d over the channels of [B, N, C]), as a 1x1x1
+    unit-weight depthwise convolution over a [B, 1, 1, N] grid with the affine as its folded scale / bias."""
+    import ctypes as C_
+    C = x.C
+    y = _tok(plan, x.N, x.npos, C, dt=x.dt)
+    w_d = plan.const(PK.pack_depthwise(torch.ones(C, 1, 1, 1, 1), C, _TORCH_DT[x.dt]))
+    sc = plan.const(scale.float().contiguous())
+    sh = plan.const(shift.float().contiguous())
+    d = L.Conv3dDesc()
+    d.dtype = x.dt
+    d.N, d.Ti, d.Hi, d.Wi, d.Ci = x.N, 1, 1, x.npos, C
+    d.To, d.Ho, d.Wo, d.Co = 1, 1, x.npos, C
+    d.kt = d.kh = d.kw = d.st = d.sh = d.sw = d.dt = d.dh = d.dw = 1
+    d.groups, d.act, d.has_residual = C, L.ACT_NONE, 0
+    lib = plan.lib
+
+    def fn(stream):
+        d.x_row_stride, d.y_row_stride = x.row_stride, y.row_stride
+        d.x_batch_stride, d.y_batch_stride = x.npos * x.row_stride, y.npos * y.row_stride
+        L.check(lib.pv_dwconv3d_fwd(C_.byref(d), x.ptr(), w_d.data_ptr(), sc.data_ptr(), sh.data_ptr(), y.ptr(), None,
+                                    stream), "pv_dwconv3d_fwd(%s)" % name)
+    plan.add(name, fn, "depthwise", 2.0 * x.N * x.npos * C, 2 * x.N * x.npos * C * _ESIZE[x.dt], reads=(x,), writes=(y,))
+    return y
 
 
 def channel_slice(x, off, C):

@@ -662,3 +662,75 @@ def map_x3d_to_efficient(x3d, eff):
     conv_bn(eff.head.lin_5, head.pool.post_conv, head.pool.post_norm)
     eff.projection.model.load_state_dict(head.proj.state_dict())
     return eff
+
+
+# ---- MViT builder variants (tests/golden/mvit_variants.pt, oracle/gen_golden_mvit_variants.py) ----------------------
+_MVIT_SMALL = dict(spatial_size=64, temporal_size=4, depth=4, embed_dim_mul=[[1, 2.0], [3, 2.0]],
+                   atten_head_mul=[[1, 2.0], [3, 2.0]], pool_q_stride_size=[[1, 1, 2, 2], [3, 1, 2, 2]],
+                   pool_kv_stride_adaptive=[1, 4, 4], pool_kvq_kernel=[3, 3, 3])
+_MVIT_B_BN = dict(spatial_size=224, temporal_size=8, norm="batchnorm", embed_dim_mul=[[1, 2.0], [3, 2.0], [14, 2.0]],
+                  atten_head_mul=[[1, 2.0], [3, 2.0], [14, 2.0]], pool_q_stride_size=[[1, 1, 2, 2], [3, 1, 2, 2], [14, 1, 2, 2]],
+                  pool_kv_stride_adaptive=[1, 8, 8], pool_kvq_kernel=[3, 3, 3], cls_embed_on=False)
+# name: (what, builder kwargs, input shape, call fuse_bn() after randomising).  what: "model" (a clip or, without a
+# patch embedding, a (B, T*H*W, C) token tensor) or "block" (a stand-alone MultiScaleBlock on tokens, thw_shape given).
+# The BatchNorm MViT-B cases keep the builder's own initialisation (seed 42) and randomise only the BatchNorms, as the
+# reference's tests/test_fuse_bn.py does: with randomize_model's linear weights the residual stream of 16 BatchNorm
+# blocks (no LayerNorm anywhere) grows to |logit| ~ 3e4 (2.7e5 after fuse_bn()), beyond the f16 range.
+MVIT_VARIANT_INIT_CASES = ("bn_mvit_b", "bn_mvit_b_fused")
+MVIT_VARIANT_CASES = {
+    "bn_mvit_b": ("model", _MVIT_B_BN, (2, 3, 8, 224, 224), False),
+    "bn_mvit_b_fused": ("model", _MVIT_B_BN, (2, 3, 8, 224, 224), True),
+    "bn_small": ("model", dict(_MVIT_SMALL, norm="batchnorm", separate_qkv=False, residual_pool=True, dim_mul_in_att=True),
+                 (2, 3, 4, 64, 64), False),
+    "pool_first_ln": ("model", dict(_MVIT_SMALL, pool_first=True), (2, 3, 4, 64, 64), False),
+    "pool_first_bn": ("model", dict(_MVIT_SMALL, pool_first=True, norm="batchnorm"), (2, 3, 4, 64, 64), False),
+    "pool_first_bn_avg": ("model", dict(_MVIT_SMALL, pool_first=True, norm="batchnorm", pooling_mode="avg",
+                                        pool_kvq_kernel=None), (2, 3, 4, 64, 64), False),
+    "avg": ("model", dict(_MVIT_SMALL, pooling_mode="avg", pool_kvq_kernel=None), (2, 3, 4, 64, 64), False),
+    "tokens": ("model", dict(spatial_size=28, temporal_size=4, depth=2, patch_embed_dim=96, enable_patch_embed=False,
+                             pool_q_stride_size=[[1, 1, 2, 2]], pool_kv_stride_adaptive=[1, 4, 4],
+                             pool_kvq_kernel=[3, 3, 3]), (2, 4 * 28 * 28, 96), False),
+    "tokens_no_cls": ("model", dict(spatial_size=28, temporal_size=4, depth=2, patch_embed_dim=96,
+                                    enable_patch_embed=False, cls_embed_on=False, pool_q_stride_size=[[1, 1, 2, 2]],
+                                    pool_kv_stride_adaptive=[1, 4, 4], pool_kvq_kernel=[3, 3, 3]),
+                      (2, 4 * 28 * 28, 96), False),
+    "head_none": ("model", dict(_MVIT_SMALL, head=None), (2, 3, 4, 64, 64), False),
+    "bn_block": ("block", dict(dim=96, dim_out=192, num_heads=2, qkv_bias=True, dim_mul_in_att=True, kernel_q=(3, 3, 3),
+                               kernel_kv=(3, 3, 3), stride_q=(1, 2, 2), stride_kv=(1, 4, 4)), (2, 1 + 4 * 8 * 8, 96),
+                 False),
+}
+MVIT_VARIANT_BLOCK_THW = (4, 8, 8)
+
+
+def build_mvit_variant_case(case, create_mvit, block_cls, weight_seed=1234, input_seed=42, fuse=None):
+    """(model, input, extra forward args) of a MVIT_VARIANT_CASES entry built with ``create_mvit`` /
+    ``block_cls`` (this package's or the reference's).  Every weight is drawn by randomize_model, BatchNorms included
+    (the ranges of the reference's tests/test_fuse_bn.py), except in MVIT_VARIANT_INIT_CASES (builder initialisation,
+    random BatchNorms); fuse_bn() runs after that where the case asks for it (or as ``fuse`` overrides)."""
+    what, kw, shape, case_fuse = MVIT_VARIANT_CASES[case]
+    fuse = case_fuse if fuse is None else fuse
+    torch.manual_seed(42 if case in MVIT_VARIANT_INIT_CASES else 0)
+    if what == "block":
+        model = block_cls(norm_layer=nn.BatchNorm1d, attn_norm_layer=nn.BatchNorm3d, **kw)
+        extra = (list(MVIT_VARIANT_BLOCK_THW),)
+    else:
+        model = create_mvit(**kw)
+        extra = ()
+    if case in MVIT_VARIANT_INIT_CASES:
+        g = torch.Generator(device="cpu")
+        g.manual_seed(weight_seed)
+        with torch.no_grad():
+            for m in model.modules():
+                if isinstance(m, nn.modules.batchnorm._BatchNorm):
+                    for t, lo, hi in ((m.weight, 0.5, 1.5), (m.bias, -0.5, 0.5), (m.running_var, 0.5, 1.5),
+                                      (m.running_mean, -0.5, 0.5)):
+                        t.copy_(torch.rand(t.shape, generator=g) * (hi - lo) + lo)
+        model.eval()
+    else:
+        model = randomize_model(model, seed=weight_seed).eval()
+    if fuse:
+        model.fuse_bn()
+    g = torch.Generator(device="cpu")
+    g.manual_seed(input_seed)
+    x = torch.rand(shape, generator=g) if len(shape) == 5 else torch.randn(shape, generator=g)
+    return model, x, extra
