@@ -141,6 +141,43 @@ int pv_clip_transform_batch(const pv_clip_batch_desc* d, const void* src, const 
 int pv_clip_transform_rrc(const pv_clip_batch_desc* d, const void* src, const int32_t* idx_t, const int32_t* boxes,
                           void* dst, void* stream);
 
+/* Detection boxes of the batched chain (transforms/functional.py:195-445: short_side_scale_with_boxes,
+ * random_crop_with_boxes, uniform_crop_with_boxes, horizontal_flip_with_boxes, clip_boxes_to_image, crop_boxes).
+ * Clip b owns boxes box_start[b] .. box_start[b+1]-1 of the (n_boxes, 4) array of (x1, y1, x2, y2); box_start is a
+ * DEVICE int32 array of n_clips + 1 non-decreasing offsets with box_start[n_clips] == n_boxes.  geom is the per-clip
+ * {new_h, new_w, top, left, hflip, first_frame} array pv_clip_transform_batch reads (or NULL: the descriptor's
+ * values for every clip), so a clip and its boxes share one crop and one flip.  The set bits of steps run in order:
+ *   PV_BOX_CLIP_SRC   x = min(in_w - 1, max(0, x)), likewise y with in_h   (clip_boxes_to_image, source frame)
+ *   PV_BOX_SCALE      x *= T(double(new_h) / in_h) if in_w < in_h, else T(double(new_w) / in_w)
+ *   PV_BOX_CROP       x -= left, y -= top
+ *   PV_BOX_CLIP_CROP  clip to out_h x out_w                                  (the crops' clip_boxes_to_image)
+ *   PV_BOX_FLIP       when the clip's hflip is set: x1' = (out_w - x2) - 1, x2' = (out_w - x1) - 1
+ *   PV_BOX_CLIP_OUT   clip to out_h x out_w                                  (clip_boxes_to_image, output frame)
+ * Each operation rounds once to the boxes' type T (float32 or float64), as the reference's eager ops do.  The boxes
+ * are written to boxes_out in T (boxes_out == boxes_in is allowed); rois_out, when not NULL, also receives the fp32
+ * (n_boxes, 5) rows (b, x1, y1, x2, y2) that pv_roi_align_fwd reads.  One launch; n_boxes == 0 launches nothing.  */
+#define PV_BOX_F32 1
+#define PV_BOX_F64 3
+#define PV_BOX_CLIP_SRC 1
+#define PV_BOX_SCALE 2
+#define PV_BOX_CROP 4
+#define PV_BOX_CLIP_CROP 8
+#define PV_BOX_FLIP 16
+#define PV_BOX_CLIP_OUT 32
+#define PV_BOX_ALL_STEPS 63
+
+typedef struct pv_boxes_desc {
+  int n_clips, n_boxes;             /* B clips, K boxes in all                                    */
+  int steps;                        /* PV_BOX_* step mask                                         */
+  int dtype;                        /* PV_BOX_F32 | PV_BOX_F64                                    */
+  int in_h, in_w;                   /* source frame                                               */
+  int new_h, new_w, top, left, hflip;  /* every clip's geometry when geom is NULL                  */
+  int out_h, out_w;                 /* crop / output frame                                        */
+} pv_boxes_desc;
+
+int pv_clip_boxes_transform(const pv_boxes_desc* d, const void* boxes_in, const int32_t* box_start,
+                            const int32_t* geom, void* boxes_out, float* rois_out, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Video augmentation (transforms/augmentations.py, rand_augment.py, augmix.py): a batch of clips of (T, 3, H, W)
  * frames, each clip with its own op per layer step.

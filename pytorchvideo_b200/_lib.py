@@ -38,6 +38,16 @@ class ClipBatchDesc(C.Structure):
                 ("div255", C.c_int), ("normalize", C.c_int), ("src_dtype", C.c_int), ("dst_dtype", C.c_int)]
 
 
+BOX_F32, BOX_F64 = 1, 3                             # pv_boxes_desc.dtype
+BOX_CLIP_SRC, BOX_SCALE, BOX_CROP, BOX_CLIP_CROP, BOX_FLIP, BOX_CLIP_OUT = 1, 2, 4, 8, 16, 32   # pv_boxes_desc.steps
+
+
+class BoxesDesc(C.Structure):
+    _fields_ = [("n_clips", C.c_int), ("n_boxes", C.c_int), ("steps", C.c_int), ("dtype", C.c_int),
+                ("in_h", C.c_int), ("in_w", C.c_int), ("new_h", C.c_int), ("new_w", C.c_int),
+                ("top", C.c_int), ("left", C.c_int), ("hflip", C.c_int), ("out_h", C.c_int), ("out_w", C.c_int)]
+
+
 class AugOp(C.Structure):
     _fields_ = [("kind", C.c_int), ("ival", C.c_int), ("ratio", C.c_float), ("omr", C.c_float),
                 ("theta", C.c_float * 6), ("fill", C.c_float * 3)]
@@ -118,6 +128,7 @@ SIGNATURES = {
                                         c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_clip_transform_batch": (C.c_int, [C.POINTER(ClipBatchDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_clip_transform_rrc": (C.c_int, [C.POINTER(ClipBatchDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_clip_boxes_transform": (C.c_int, [C.POINTER(BoxesDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_augment_stats": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, c_vp]),
     "pv_augment_apply": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_augment_mix": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp]),

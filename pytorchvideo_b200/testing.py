@@ -734,3 +734,120 @@ def build_mvit_variant_case(case, create_mvit, block_cls, weight_seed=1234, inpu
     g.manual_seed(input_seed)
     x = torch.rand(shape, generator=g) if len(shape) == 5 else torch.randn(shape, generator=g)
     return model, x, extra
+
+
+# ---- detection input transforms (tests/golden/boxes.pt, oracle/gen_golden_boxes.py) -------------------------------
+def synthetic_xyxy(n_boxes, H, W, seed, dtype=torch.float32):
+    """(n, 4) (x1, y1, x2, y2) boxes in source pixels, drawn in float64 and rounded once to ``dtype``: random boxes that
+    may reach past every edge, plus (n >= 4) a degenerate box, one wholly outside the frame, the whole frame and one
+    with fractional edges just past the far corner."""
+    g = torch.Generator().manual_seed(seed)
+    x1 = torch.rand(n_boxes, generator=g, dtype=torch.float64) * (1.4 * W) - 0.2 * W
+    y1 = torch.rand(n_boxes, generator=g, dtype=torch.float64) * (1.4 * H) - 0.2 * H
+    x2 = x1 + torch.rand(n_boxes, generator=g, dtype=torch.float64) * (0.6 * W)
+    y2 = y1 + torch.rand(n_boxes, generator=g, dtype=torch.float64) * (0.6 * H)
+    b = torch.stack([x1, y1, x2, y2], 1)
+    if n_boxes >= 4:
+        b[0] = torch.tensor([W * 0.37, H * 0.61, W * 0.37, H * 0.61], dtype=torch.float64)
+        b[1] = torch.tensor([-30.25, -9.5, -3.125, -0.5], dtype=torch.float64)
+        b[2] = torch.tensor([0.0, 0.0, float(W), float(H)], dtype=torch.float64)
+        b[3] = torch.tensor([W - 1.3, H - 2.7, W + 0.49, H - 0.51], dtype=torch.float64)
+    return b.to(dtype).contiguous()
+
+
+# name: (function of transforms.functional, frame (H, W), number of boxes, keyword arguments).  Every case runs on
+# float32 and float64 boxes; the torch and numpy global seeds are BOX_SEED + the case's position before the call.
+BOX_SEED = 2024
+BOX_FUNCTIONAL_CASES = {
+    "clip_landscape": ("clip_boxes_to_image", (48, 64), 9, {}),
+    "clip_portrait": ("clip_boxes_to_image", (64, 40), 9, {}),
+    "clip_empty": ("clip_boxes_to_image", (48, 64), 0, {}),
+    "crop": ("crop_boxes", (48, 64), 9, {"x_offset": 7, "y_offset": 3}),
+    "crop_negative": ("crop_boxes", (48, 64), 6, {"x_offset": -4, "y_offset": 11}),
+    "scale_landscape_up": ("short_side_scale_with_boxes", (48, 64), 9, {"size": 71}),
+    "scale_portrait_down": ("short_side_scale_with_boxes", (64, 40), 9, {"size": 27}),
+    "scale_square": ("short_side_scale_with_boxes", (48, 48), 7, {"size": 37}),
+    "scale_empty": ("short_side_scale_with_boxes", (48, 64), 0, {"size": 33}),
+    "random_scale_landscape": ("random_short_side_scale_with_boxes", (48, 64), 9, {"min_size": 30, "max_size": 90}),
+    "random_scale_portrait": ("random_short_side_scale_with_boxes", (64, 40), 9, {"min_size": 20, "max_size": 50}),
+    "random_crop_landscape": ("random_crop_with_boxes", (48, 64), 9, {"size": 32}),
+    "random_crop_portrait": ("random_crop_with_boxes", (64, 40), 9, {"size": 32}),
+    "random_crop_wide": ("random_crop_with_boxes", (32, 64), 8, {"size": 32}),
+    "random_crop_equal": ("random_crop_with_boxes", (32, 32), 8, {"size": 32}),
+    "random_crop_empty": ("random_crop_with_boxes", (48, 64), 0, {"size": 32}),
+    "uniform_crop_landscape_0": ("uniform_crop_with_boxes", (48, 64), 9, {"size": 40, "spatial_idx": 0}),
+    "uniform_crop_landscape_1": ("uniform_crop_with_boxes", (48, 64), 9, {"size": 40, "spatial_idx": 1}),
+    "uniform_crop_landscape_2": ("uniform_crop_with_boxes", (48, 64), 9, {"size": 40, "spatial_idx": 2}),
+    "uniform_crop_portrait_0": ("uniform_crop_with_boxes", (64, 40), 9, {"size": 35, "spatial_idx": 0}),
+    "uniform_crop_portrait_1": ("uniform_crop_with_boxes", (64, 40), 9, {"size": 35, "spatial_idx": 1}),
+    "uniform_crop_portrait_2": ("uniform_crop_with_boxes", (64, 40), 9, {"size": 35, "spatial_idx": 2}),
+    "flip_p0": ("horizontal_flip_with_boxes", (48, 64), 9, {"prob": 0.0}),
+    "flip_p1": ("horizontal_flip_with_boxes", (48, 64), 9, {"prob": 1.0}),
+    "flip_p1_portrait": ("horizontal_flip_with_boxes", (64, 40), 9, {"prob": 1.0}),
+    "flip_half": ("horizontal_flip_with_boxes", (48, 64), 9, {"prob": 0.5}),
+    "flip_empty": ("horizontal_flip_with_boxes", (48, 64), 0, {"prob": 1.0}),
+}
+
+
+def box_case_inputs(name, dtype):
+    """(seed, float32 (3, 2, H, W) clip, (K, 4) boxes of ``dtype``) of a BOX_FUNCTIONAL_CASES entry."""
+    fn, (H, W), K, _ = BOX_FUNCTIONAL_CASES[name]
+    i = list(BOX_FUNCTIONAL_CASES).index(name)
+    return BOX_SEED + i, synthetic_clip(1, 2, H, W, seed=BOX_SEED + i)[0], synthetic_xyxy(K, H, W, seed=BOX_SEED + 100 + i,
+                                                                                         dtype=dtype)
+
+
+def call_box_case(F, name, images, boxes):
+    """Call the case's function from the functional module ``F`` (the reference's or this package's)."""
+    fn, _, _, kw = BOX_FUNCTIONAL_CASES[name]
+    f = getattr(F, fn)
+    if fn == "clip_boxes_to_image":
+        return f(boxes, images.shape[2], images.shape[3])
+    if fn == "crop_boxes":
+        return f(boxes, kw["x_offset"], kw["y_offset"])
+    if fn == "short_side_scale_with_boxes":
+        return f(images, boxes, kw["size"])
+    if fn == "random_short_side_scale_with_boxes":
+        return f(images, boxes, kw["min_size"], kw["max_size"])
+    if fn == "random_crop_with_boxes":
+        return f(images, kw["size"], boxes)
+    if fn == "uniform_crop_with_boxes":
+        return f(images, kw["size"], kw["spatial_idx"], boxes)
+    return f(kw["prob"], images, boxes)
+
+
+# The train chain of the detection transforms: per clip clip_boxes_to_image, random_short_side_scale_with_boxes,
+# random_crop_with_boxes, horizontal_flip_with_boxes, clip_boxes_to_image, on 4 clips with 0, 1, 3 and 7 boxes.
+BOX_TRAIN_CHAIN = {"T": 12, "H": 60, "W": 80, "num_samples": 4, "box_counts": (0, 1, 3, 7), "random_short_side": (40, 56),
+                   "crop": 36, "hflip_prob": 0.5, "seed": 85}
+# The detection tutorial's ava_inference_transform on uint8 frames, then the reference detection models.
+# name: (hub builder, clip frames, num_frames, slow_fast_alpha); 2 clips of 72 x 96 frames with 3 and 4 boxes.
+BOX_TUTORIAL_CASES = {
+    "slow_r50_detection": ("slow_r50_detection", 12, 4, None),
+    "slowfast_r50_detection": ("slowfast_r50_detection", 40, 32, 4),
+}
+BOX_TUTORIAL = {"H": 72, "W": 96, "crop_size": 80, "box_counts": (3, 4), "mean": (0.45, 0.45, 0.45),
+                "std": (0.225, 0.225, 0.225)}
+
+
+def train_chain_inputs():
+    """(uint8 (4, 3, T, H, W) clips, float32 box list) of BOX_TRAIN_CHAIN."""
+    c = BOX_TRAIN_CHAIN
+    clips = torch.stack([synthetic_u8_clip(c["T"], c["H"], c["W"], seed=c["seed"] + b) for b in range(4)])
+    boxes = [synthetic_xyxy(k, c["H"], c["W"], seed=c["seed"] + 10 + b) for b, k in enumerate(c["box_counts"])]
+    return clips, boxes
+
+
+def tutorial_inputs(case):
+    """(uint8 (2, 3, T, H, W) clips, float32 box list) of a BOX_TUTORIAL_CASES entry."""
+    _, T, _, _ = BOX_TUTORIAL_CASES[case]
+    c = BOX_TUTORIAL
+    clips = torch.stack([synthetic_u8_clip(T, c["H"], c["W"], seed=300 + b) for b in range(2)])
+    boxes = [synthetic_xyxy(k, c["H"], c["W"], seed=310 + b) for b, k in enumerate(c["box_counts"])]
+    return clips, boxes
+
+
+def build_tutorial_model(case, hub_module, weight_seed=1234):
+    """The case's detection model with logits out and weights randomised as build_detection_case does."""
+    hub = BOX_TUTORIAL_CASES[case][0]
+    return randomize_model(getattr(hub_module, hub)(head_activation=None), seed=weight_seed, f16_weights=True).eval()

@@ -1,6 +1,6 @@
 from .transforms import (ApplyTransformToKey, CenterCropVideo, ConvertUint8ToFloat, Div255,  # noqa: F401
                          FusedClipTransform, Normalize, RandomCropVideo, RandomShortSideScale, ShortSideScale,
                          UniformCropVideo, UniformTemporalSubsample, create_video_transform, SlowFastPackPathway,
-                         RemoveKey, RandomResizedCrop, Permute, RandAugment, AugMix)
+                         RemoveKey, RandomResizedCrop, Permute, RandAugment, AugMix, FusedDetectionTransform)
 from .mix import CutMix, MixUp, MixVideo  # noqa: F401
 from . import functional  # noqa: F401

@@ -478,3 +478,165 @@ def random_resized_crop(frames, target_height, target_width, scale, aspect_ratio
              for _ in range(x.shape[0])]
     out = clip_transform_rrc(x, boxes, (target_height, target_width))
     return out[0] if frames.dim() == 4 else out
+
+
+# ---- detection boxes (functional.py:195-445): pv_clip_boxes_transform ---------------------------------------------
+# The box functions take (K, 4) (x1, y1, x2, y2) boxes as CUDA tensors, CPU tensors or numpy arrays (the reference's
+# detection tutorial passes numpy).  Host boxes are copied to the clip's device, or to the current CUDA device when
+# there is no clip, and every result is a CUDA tensor of the boxes' dtype (float32 or float64): the engine has no CPU
+# path.  That is the one difference from the reference.
+_BOX_DT = {torch.float32: L.BOX_F32, torch.float64: L.BOX_F64}
+
+
+def _check_clip(images):
+    if not torch.is_tensor(images) or images.dim() != 4:
+        raise RuntimeError("expected a (C, T, H, W) clip")
+    if images.device.type != "cuda":
+        raise RuntimeError("pytorchvideo_b200 transforms run on the GPU only (no CPU path)")
+
+
+def _boxes_on(boxes, dev=None):
+    """``boxes`` as a contiguous (K, 4) float32 / float64 CUDA tensor on ``dev`` (default: its own CUDA device, or the
+    current one for host boxes).  Returns the tensor itself when it already is one."""
+    if isinstance(boxes, np.ndarray):
+        boxes = torch.from_numpy(boxes)
+    if not torch.is_tensor(boxes):
+        raise RuntimeError("boxes must be a tensor or a numpy array (got %s)" % type(boxes).__name__)
+    if boxes.dim() != 2 or boxes.shape[1] != 4:
+        raise RuntimeError("boxes must be (K, 4) (x1, y1, x2, y2) rows (got shape %s)" % (tuple(boxes.shape),))
+    if boxes.dtype not in _BOX_DT:
+        raise RuntimeError("boxes must be float32 or float64 (got %s)" % boxes.dtype)
+    if dev is None:
+        dev = boxes.device if boxes.device.type == "cuda" else torch.device("cuda", torch.cuda.current_device())
+    return boxes.to(dev).contiguous()
+
+
+def _int_arg(v, what):
+    if int(v) != v:
+        raise RuntimeError("%s must be an integer (got %r)" % (what, v))
+    return int(v)
+
+
+def clip_boxes_transform(boxes, steps, in_hw=(0, 0), new_hw=(0, 0), offset=(0, 0), hflip=False, out_hw=(0, 0),
+                         n_clips=1, box_start=None, geom=None, out=None, rois=False):
+    """Run pv_clip_boxes_transform on a contiguous (K, 4) float32 / float64 CUDA tensor ``boxes``.
+
+    steps   : mask of _lib.BOX_* steps, applied in the order CLIP_SRC, SCALE, CROP, CLIP_CROP, FLIP, CLIP_OUT
+    in_hw   : source frame (CLIP_SRC; the scale factor is new / in of the short side's axis)
+    new_hw, offset=(top, left), hflip : every clip's geometry, unless ``geom`` (device int32 [n_clips][6], the layout
+              pv_clip_transform_batch reads) gives it per clip
+    out_hw  : crop / output frame (CLIP_CROP, FLIP, CLIP_OUT)
+    box_start: device int32 [n_clips + 1] offsets of each clip's boxes (None: one clip owns them all)
+    out     : destination (K, 4) tensor of the boxes' dtype (None: a new tensor; ``boxes`` itself scales in place)
+    Returns (out, rois): rois is the fp32 (K, 5) (clip, x1, y1, x2, y2) tensor when ``rois`` is set, else None."""
+    dev = boxes.device
+    K = int(boxes.shape[0])
+    if out is None:
+        out = torch.empty_like(boxes)
+    r = torch.empty((K, 5), dtype=torch.float32, device=dev) if rois else None
+    if K == 0:
+        return out, r
+    if box_start is None:
+        if n_clips != 1:
+            raise RuntimeError("box_start is needed for more than one clip")
+        box_start = _dev_i32([0, K], dev)
+    d = L.BoxesDesc()
+    d.n_clips, d.n_boxes, d.steps, d.dtype = int(n_clips), K, int(steps), _BOX_DT[boxes.dtype]
+    d.in_h, d.in_w = int(in_hw[0]), int(in_hw[1])
+    d.new_h, d.new_w = int(new_hw[0]), int(new_hw[1])
+    d.top, d.left, d.hflip = int(offset[0]), int(offset[1]), 1 if hflip else 0
+    d.out_h, d.out_w = int(out_hw[0]), int(out_hw[1])
+    L.check(L.load().pv_clip_boxes_transform(C.byref(d), boxes.data_ptr(), box_start.data_ptr(),
+                                             geom.data_ptr() if geom is not None else None, out.data_ptr(),
+                                             r.data_ptr() if r is not None else None,
+                                             torch.cuda.current_stream(dev).cuda_stream), "pv_clip_boxes_transform")
+    out._pv_keepalive = (boxes, box_start, geom)     # inputs must outlive the asynchronous launch
+    return out, r
+
+
+def short_side_scale_with_boxes(images, boxes, size, interpolation="bilinear", backend="pytorch"):
+    """functional.py:195-230: the clip's short side scaled to ``size`` (short_side_scale) and the boxes multiplied by
+    the same factor, in place when ``boxes`` is a CUDA tensor (the reference's ``boxes *=``).  Returns (images, boxes)."""
+    _check_clip(images)
+    _, _, h, w = images.shape
+    b = _boxes_on(boxes, images.device)
+    images = short_side_scale(images, size, interpolation, backend)
+    _, _, new_h, new_w = images.shape
+    res, _ = clip_boxes_transform(b, L.BOX_SCALE, in_hw=(h, w), new_hw=(new_h, new_w), out=b)
+    if torch.is_tensor(boxes) and boxes.device == b.device and b is not boxes:
+        boxes.copy_(b)               # a non-contiguous CUDA view: write the result back into it
+        res = boxes
+    return images, res
+
+
+def random_short_side_scale_with_boxes(images, boxes, min_size, max_size, interpolation="bilinear",
+                                       backend="pytorch"):
+    """functional.py:233-264: the short side drawn with torch.randint(min_size, max_size + 1) (torch's global RNG)."""
+    size = torch.randint(min_size, max_size + 1, (1,)).item()
+    return short_side_scale_with_boxes(images, boxes, size, interpolation, backend)
+
+
+def random_crop_offsets(height, width, size):
+    """The offsets random_crop_with_boxes draws (functional.py:284-293): numpy's global RNG, exclusive upper bound,
+    y first and each only when that side is longer than ``size``.  None when the frame already is size x size (the
+    reference then returns the clip alone and draws nothing)."""
+    if height == size and width == size:
+        return None
+    y = int(np.random.randint(0, height - size)) if height > size else 0
+    x = int(np.random.randint(0, width - size)) if width > size else 0
+    return y, x
+
+
+def _crop_boxes_of(cropped, b, y, x):
+    out, _ = clip_boxes_transform(b, L.BOX_CROP | L.BOX_CLIP_CROP, offset=(y, x), out_hw=tuple(cropped.shape[-2:]))
+    return out
+
+
+def random_crop_with_boxes(images, size, boxes):
+    """functional.py:267-299.  Returns (cropped view, boxes) - or ``images`` alone, as the reference does, when the
+    clip already is size x size."""
+    _check_clip(images)
+    b = _boxes_on(boxes, images.device)      # argument checks before any draw
+    yx = random_crop_offsets(images.shape[2], images.shape[3], size)
+    if yx is None:
+        return images
+    y, x = yx
+    cropped = images[:, :, y:y + size, x:x + size]
+    return cropped, _crop_boxes_of(cropped, b, y, x)
+
+
+def uniform_crop_with_boxes(images, size, spatial_idx, boxes):
+    """functional.py:350-377: the uniform_crop window (a view) and the boxes cropped, then clipped to it."""
+    _check_clip(images)
+    y, x, _, _ = uniform_crop_window(images.shape[2], images.shape[3], size, spatial_idx)
+    if y < 0 or x < 0:
+        raise RuntimeError("crop size %d larger than the %dx%d frame" % (size, images.shape[2], images.shape[3]))
+    cropped = images[:, :, y:y + size, x:x + size]
+    return cropped, _crop_boxes_of(cropped, _boxes_on(boxes, images.device), y, x)
+
+
+def horizontal_flip_with_boxes(prob, images, boxes):
+    """functional.py:380-404: flips when np.random.uniform() < prob (numpy's global RNG, drawn on every call).  The
+    clip is mirrored by the batched transform kernel with identity geometry (dtype preserved); the boxes become
+    x1' = (W - x2) - 1, x2' = (W - x1) - 1.  Returns (images, a new boxes tensor)."""
+    _check_clip(images)
+    b = _boxes_on(boxes, images.device)
+    flip = np.random.uniform() < prob
+    if flip:
+        images = clip_transform_batch(images, hflip=True, out_dtype=images.dtype)
+    out, _ = clip_boxes_transform(b, L.BOX_FLIP if flip else 0, hflip=flip, out_hw=tuple(images.shape[-2:]))
+    return images, out
+
+
+def clip_boxes_to_image(boxes, height, width):
+    """functional.py:407-426: x to [0, width - 1], y to [0, height - 1] (numpy's minimum / maximum)."""
+    b = _boxes_on(boxes)
+    out, _ = clip_boxes_transform(b, L.BOX_CLIP_OUT, out_hw=(_int_arg(height, "height"), _int_arg(width, "width")))
+    return out
+
+
+def crop_boxes(boxes, x_offset, y_offset):
+    """functional.py:429-445: x - x_offset, y - y_offset."""
+    b = _boxes_on(boxes)
+    out, _ = clip_boxes_transform(b, L.BOX_CROP, offset=(_int_arg(y_offset, "y_offset"), _int_arg(x_offset, "x_offset")))
+    return out

@@ -5,9 +5,11 @@ ShortSideScale -> crop as ONE kernel launch reading uint8 frames (CTHW or the de
 view) and writing the f16/f32 network input.  The single-op modules run the same kernel with
 identity settings so that a torchvision ``Compose`` of them still works (one launch per op).
 """
+import numpy as np
 import torch
 import torch.nn as nn
 
+from .. import _lib as L
 from . import functional as Fv
 from .augment import AugMix, RandAugment  # noqa: F401
 
@@ -236,6 +238,126 @@ class FusedClipTransform(nn.Module):
 
     def _is_random(self):
         return self.random_short_side is not None or self.hflip_prob > 0.0 or (self.crop is not None and self.crop[0] == "random")
+
+
+class FusedDetectionTransform(nn.Module):
+    """The detection input chain on a batch of clips with ragged box lists: ONE pv_clip_transform_batch launch for the
+    clips and ONE pv_clip_boxes_transform launch for the boxes and the RoI rows.
+
+    Per clip, the output is what these reference calls give, in this order (transforms/functional.py, and the
+    ``ava_inference_transform`` of the detection tutorial): uniform_temporal_subsample, /255, clip_boxes_to_image
+    (source frame), [random_]short_side_scale_with_boxes, random_crop_with_boxes or uniform_crop_with_boxes
+    (``crop``), horizontal_flip_with_boxes (``hflip_prob`` > 0), normalize, clip_boxes_to_image (output frame) and
+    the slow / fast split.  With ``short_side`` and no crop this is ``ava_inference_transform``.
+
+    crop: None | ("random", size) | ("uniform", size, spatial_idx).  The draws are the reference functions' own, per
+    clip in clip order: torch.randint (random short side), np.random.randint for y then x (random crop, each only when
+    that side is longer than the crop), np.random.uniform (flip), so a batch reproduces B sequential reference calls
+    under the same torch and numpy seeds."""
+
+    def __init__(self, num_samples, mean, std, short_side=None, random_short_side=None, crop=None, hflip_prob=0.0,
+                 slowfast_alpha=None, div255=True, out_dtype=torch.float16):
+        super().__init__()
+        if short_side is not None and random_short_side is not None:
+            raise ValueError("give short_side or random_short_side, not both")
+        if crop is not None and not ((crop[0] == "random" and len(crop) == 2) or (crop[0] == "uniform" and len(crop) == 3)):
+            raise ValueError("crop must be None, ('random', size) or ('uniform', size, spatial_idx) (got %r)" % (crop,))
+        if crop is not None and crop[0] == "uniform" and crop[2] not in (0, 1, 2):
+            raise ValueError("spatial_idx must be 0, 1 or 2")
+        self.num_samples, self.mean, self.std = num_samples, mean, std
+        self.short_side, self.random_short_side, self.crop = short_side, random_short_side, crop
+        self.hflip_prob, self.slowfast_alpha = float(hflip_prob), slowfast_alpha
+        self.div255, self.out_dtype = div255, out_dtype
+
+    def plan(self, shape):
+        """One clip's host draws for an input of ``shape`` (C, T, H, W): ((new_h, new_w), (top, left, out_h, out_w),
+        flip)."""
+        _, _, H, W = shape
+        side = self.short_side
+        if self.random_short_side is not None:
+            lo, hi = self.random_short_side
+            side = torch.randint(lo, hi + 1, (1,)).item()
+        nh, nw = (H, W) if side is None else Fv.short_side_size(H, W, side)
+        top, left, oh, ow = 0, 0, nh, nw
+        if self.crop is not None and self.crop[0] == "random":
+            size = self.crop[1]
+            # A frame that already is size x size draws nothing and is not cropped.  Its boxes still take the crop's
+            # clip at offset 0: clip, flip and the final clip give the boxes that flip and the final clip alone give.
+            top, left = Fv.random_crop_offsets(nh, nw, size) or (0, 0)
+            oh, ow = min(size, nh - top), min(size, nw - left)
+        elif self.crop is not None:
+            top, left, oh, ow = Fv.uniform_crop_window(nh, nw, self.crop[1], self.crop[2])
+            if top < 0 or left < 0:
+                raise RuntimeError("crop size %d larger than the %dx%d frame" % (self.crop[1], nh, nw))
+        flip = bool(np.random.uniform() < self.hflip_prob) if self.hflip_prob > 0.0 else False
+        return (nh, nw), (top, left, oh, ow), flip
+
+    def _boxes(self, boxes, B, dev):
+        """The box lists as one contiguous (K, 4) device tensor and the host offsets of each clip's rows."""
+        if torch.is_tensor(boxes) or isinstance(boxes, np.ndarray):
+            if B != 1:
+                raise RuntimeError("a batch of %d clips needs a list of %d box arrays" % (B, B))
+            boxes = [boxes]
+        if not isinstance(boxes, (list, tuple)) or len(boxes) != B:
+            raise RuntimeError("expected one (K, 4) box array per clip (%d clips)" % B)
+        rows = [torch.from_numpy(b) if isinstance(b, np.ndarray) else b for b in boxes]
+        for b in rows:
+            if not torch.is_tensor(b) or b.dim() != 2 or b.shape[1] != 4:
+                raise RuntimeError("every box array must be (K, 4) (x1, y1, x2, y2) rows")
+        dtypes = set(b.dtype for b in rows)
+        if len(dtypes) != 1 or rows[0].dtype not in Fv._BOX_DT:
+            raise RuntimeError("boxes must all be float32 or all float64 (got %s)" % sorted(str(d) for d in dtypes))
+        start = [0]
+        for b in rows:
+            start.append(start[-1] + int(b.shape[0]))
+        if all(b.device.type == "cpu" for b in rows):
+            flat = torch.cat(rows, 0).to(dev) if start[-1] else torch.empty((0, 4), dtype=rows[0].dtype, device=dev)
+        else:
+            flat = torch.empty((start[-1], 4), dtype=rows[0].dtype, device=dev)
+            for b, s, e in zip(rows, start[:-1], start[1:]):
+                flat[s:e].copy_(b)
+        return flat.contiguous(), start
+
+    def forward(self, clips, boxes):
+        """clips: (C, T, H, W) or (B, C, T, H, W) uint8 / float32 CUDA clip(s), CTHW or the decoder's THWC-strided
+        layout; boxes: a list of B (K_b, 4) arrays in source pixels (or one array for one clip).  Returns (inputs,
+        rois): the clip batch, or [slow, fast], and the fp32 (sum K_b, 5) (clip, x1, y1, x2, y2) RoI rows."""
+        if not torch.is_tensor(clips) or clips.dim() not in (4, 5):
+            raise RuntimeError("expected a (C, T, H, W) or (B, C, T, H, W) clip tensor")
+        if clips.device.type != "cuda":
+            raise RuntimeError("pytorchvideo_b200 transforms run on the GPU only (no CPU path)")
+        x = clips.unsqueeze(0) if clips.dim() == 4 else clips
+        B, _, T, H, W = x.shape
+        dev = x.device
+        flat, start = self._boxes(boxes, B, dev)
+        plans = [self.plan(x.shape[1:]) for _ in range(B)]
+        (oh, ow) = plans[0][1][2:]
+        if any(p[1][2:] != (oh, ow) for p in plans):
+            raise RuntimeError("the clips of a batch come out at different sizes (random short side without a crop?)")
+        idx = Fv.temporal_indices(T, self.num_samples)
+        geom = [(p[0], p[1], p[2]) for p in plans]
+        inputs = Fv.clip_transform_batch(x, frame_idx=idx, resize_hw=plans[0][0], window=plans[0][1], mean=self.mean,
+                                         std=self.std, div255=self.div255, out_dtype=self.out_dtype, geom=geom,
+                                         slow_alpha=self.slowfast_alpha)
+        if clips.dim() == 4:
+            inputs = [t[0] for t in inputs] if self.slowfast_alpha is not None else inputs[0]
+        steps = L.BOX_CLIP_SRC | L.BOX_CLIP_OUT
+        if self.short_side is not None or self.random_short_side is not None:
+            steps |= L.BOX_SCALE
+        if self.crop is not None:
+            steps |= L.BOX_CROP | L.BOX_CLIP_CROP
+        if self.hflip_prob > 0.0:
+            steps |= L.BOX_FLIP
+        if start[-1] == 0:
+            return inputs, torch.empty((0, 5), dtype=torch.float32, device=dev)
+        table = []
+        for (nh, nw), (top, left, _, _), flip in plans:
+            table += [nh, nw, top, left, 1 if flip else 0, 0]
+        table = torch.tensor(table + start, dtype=torch.int32).to(dev)      # one copy: geometry, then offsets
+        _, rois = Fv.clip_boxes_transform(flat, steps, in_hw=(H, W), out_hw=(oh, ow), n_clips=B,
+                                          box_start=table[6 * B:], geom=table[:6 * B], rois=True)
+        rois._pv_keepalive = (flat, table)
+        return inputs, rois
 
 
 class SlowFastPackPathway(nn.Module):
