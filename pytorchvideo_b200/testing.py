@@ -322,8 +322,11 @@ F16_EPS = 2.0 ** -11          # unit roundoff of f16 (one round-to-nearest of th
 ACC_EPS = 2.0 ** -20          # fp32 accumulation allowance per unit of |x|.|w| magnitude, see assert_close_to_f64
 
 
-def assert_close_to_f64(got, ref64, absref64, k_len, acc_eps=ACC_EPS, what="", extra64=None):
-    """Compare an f16-storage kernel result with its float64 reference.
+F32_EPS = 2.0 ** -24          # unit roundoff of fp32 (rnd_eps of a kernel that stores fp32)
+
+
+def assert_close_to_f64(got, ref64, absref64, k_len, acc_eps=ACC_EPS, what="", extra64=None, rnd_eps=F16_EPS):
+    """Compare an f16-storage (or, with rnd_eps=F32_EPS, fp32-storage) kernel result with its float64 reference.
 
     ref64: the operation in float64 on the exact f16-grid operands the kernel received.  absref64: the same operation
     on |x| and |w| with |scale|, plus |bias| and |residual| - the magnitude the result is summed from.  Each element
@@ -339,21 +342,24 @@ def assert_close_to_f64(got, ref64, absref64, k_len, acc_eps=ACC_EPS, what="", e
     check must see.  Returns (largest err / tol,
     largest share of the accumulation term used, largest share of extra64 used): a correctly rounded result may use
     nearly all of the rounding term, so the second number is the margin of the accumulation constant; the third
-    charges everything beyond the rounding term to extra64 (0.0 without extra64)."""
+    charges everything beyond the rounding term to extra64 (0.0 without extra64).
+    rnd_eps: the unit roundoff of the stored result; the absolute floor scales with it (2^-24 for f16 storage, half
+    its smallest subnormal step; 2^-37 for fp32 storage)."""
     got64 = got.detach().double().cpu()
     ref64, absref64 = ref64.double().cpu(), absref64.double().cpu()
     assert got64.shape == ref64.shape, (what, tuple(got64.shape), tuple(ref64.shape))
     assert bool(torch.isfinite(got64).all()), "%s: non-finite output" % what
     err = got64 - ref64
     acc = acc_eps * (1.0 + k_len / 64.0) * absref64
-    tol = F16_EPS * ref64.abs() + acc + 2.0 ** -24
+    floor = 2.0 ** -24 * (rnd_eps / F16_EPS)
+    tol = rnd_eps * ref64.abs() + acc + floor
     if extra64 is not None:
         extra64 = extra64.double().cpu()
         assert extra64.shape == ref64.shape and bool((extra64 >= 0).all()), what
         tol = tol + extra64
     ratio = (err.abs() / tol)
     worst = int(ratio.argmax())
-    excess = (err.abs() - F16_EPS * ref64.abs() - 2.0 ** -24).clamp_min(0)
+    excess = (err.abs() - rnd_eps * ref64.abs() - floor).clamp_min(0)
     acc_ratio = float((excess / acc.clamp_min(1e-300)).max()) if bool((acc > 0).any()) else 0.0
     extra_ratio = 0.0
     if extra64 is not None and bool((extra64 > 0).any()):
@@ -365,7 +371,7 @@ def assert_close_to_f64(got, ref64, absref64, k_len, acc_eps=ACC_EPS, what="", e
     n = int(normal.sum())
     if n >= 256:
         bias = float((err[normal] * ref64[normal].sign()).mean())
-        step = F16_EPS * float(ref64[normal].abs().mean())
+        step = rnd_eps * float(ref64[normal].abs().mean())
         limit = 0.25 * step + acc_eps * float(absref64[normal].mean())
         assert abs(bias) <= limit, "%s: mean signed error %.3g exceeds %.3g (biased rounding)" % (what, bias, limit)
     return float(ratio.max()), acc_ratio, extra_ratio

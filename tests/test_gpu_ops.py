@@ -149,88 +149,6 @@ def test_dwconv3d_se_sums(case, dtype):
         float((sums - ref_sums).abs().max())
 
 
-@pytest.mark.parametrize("mode,k,s,p", [("max", (1, 3, 3), (1, 2, 2), (0, 1, 1)), ("avg", (4, 5, 5), (1, 1, 1), (0, 0, 0)),
-                                        ("max", (3, 3, 3), (1, 2, 2), (1, 1, 1)), ("avg", (2, 1, 1), (2, 1, 1), (0, 0, 0))])
-def test_pool3d(mode, k, s, p):
-    from pytorchvideo_b200 import ops
-    x = torch.randn(2, 24, 4, 11, 11, generator=torch.Generator().manual_seed(3))
-    ref = F.max_pool3d(x, k, s, p) if mode == "max" else F.avg_pool3d(x, k, s, p)
-    got = ops.pool3d(x.to(_dev()), mode, k, s, p, "f32").cpu()
-    assert torch.allclose(got, ref, rtol=1e-5, atol=1e-6)
-
-
-@pytest.mark.parametrize("dtype", ["f32", "f16"])
-@pytest.mark.parametrize("rows,C", [(77, 96), (5, 8), (130, 192), (33, 384), (19, 768), (7, 1024), (64, 40)])
-def test_layernorm(rows, C, dtype):
-    """C <= 768 runs the row-in-registers kernel (sub-warp groups for narrow rows), wider rows the generic one."""
-    from pytorchvideo_b200 import ops
-    g = torch.Generator().manual_seed(4 + C)
-    x = torch.randn(rows, C, generator=g) * 3 + 1
-    gamma, beta = torch.rand(C, generator=g) + 0.5, torch.rand(C, generator=g) - 0.5
-    if dtype == "f16":
-        x = x.half().float()
-    ref = F.layer_norm(x, (C,), gamma, beta, 1e-6)
-    got = ops.layernorm(x.to(_dev()), gamma, beta, 1e-6, dtype).cpu()
-    if dtype == "f32":
-        assert torch.allclose(got, ref, rtol=1e-4, atol=1e-5), float((got - ref).abs().max())
-    else:   # one f16 rounding of the stored output
-        assert torch.allclose(got, ref, rtol=2e-3, atol=2e-3), float((got - ref).abs().max())
-
-
-@pytest.mark.parametrize("dtype", ["f16", "f32"])
-@pytest.mark.parametrize("B,npos,heads,hd", [(3, 11, 2, 96), (2, 50, 4, 96), (2, 7, 1, 8)])
-def test_layernorm_sets_and_cls_rows(B, npos, heads, hd, dtype):
-    """pv_layernorm_sets: pooled K | V (adjacent channel slices, norm_k | norm_v) normalised per head by one in-place
-    launch; the cls row of every sample is read from the un-pooled tensor (attention.py:184-205)."""
-    from pytorchvideo_b200 import _lib as L
-    lib = L.load()
-    tdt = torch.float16 if dtype == "f16" else torch.float32
-    g = torch.Generator().manual_seed(5 + npos)
-    dim = heads * hd
-    src_npos = npos + 9                                            # the un-pooled tensor has more rows per sample
-    src = (torch.randn(B, src_npos, 3 * dim, generator=g) * 2).to(tdt)     # qkv buffer: k | v = channels [dim, 3 dim)
-    y = (torch.randn(B, npos, 2 * dim, generator=g) * 2 + 0.5).to(tdt)
-    gam = torch.rand(2, hd, generator=g) + 0.5
-    bet = torch.rand(2, hd, generator=g) - 0.5
-    full = y.float().clone()
-    full[:, 0] = src[:, 0, dim:].float()
-    ref = torch.empty_like(full)
-    for sset in range(2):
-        blk = full[..., sset * dim:(sset + 1) * dim].reshape(B, npos, heads, hd)
-        ref[..., sset * dim:(sset + 1) * dim] = F.layer_norm(blk, (hd,), gam[sset], bet[sset], 1e-6).reshape(B, npos, dim)
-    dev = _dev()
-    src_d, y_d, gam_d, bet_d = src.to(dev), y.to(dev), gam.to(dev).contiguous(), bet.to(dev).contiguous()
-    esz = src_d.element_size()
-    L.check(lib.pv_layernorm_sets(y_d.data_ptr(), y_d.data_ptr(), L.PV_F16 if dtype == "f16" else L.PV_F32, B * npos,
-                                  2 * heads, hd, 2 * dim, 2 * dim, gam_d.data_ptr(), bet_d.data_ptr(), heads,
-                                  src_d.data_ptr() + dim * esz, src_npos * 3 * dim, npos, 1e-6,
-                                  torch.cuda.current_stream().cuda_stream), "pv_layernorm_sets")
-    torch.cuda.synchronize()
-    got = y_d.float().cpu()
-    tol = dict(rtol=1e-4, atol=1e-5) if dtype == "f32" else dict(rtol=2e-3, atol=2e-3)
-    assert torch.allclose(got, ref, **tol), float((got - ref).abs().max())
-
-
-@pytest.mark.parametrize("a_dtype", ["f32", "f16"])
-@pytest.mark.parametrize("with_b", [True, False])
-@pytest.mark.parametrize("rows,C", [(77, 96), (130, 192), (33, 384), (19, 768), (5, 8)])
-def test_add_layernorm_fp32_trunk(rows, C, with_b, a_dtype):
-    """pv_add_layernorm (MViT fp32 residual trunk): the sum is exact fp32, the LayerNorm output takes one f16 rounding."""
-    from pytorchvideo_b200 import ops
-    g = torch.Generator().manual_seed(11 + C)
-    a = torch.randn(rows, C, generator=g) * 3 + 1
-    b = (torch.randn(rows, C, generator=g) * 0.5).half()
-    if a_dtype == "f16":
-        a = a.half()
-    gamma, beta = torch.rand(C, generator=g) + 0.5, torch.rand(C, generator=g) - 0.5
-    ref_s = a.float() + (b.float() if with_b else 0.0)
-    ref_y = F.layer_norm(ref_s, (C,), gamma, beta, 1e-6)
-    s, y = ops.add_layernorm(a.to(_dev()), b.to(_dev()) if with_b else None, gamma, beta, 1e-6)
-    assert s.dtype == torch.float32 and y.dtype == torch.float16
-    assert torch.equal(s.cpu(), ref_s)                      # one fp32 add: bit-exact
-    assert torch.allclose(y.float().cpu(), ref_y, rtol=2e-3, atol=2e-3), float((y.float().cpu() - ref_y).abs().max())
-
-
 @pytest.mark.parametrize("Nq,Nk,resid", [(50, 50, False), (393, 393, False), (130, 37, True)])
 def test_attention(Nq, Nk, resid):
     from pytorchvideo_b200 import ops
