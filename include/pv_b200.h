@@ -35,7 +35,7 @@ typedef enum pv_status {
   PV_ERR_NO_DEVICE = -4    /* no sm_90 device visible                                */
 } pv_status;
 
-typedef enum pv_dtype { PV_F16 = 0, PV_F32 = 1, PV_U8 = 2 } pv_dtype;
+typedef enum pv_dtype { PV_F16 = 0, PV_F32 = 1, PV_U8 = 2, PV_I64 = 3 /* pv_soft_target_ce targets only */ } pv_dtype;
 
 typedef enum pv_act {
   PV_ACT_NONE = 0,
@@ -612,6 +612,52 @@ int pv_reduce_fusion(const void* const* xs, const long long* x_row_strides, int 
  * memory every step and multiply on the CUDA cores.                                                               */
 int pv_lstm_recurrence(const void* G, int dtype, long long g_row_stride, const float* w_hh_t, const unsigned char* mask,
                        int B, int T, int H, int ndir, void* y, long long y_row_stride, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Self-supervised objectives (models/simclr.py, byol.py, memory_bank.py) and the soft-target cross entropy
+ * (losses/soft_target_cross_entropy.py), csrc/pv_contrastive.cu.  Embeddings, logits and losses are fp32; every
+ * reduction runs in a fixed order (no atomics on values), so repeated calls are bitwise identical.  Row strides are in
+ * elements.  row_loss is a caller-owned fp32 [rows] workspace that receives the per-row terms; loss one fp32.
+ * pv_rows_l2_normalize : y[r] = x[r] / max(||x[r]||_2, 1e-12) (F.normalize(x, p=2, dim=1), simclr.py:43,48,
+ *                        byol.py:112,122, memory_bank.py:90); x f16 | f32, y fp32.
+ * pv_contrastive_ce    : mode 0 (SimCLR, simclr.py:51-65): logits q_n . k_m / temperature for the M <= 16384 key rows
+ *                        (fp32 FMA, kept in shared memory), row_loss[n] = logsumexp_m - logit[n][row_offset + n],
+ *                        loss = mean.  mode 1 (BYOL, byol.py:68-77): M == N, loss = -mean_n(q_n . k_n).
+ * pv_memory_bank_ce    : memory_bank.py:92-103 for B samples: logits[b][j] = memory[idx[b][j]] . x[b] / temperature
+ *                        over the K1 = neg_size + 1 indices of row b (int64 [B][K1], dense fp32 bank of bank_rows x dim,
+ *                        64-bit offsets), row_loss[b] = logsumexp_j - logits[b][0], loss = mean.  logits is an fp32
+ *                        [B][K1] workspace.  An index outside [0, bank_rows) sets *flag (device int, cleared by the
+ *                        call) and its row is never read; the caller raises.  dim <= 12288.
+ * pv_soft_target_ce    : soft_target_cross_entropy.py:66-81: t = target (t / (eps + sum t) with normalize),
+ *                        row_loss[n] = sum_c -t_c * log_softmax(x[n])_c, and with reduce_mean loss = mean_n.
+ *                        x f16 | f32, target f16 | f32 | PV_I64 (one-hot rows of int64).
+ * pv_ema_update        : byol.py:93-101 over many tensors in one launch: dst[t][i] = dst[t][i] * mmt + src[t][i] *
+ *                        one_minus_mmt, each product and the sum rounded once (no FMA).  dst / src / numel are DEVICE
+ *                        arrays of the fp32 tensors; chunks[b] = (t << 40) | start names the 4096 elements of tensor t
+ *                        from `start` that block b updates.
+ * ------------------------------------------------------------------------------------------- */
+int pv_rows_l2_normalize(const void* x, int dtype, long long x_row_stride, float* y, long long y_row_stride, int rows,
+                         int C, void* stream);
+int pv_contrastive_ce(const float* q, long long q_row_stride, const float* k, long long k_row_stride, int N, int M, int C,
+                      float temperature, long long row_offset, int mode, float* row_loss, float* loss, void* stream);
+int pv_memory_bank_ce(const float* x, long long x_row_stride, const float* memory, long long bank_rows, int dim,
+                      const long long* idx, int B, int K1, float temperature, float* logits, float* row_loss, float* loss,
+                      int* flag, void* stream);
+int pv_soft_target_ce(const void* x, int x_dtype, long long x_row_stride, const void* target, int t_dtype,
+                      long long t_row_stride, int N, int C, int normalize, float eps, int reduce_mean, float* row_loss,
+                      float* loss, void* stream);
+int pv_ema_update(float* const* dst, const float* const* src, const long long* numel, const long long* chunks,
+                  int n_chunks, float mmt, float one_minus_mmt, void* stream);
+/* pv_weights_refresh (byol.py:93-101 without a recompile: BYOL's momentum plan after pv_ema_update): rewrites a compiled
+ * plan's constants in place, so a captured CUDA graph stays valid.  Gather: gather_jobs holds 5 int64 per constant
+ * (dst pointer, PV_F16 | PV_F32, n elements, offset into map, source slot); dst[i] = map[off + i] < 0 ? 0 :
+ * srcs[slot][map[off + i]] (fp32 sources, stored with one round to nearest even); gather_chunks[b] = (job << 40) | start
+ * names the 4096 elements block b writes.  Fold: fold_jobs holds 9 int64 per BatchNorm fold (scale dst, bias dst, c_out,
+ * conv_bias, gamma, beta, running_mean, running_var as device pointers or 0, eps as the bits of a double) and computes
+ * packing.fold_bn in fp64, each operation correctly rounded, then fp32: the bytes of a fresh compile.  All tables are
+ * DEVICE arrays.                                                                                                   */
+int pv_weights_refresh(const long long* gather_jobs, const long long* gather_chunks, int n_gather_chunks, const int* map,
+                       const float* const* srcs, const long long* fold_jobs, int n_fold_jobs, void* stream);
 
 #ifdef __cplusplus
 }

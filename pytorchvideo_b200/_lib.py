@@ -8,7 +8,7 @@ import os
 
 from . import _build
 
-PV_F16, PV_F32, PV_U8 = 0, 1, 2
+PV_F16, PV_F32, PV_U8, PV_I64 = 0, 1, 2, 3
 ACT_NONE, ACT_RELU, ACT_SWISH, ACT_GELU, ACT_SIGMOID, ACT_HSWISH = 0, 1, 2, 3, 4, 5
 ALGO_AUTO, ALGO_DIRECT, ALGO_TCGEN05 = 0, 1, 2
 POOL_MAX, POOL_AVG = 0, 1
@@ -189,6 +189,15 @@ SIGNATURES = {
     "pv_reduce_fusion": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, c_ll, C.c_int, C.c_int, c_vp, c_ll, c_vp]),
     "pv_lstm_recurrence": (C.c_int, [c_vp, C.c_int, c_ll, c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_ll,
                                      c_vp]),
+    "pv_rows_l2_normalize": (C.c_int, [c_vp, C.c_int, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp]),
+    "pv_contrastive_ce": (C.c_int, [c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, C.c_int, C.c_float, c_ll, C.c_int, c_vp,
+                                    c_vp, c_vp]),
+    "pv_memory_bank_ce": (C.c_int, [c_vp, c_ll, c_vp, c_ll, C.c_int, c_vp, C.c_int, C.c_int, C.c_float, c_vp, c_vp, c_vp,
+                                    c_vp, c_vp]),
+    "pv_soft_target_ce": (C.c_int, [c_vp, C.c_int, c_ll, c_vp, C.c_int, c_ll, C.c_int, C.c_int, C.c_int, C.c_float,
+                                    C.c_int, c_vp, c_vp, c_vp]),
+    "pv_ema_update": (C.c_int, [c_vp, c_vp, c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp]),
+    "pv_weights_refresh": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int, c_vp]),
 }
 
 _lib = None

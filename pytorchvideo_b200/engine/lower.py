@@ -89,6 +89,7 @@ class Lowering:
         self.p = plan
         self.extra = tuple(extra)     # non-tensor forward arguments of the root module (thw_shape)
         self.aux_out = None           # host-side second result of the root module (pooled thw)
+        self.fuse_rows = False        # Linear -> ReLU as one launch (models/embedding.py EmbeddingChain)
 
     # ---- leaf helpers --------------------------------------------------------------------
     def conv(self, x: TRef, conv: nn.Conv3d, bn=None, act=None, residual=None, name="conv", se_sums=False, addend=None):
@@ -207,8 +208,17 @@ class Lowering:
         return x
 
     def lower_Sequential(self, m, x, name):
-        for i, blk in enumerate(m):
-            x = self.lower(blk, x, "%s.%d" % (name, i))
+        mods = list(m)
+        i = 0
+        while i < len(mods):
+            # Linear -> BatchNorm (which has no lowering of its own) always fuses; inside the embedding path of the
+            # self-supervised models (``fuse_rows``) a Linear -> ReLU fuses as well
+            if isinstance(mods[i], nn.Linear) and isinstance(x, TRef) and (
+                    self.fuse_rows or (i + 1 < len(mods) and _is_bn(mods[i + 1]))):
+                x, i = _lower_linear_chain(self, mods, i, x, name)
+                continue
+            x = self.lower(mods[i], x, "%s.%d" % (name, i))
+            i += 1
         return x
 
     def lower_ResNetBasicStem(self, m, x, name, addend=None):
@@ -619,6 +629,8 @@ class Lowering:
         if pool is not None:
             x = self.lower(pool, x, name + ".pool") if type(pool).__name__ == "ProjectedPool" else self.pool(x, pool, name + ".pool")
         proj = m.proj
+        if proj is None:
+            return _lower_headless(self, m, x, name)
         if not isinstance(proj, nn.Linear):
             raise NotImplementedError("head proj %s unsupported" % type(proj).__name__)
         w = proj.weight.reshape(proj.out_features, proj.in_features, 1, 1, 1)
@@ -1671,3 +1683,54 @@ Lowering.lower_EfficientX3d = _lower_efficient_x3d
 Lowering.lower_AdaptiveAvgPool3dOutSize1 = _lower_pool_size1
 Lowering.lower_HardSwish = _lower_hardswish
 Lowering.lower_Hardswish = _lower_hardswish
+
+
+# =============================================================================================
+# Projector MLPs on (B, C) rows (layers/mlp.py make_multilayer_perceptron, the BYOL predictor of models/byol.py:59-64)
+# and the headless ResNet trunk they follow (head.py:371-391 with ``proj = None``).  A row tensor is a TRef of
+# N rows with T = H = 1 and W = 1 (a pooled clip) or W = tokens (a (B, C) network input).
+# =============================================================================================
+def _lower_linear_chain(self, mods, i, x, name):
+    """``mods[i]`` (a Linear) with an eval BatchNorm (BatchNorm1d, SyncBatchNorm, NaiveSyncBatchNorm1d) and / or a ReLU
+    right after it, as ONE GEMM launch: the BatchNorm folds into the epilogue scale and bias (packing.fold_bn), the ReLU
+    is the epilogue activation.  Returns (rows, index of the next module)."""
+    lin = mods[i]
+    lname = "%s.%d" % (name, i)
+    _token_input(x, lname, "Linear")
+    if lin.in_features != x.C:
+        raise RuntimeError("%s: in_features %d, input has %d features" % (lname, lin.in_features, x.C))
+    j = i + 1
+    bn = None
+    if j < len(mods) and _is_bn(mods[j]):
+        bn = mods[j]
+        if bn.running_mean is None or bn.running_var is None:
+            raise NotImplementedError("%s.%d: BatchNorm without running statistics normalises with batch statistics, "
+                                      "which the eval-mode engine does not compute" % (name, j))
+        if bn.num_features != lin.out_features:
+            raise RuntimeError("%s.%d: BatchNorm has %d features, the Linear %d" % (name, j, bn.num_features,
+                                                                                  lin.out_features))
+        j += 1
+    act = L.ACT_NONE
+    if j < len(mods) and type(mods[j]).__name__ == "ReLU":
+        act = L.ACT_RELU
+        j += 1
+    w = lin.weight.reshape(lin.out_features, lin.in_features, 1, 1, 1)
+    y = self.p.emit_conv(x, w, lin.bias, bn, (1, 1, 1), (0, 0, 0), (1, 1, 1), 1, act, None, lname)
+    y.is_tokens = getattr(x, "is_tokens", False)
+    return _mark(y, x, retargetable=True), j
+
+
+def _lower_headless(self, m, x, name):
+    """ResNetBasicHead with its projection removed (``blocks[-1].proj = None``, the trunk of a self-supervised
+    checkpoint): [pool] -> [activation] -> [output_pool + view(B, -1)], the pooled features as (B, C) rows."""
+    act = getattr(m, "activation", None)
+    if act is not None:
+        an = type(act).__name__
+        if an != "Sigmoid":
+            raise NotImplementedError("%s: activation %s of a head without proj unsupported" % (name, an))
+        x = self.p.emit_act(x, L.ACT_SIGMOID, name + ".activation")
+    if getattr(m, "output_pool", None) is None:
+        return x
+    if x.npos != 1:
+        x = self.p.emit_pool(x, L.POOL_AVG, (x.T, x.H, x.W), (x.T, x.H, x.W), (0, 0, 0), name + ".output_pool")
+    return _tok_out(x, squeeze=True)

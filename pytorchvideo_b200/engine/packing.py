@@ -38,6 +38,8 @@ def fold_bn(conv_bias, bn, c_out, c_out_pad):
     out_b = torch.zeros(c_out_pad, dtype=torch.float32)
     out_s[:c_out] = scale.float()
     out_b[:c_out] = bias.float()
+    # where the vectors come from, for the in-place weight refresh of a compiled plan (engine/refresh.py)
+    out_s._pv_fold, out_b._pv_fold = (conv_bias, bn, int(c_out), 0), (conv_bias, bn, int(c_out), 1)
     return out_s, out_b
 
 

@@ -101,6 +101,7 @@ class Plan:
         self.side_outputs = []      # (weakref to module, Buf, shape): per-module results besides the output (attention weights)
         self.bufs = []
         self.consts = []       # keep device parameter tensors alive
+        self.const_folds = []  # per const: (conv_bias, bn, c_out, 0 scale | 1 bias) of a packing.fold_bn vector, else None
         self.zero_bufs = []    # f32 accumulators that must be cleared every run (SE sums)
         self.finalized = False
         self.graph = None
@@ -131,8 +132,10 @@ class Plan:
         return TRef(b, N, T, H, W, C, Cp)
 
     def const(self, t, dtype=None):
+        fold = getattr(t, "_pv_fold", None)
         t = t.detach().to(device=self.device, dtype=dtype if dtype is not None else t.dtype).contiguous()
         self.consts.append(t)
+        self.const_folds.append(fold if dtype is None else None)   # packing.fold_bn origin (engine/refresh.py)
         return t
 
     def finalize(self):
@@ -742,6 +745,10 @@ class Plan:
         (the layout MViT blocks exchange).  One cast/copy launch into the plan's dtype."""
         shp = tuple(static_in.shape)
         B, N, Cc = (shp[0], 1, shp[1]) if len(shp) == 2 else shp
+        if Cc % 8 and self.dt == L.PV_F16 and len(shp) == 2:
+            # (batch, feature) rows of any width (the projector MLPs of the self-supervised models): rows padded to a
+            # multiple of 8 with zero channels, the layout of a (B, C, 1, 1, 1) clip
+            return self.materialize_input(self.emit_input_ncdhw(static_in.view(B, Cc, 1, 1, 1), Cc, PK.pad8(Cc)))
         if Cc % 8 and self.dt == L.PV_F16:
             raise RuntimeError("token width %d is not a multiple of 8 (16-byte rows are required in f16 mode)" % Cc)
         x = self.new_tensor(B, 1, 1, N, Cc, Cp=Cc)
@@ -760,6 +767,18 @@ class Plan:
         """Token TRef [B, N, C] -> f32 output buffer laid out (B, N, C) (or (B, C) with squeeze)."""
         self.materialize_input(x)
         lib = self.lib
+        if x.npos == 1 and x.C % 8 and (x.row_stride != x.C or x.Cp != x.C):
+            # padded (B, C) rows narrower than a 16-byte vector (the projector outputs of the self-supervised models),
+            # which pv_copy_rows does not take: the NDHWC -> NCDHW conversion of (B, C, 1, 1, 1) drops the pad
+            # channels on the way out
+            out = self.new_buf(x.N * x.C, L.PV_F32)
+            src = x
+
+            def fn_r(stream):
+                L.check(lib.pv_ndhwc_to_ncdhw(src.ptr(), src.dt, src.row_stride, out.tensor.data_ptr(), src.N, src.C, 1,
+                                              1, 1, stream), "pv_ndhwc_to_ncdhw(%s)" % name)
+            self.add(name, fn_r, reads=(src,), writes=(out,))
+            return out, ((x.N, x.C) if squeeze else (x.N, 1, x.C))
         if x.row_stride != x.C or x.Cp != x.C:
             dense = self.new_tensor(x.N, 1, 1, x.npos, x.C, Cp=x.C, dt=x.dt)
             src = x

@@ -7,3 +7,5 @@ from .attention import Mlp, MultiScaleAttention, MultiScaleBlock  # noqa: F401,E
 from .positional_encoding import SpatioTemporalClsPositionalEncoding  # noqa: F401,E402
 from .positional_encoding import PositionalEncoding  # noqa: F401,E402
 from .fusion import ConcatFusion, ReduceFusion, TemporalConcatFusion, make_fusion_layer  # noqa: F401,E402
+from .mlp import make_multilayer_perceptron  # noqa: F401,E402
+from .batch_norm import NaiveSyncBatchNorm1d, NaiveSyncBatchNorm2d, NaiveSyncBatchNorm3d  # noqa: F401,E402

@@ -857,3 +857,90 @@ def build_tutorial_model(case, hub_module, weight_seed=1234):
     """The case's detection model with logits out and weights randomised as build_detection_case does."""
     hub = BOX_TUTORIAL_CASES[case][0]
     return randomize_model(getattr(hub_module, hub)(head_activation=None), seed=weight_seed, f16_weights=True).eval()
+
+
+# ---- self-supervised models (models/simclr.py, byol.py, memory_bank.py; oracle/gen_golden_ssl.py) -----------------
+SSL_VIDEO_CLIP = (2, 8, 224, 224)          # (batch, frames, height, width) of the video cases
+SSL_CASES = ("simclr_unit_b1", "simclr_unit", "byol_unit", "byol_unit_mmt", "byol_syncbn", "memory_bank_unit",
+             "simclr_video", "byol_video", "memory_bank_video")
+
+
+def _slow_r50_trunk(ns):
+    """Slow-R50 (the torch.hub slow_r50 configuration) with its head projection removed, as a self-supervised
+    checkpoint is stored (``blocks[-1].proj = None``)."""
+    net = ns.create_resnet(model_depth=50, model_num_class=400, stem_conv_kernel_size=(1, 7, 7),
+                           head_pool_kernel_size=(8, 7, 7))
+    net.blocks[-1].proj = None
+    return net
+
+
+def build_ssl_case(name, ns, seed=2718):
+    """(module, forward args) of an SSL_CASES entry built from ``ns`` (a namespace with SimCLR, BYOL, MemoryBank,
+    make_multilayer_perceptron and create_resnet: this package's or the reference's).  The constructors run under
+    torch.manual_seed(seed) (MemoryBank draws its bank there), then randomize_model sets every weight; BYOL's momentum
+    backbone starts as a copy of the online one, as the reference's deepcopy makes it.  Inputs come from their own
+    generator."""
+    g = torch.Generator().manual_seed(seed + 1)
+    torch.manual_seed(seed)
+    video = name.endswith("_video")
+    if video:
+        B, T, H, W = SSL_VIDEO_CLIP
+        x1 = torch.rand((B, 3, T, H, W), generator=g)
+        x2 = torch.rand((B, 3, T, H, W), generator=g)
+        mlp = ns.make_multilayer_perceptron([2048, 2048, 128], norm=nn.BatchNorm1d)[0]
+    if name.startswith("simclr"):
+        if video:
+            m = ns.SimCLR(mlp=mlp, backbone=_slow_r50_trunk(ns))
+        else:
+            B = 1 if name.endswith("b1") else 2
+            m = ns.SimCLR(backbone=nn.Linear(8, 4), mlp=nn.Linear(4, 2), temperature=0.07)
+            x1, x2 = torch.rand((B, 8), generator=g), torch.rand((B, 8), generator=g)
+        args = (x1, x2)
+    elif name.startswith("byol"):
+        if video:
+            m = ns.BYOL(backbone=_slow_r50_trunk(ns), projector=mlp, feature_dim=128, predictor_inner=512,
+                        norm=nn.BatchNorm1d)
+        elif name in ("byol_unit", "byol_unit_mmt"):
+            m = ns.BYOL(backbone=nn.Linear(8, 4), projector=nn.Linear(4, 4), feature_dim=4, norm=nn.BatchNorm1d)
+            x1, x2 = torch.rand((2, 8), generator=g), torch.rand((2, 8), generator=g)
+        else:                                   # the default predictor norm, nn.SyncBatchNorm
+            m = ns.BYOL(backbone=nn.Linear(16, 8), feature_dim=8, predictor_inner=32)
+            x1, x2 = torch.rand((4, 16), generator=g), torch.rand((4, 16), generator=g)
+        args = (x1, x2)
+    else:
+        if video:
+            m = ns.MemoryBank(backbone=_slow_r50_trunk(ns), mlp=mlp, neg_size=4096, temperature=0.07, bank_size=4096,
+                              dim=128)
+        else:
+            m = ns.MemoryBank(backbone=nn.Linear(8, 4), mlp=nn.Linear(4, 2), temperature=0.07, bank_size=8, dim=2)
+            x1 = torch.rand((2, 8), generator=g)
+        args = (x1, torch.randint(0, m.bank_size, (x1.shape[0],), generator=g))
+    randomize_model(m, seed=seed + 2)
+    if name.startswith("byol"):
+        m.backbone_mmt.load_state_dict(m.backbone.state_dict())
+    if name == "byol_unit_mmt":               # online and momentum weights apart, a momentum that moves them far
+        randomize_model(m.backbone, seed=seed + 3)
+        m.update_mmt(0.5)
+    return m.eval(), args
+
+
+SOFT_CE_CASES = {                          # name: (N, C, target kind, normalize_targets, reduction)
+    "c2_dense": (5, 2, "dense", True, "mean"),
+    "c4_index": (7, 4, "index", True, "mean"),
+    "c128_dense_none": (33, 128, "dense", True, "none"),
+    "c2048_dense_raw": (3, 2048, "dense", False, "mean"),
+    "c400_index_none": (9, 400, "index", False, "none"),
+}
+
+
+def soft_ce_case(name, seed=404):
+    """(logits, targets, kwargs) of a SOFT_CE_CASES entry: logits with a spread of 8, soft rows that do not sum to 1
+    (the normalisation then matters), or int64 class indices."""
+    N, C, kind, norm, red = SOFT_CE_CASES[name]
+    g = torch.Generator().manual_seed(seed + C)
+    x = torch.randn((N, C), generator=g) * 4
+    if kind == "dense":
+        t = torch.rand((N, C), generator=g) * (torch.rand((N, C), generator=g) < 0.3)
+    else:
+        t = torch.randint(0, C, (N,), generator=g)
+    return x, t, {"normalize_targets": norm, "reduction": red}
