@@ -659,6 +659,48 @@ int pv_ema_update(float* const* dst, const float* const* src, const long long* n
 int pv_weights_refresh(const long long* gather_jobs, const long long* gather_chunks, int n_gather_chunks, const int* map,
                        const float* const* srcs, const long long* fold_jobs, int n_fold_jobs, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Contrastive view colour augmentation (pytorchvideo_trainer datamodule/transforms.py ColorJitterVideoSSl): torchvision's
+ * PIL ColorJitter, RandomGrayscale and Pillow's GaussianBlur on each clip stacked into one tall (n_t*H, W) RGB image,
+ * in Pillow's integer and float arithmetic (blend in C float, RGB<->HSV with its double steps, 16-bit fixed-point luma,
+ * 24-bit fixed-point box blur).  Every view k of the table reads the kept frames frame_idx[0..n_t) of source clip
+ * views[k].clip at src[clip*s_clip + c*sc + frame*st + y*sh + x*sw] and is written as uint8 to
+ * dst[k][3][n_t][H][W] (contiguous).  A source byte is the uint8 value itself (PV_U8), or for PV_F32 the truncation of
+ * x*255 (src_scale 0: x in [0, 1], torchvision's ToPILImage) or of (x/255)*255 (src_scale 1: 0..255 values after
+ * Div255), each step in fp32.
+ *   pv_colorjitter_stats   zeroes sums[0..n_views) and adds, for each view whose ops include Contrast, the integer sum
+ *                          of the luma over its stacked clip with the ops before Contrast applied (Contrast's mean).
+ *   pv_colorjitter_apply   one thread per pixel: the view's ops in order, then grayscale, then the horizontal box-blur
+ *                          passes of a blurred view on its rows in shared memory.
+ *   pv_colorjitter_vblur   the vertical passes of the blurred views over the stacked image, in column strips kept in
+ *                          shared memory, in place on dst.  Only the clip's first and last rows are image edges.
+ * views and sums are DEVICE arrays; each entry point is one launch whatever the number of views.                 */
+#define PV_CJ_BLUR_PASSES 3
+
+typedef struct pv_cj_view {
+  int clip;                          /* source clip                                                      */
+  int n_ops;                         /* ColorJitter ops applied, 0..4                                    */
+  int ops[4];                        /* in application order: 0 brightness, 1 contrast, 2 saturation, 3 hue */
+  float factor[3];                   /* blend factors of brightness, contrast, saturation (Pillow's C float) */
+  int hue_shift;                     /* byte added to H modulo 256                                       */
+  int gray;                          /* RandomGrayscale: luma to all three channels                     */
+  int blur_r;                        /* integer box radius; -1 = no blur                                 */
+  unsigned int blur_ww, blur_fw;     /* box weights of the window and of its two edge pixels, in 2^-24    */
+} pv_cj_view;
+
+typedef struct pv_colorjitter_desc {
+  int n_views, n_t, H, W;
+  long long s_clip, sc, st, sh, sw;  /* source strides in elements                                       */
+  int src_dtype;                     /* PV_U8 | PV_F32                                                   */
+  int src_scale;                     /* PV_F32: 0 = values in [0, 1], 1 = values 0..255                  */
+} pv_colorjitter_desc;
+
+int pv_colorjitter_stats(const pv_colorjitter_desc* d, const void* src, const int32_t* frame_idx,
+                         const pv_cj_view* views, unsigned long long* sums, void* stream);
+int pv_colorjitter_apply(const pv_colorjitter_desc* d, const void* src, const int32_t* frame_idx,
+                         const pv_cj_view* views, const unsigned long long* sums, uint8_t* dst, void* stream);
+int pv_colorjitter_vblur(const pv_colorjitter_desc* d, const pv_cj_view* views, uint8_t* dst, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

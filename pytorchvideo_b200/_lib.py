@@ -73,6 +73,18 @@ class MixLabelDesc(C.Structure):
                 ("s_row", c_ll), ("s_col", c_ll)]
 
 
+class CjView(C.Structure):
+    _fields_ = [("clip", C.c_int), ("n_ops", C.c_int), ("ops", C.c_int * 4), ("factor", C.c_float * 3),
+                ("hue_shift", C.c_int), ("gray", C.c_int), ("blur_r", C.c_int), ("blur_ww", C.c_uint),
+                ("blur_fw", C.c_uint)]
+
+
+class ColorJitterDesc(C.Structure):
+    _fields_ = [("n_views", C.c_int), ("n_t", C.c_int), ("H", C.c_int), ("W", C.c_int),
+                ("s_clip", c_ll), ("sc", c_ll), ("st", c_ll), ("sh", c_ll), ("sw", c_ll),
+                ("src_dtype", C.c_int), ("src_scale", C.c_int)]
+
+
 class BottleneckDesc(C.Structure):
     _fields_ = [("N", C.c_int), ("T", C.c_int), ("H", C.c_int), ("W", C.c_int),
                 ("Cin", C.c_int), ("Cmid", C.c_int), ("Cout", C.c_int), ("kt", C.c_int), ("sb", C.c_int),
@@ -198,6 +210,9 @@ SIGNATURES = {
                                     C.c_int, c_vp, c_vp, c_vp]),
     "pv_ema_update": (C.c_int, [c_vp, c_vp, c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp]),
     "pv_weights_refresh": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int, c_vp]),
+    "pv_colorjitter_stats": (C.c_int, [C.POINTER(ColorJitterDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_colorjitter_apply": (C.c_int, [C.POINTER(ColorJitterDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_colorjitter_vblur": (C.c_int, [C.POINTER(ColorJitterDesc), c_vp, c_vp, c_vp]),
 }
 
 _lib = None
