@@ -59,7 +59,9 @@ def bilinear_table(in_size, out_size):
         return i, i.copy(), np.zeros(out_size, np.float32)
     scale = np.float32(in_size) / np.float32(out_size)
     d = np.arange(out_size, dtype=np.float32) + np.float32(0.5)
-    src = (np.float64(scale) * np.float64(d) - 0.5).astype(np.float32)      # single rounding (fma)
+    # fma(scale, d, -0.5) with one rounding; astype, not np.float64(d), which turns a one-element array (out_size 1)
+    # into a scalar
+    src = (np.float64(scale) * d.astype(np.float64) - 0.5).astype(np.float32)
     src = np.maximum(src, np.float32(0))
     i0 = np.minimum(np.floor(src).astype(np.int64), in_size - 1)
     l1 = np.clip(src - i0.astype(np.float32), np.float32(0), np.float32(1)).astype(np.float32)

@@ -11,6 +11,10 @@
 //   outside [-1, H] x [-1, W] -> contributes 0;  y <= 0 -> 0;  y_low >= H-1 -> y_low = y_high = H-1, y = y_low
 //   value = w1*v1 + w2*v2 + w3*v3 + w4*v4 summed in sample order (iy outer, ix inner), divided by count
 // all in fp32 (the stored result is rounded once to the plan's storage type).
+// The geometry (roi sizes, bin sizes, grid counts, sample positions) is written with explicitly rounded intrinsics:
+// nvcc would otherwise contract `end * scale - start` and `start + ph * bin` into FMAs, which moves a sample by an
+// ulp - enough to switch it across the -1 / H cutoffs or change ceil(roi / pooled) at a non-power-of-two scale.
+// With the intrinsics the positions, indices and weights are bit-identical to torchvision's fp32 arithmetic.
 #include "pv_common.cuh"
 
 namespace pv {
@@ -26,12 +30,14 @@ roi_align_kernel(const T* __restrict__ x, const float* __restrict__ rois, T* __r
   const int k = bin / (pw_n * ph_n);
   const float* r = rois + (long long)k * 5;
   const int n = (int)__ldg(r);
-  const float roi_start_w = __ldg(r + 1) * spatial_scale, roi_start_h = __ldg(r + 2) * spatial_scale;
-  const float roi_end_w = __ldg(r + 3) * spatial_scale, roi_end_h = __ldg(r + 4) * spatial_scale;
-  const float roi_w = fmaxf(roi_end_w - roi_start_w, 1.f), roi_h = fmaxf(roi_end_h - roi_start_h, 1.f);
-  const float bin_h = roi_h / (float)ph_n, bin_w = roi_w / (float)pw_n;
-  const int grid_h = sampling_ratio > 0 ? sampling_ratio : (int)ceilf(roi_h / (float)ph_n);
-  const int grid_w = sampling_ratio > 0 ? sampling_ratio : (int)ceilf(roi_w / (float)pw_n);
+  const float roi_start_w = __fmul_rn(__ldg(r + 1), spatial_scale), roi_start_h = __fmul_rn(__ldg(r + 2), spatial_scale);
+  const float roi_end_w = __fmul_rn(__ldg(r + 3), spatial_scale), roi_end_h = __fmul_rn(__ldg(r + 4), spatial_scale);
+  const float roi_w = fmaxf(__fsub_rn(roi_end_w, roi_start_w), 1.f), roi_h = fmaxf(__fsub_rn(roi_end_h, roi_start_h), 1.f);
+  const float bin_h = __fdiv_rn(roi_h, (float)ph_n), bin_w = __fdiv_rn(roi_w, (float)pw_n);
+  const int grid_h = sampling_ratio > 0 ? sampling_ratio : (int)ceilf(__fdiv_rn(roi_h, (float)ph_n));
+  const int grid_w = sampling_ratio > 0 ? sampling_ratio : (int)ceilf(__fdiv_rn(roi_w, (float)pw_n));
+  const float start_y = __fadd_rn(roi_start_h, __fmul_rn((float)ph, bin_h));   // torchvision: start + ph * bin
+  const float start_x = __fadd_rn(roi_start_w, __fmul_rn((float)pw, bin_w));
   const float count = (float)max(grid_h * grid_w, 1);
   const bool valid_n = n >= 0 && n < N;
   const T* xn = x + (long long)(valid_n ? n : 0) * H * W * x_row_stride;
@@ -41,9 +47,9 @@ roi_align_kernel(const T* __restrict__ x, const float* __restrict__ rois, T* __r
 #pragma unroll
     for (int i = 0; i < 8; ++i) acc[i] = 0.f;
     for (int iy = 0; iy < grid_h; ++iy) {
-      const float yy0 = roi_start_h + (float)ph * bin_h + ((float)iy + .5f) * bin_h / (float)grid_h;
+      const float yy0 = __fadd_rn(start_y, __fdiv_rn(__fmul_rn((float)iy + .5f, bin_h), (float)grid_h));
       for (int ix = 0; ix < grid_w; ++ix) {
-        const float xx0 = roi_start_w + (float)pw * bin_w + ((float)ix + .5f) * bin_w / (float)grid_w;
+        const float xx0 = __fadd_rn(start_x, __fdiv_rn(__fmul_rn((float)ix + .5f, bin_w), (float)grid_w));
         float yy = yy0, xx = xx0;
         if (!valid_n || yy < -1.f || yy > (float)H || xx < -1.f || xx > (float)W) continue;   // zero weights
         if (yy <= 0.f) yy = 0.f;
@@ -86,12 +92,14 @@ extern "C" int pv_roi_align_fwd(const void* x, int dtype, long long x_row_stride
   const unsigned bins = (unsigned)((long long)K * pooled_h * pooled_w);
   int threads = ((C / 8 + 31) / 32) * 32;
   if (threads > 256) threads = 256;
-  if (dtype == PV_F16)
+  if (dtype == PV_F16) {
     pv::roi_align_kernel<__half><<<bins, threads, 0, s>>>((const __half*)x, rois, (__half*)y, N, H, W, C, x_row_stride,
                                                          y_row_stride, K, pooled_h, pooled_w, spatial_scale, sampling_ratio);
-  else
+    PV_LAUNCH_OK("roi_align_kernel<__half>");
+  } else {
     pv::roi_align_kernel<float><<<bins, threads, 0, s>>>((const float*)x, rois, (float*)y, N, H, W, C, x_row_stride,
                                                         y_row_stride, K, pooled_h, pooled_w, spatial_scale, sampling_ratio);
-  PV_LAUNCH_OK("roi_align_kernel");
+    PV_LAUNCH_OK("roi_align_kernel<float>");
+  }
   return PV_OK;
 }

@@ -275,9 +275,12 @@ extern "C" int pv_clip_transform_fwd(const pv_clip_transform_desc* d, const void
   cudaStream_t s = (cudaStream_t)stream;
   constexpr int PX = 2;
   dim3 grid((unsigned)pv::cdiv(d->out_w, PX * 128), d->out_h, d->C * d->n_t), block(128);
-#define PV_TR(ST, OT)                                                                         \
-  pv::clip_transform_kernel<ST, OT, PX><<<grid, block, 0, s>>>(*d, (const ST*)src, idx_t, y0, y1, ly, \
-                                                              x0, x1, lx, (OT*)dst)
+#define PV_TR(ST, OT)                                                                                     \
+  do {                                                                                                    \
+    pv::clip_transform_kernel<ST, OT, PX><<<grid, block, 0, s>>>(*d, (const ST*)src, idx_t, y0, y1, ly,   \
+                                                                x0, x1, lx, (OT*)dst);                    \
+    PV_LAUNCH_OK("clip_transform_kernel<" #ST "," #OT ">");                                               \
+  } while (0)
   const bool h = d->dst_dtype == PV_F16;
   switch (d->src_dtype) {
     case PV_U8: if (h) PV_TR(uint8_t, __half); else PV_TR(uint8_t, float); break;
@@ -286,7 +289,6 @@ extern "C" int pv_clip_transform_fwd(const pv_clip_transform_desc* d, const void
     default: pv::set_error("src dtype %d unsupported", d->src_dtype); return PV_ERR_INVALID;
   }
 #undef PV_TR
-  PV_LAUNCH_OK("clip_transform_kernel");
   return PV_OK;
 }
 
@@ -294,17 +296,20 @@ extern "C" int pv_clip_transform_fwd(const pv_clip_transform_desc* d, const void
 namespace pv {
 // Test-time ensembling over the views of a video (pytorchvideo_trainer module/video_classification.py:290-311:
 // per-video accumulation of the per-clip predictions, "sum" or "max", then division by the clip count):
-// out[v][k] = reduce_{i < n_views} preds[(v*n_views + i)][k];  mode 0 = sum, 1 = mean, 2 = max.
+// out[v][k] = reduce_{i < n_views} preds[(v*n_views + i)][k];  mode 0 = sum, 1 = mean (sum / n_views), 2 = max.
+// Both accumulators are the reference's: they start from torch.zeros, and "max" folds with torch.max, so it is
+// max(0, max_i p_i) and a NaN in any view propagates (fmaxf would drop it).
 __global__ void view_reduce_kernel(const float* __restrict__ preds, float* __restrict__ out, int n_videos, int n_views,
                                    int K, int mode) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_videos * K) return;
   const int v = i / K, k = i - v * K;
   const float* p = preds + (long long)v * n_views * K + k;
-  float acc = mode == 2 ? -INFINITY : 0.f;
+  float acc = 0.f;
   for (int j = 0; j < n_views; ++j) {
     const float x = p[(long long)j * K];
-    acc = mode == 2 ? fmaxf(acc, x) : acc + x;
+    if (mode != 2) acc = acc + x;
+    else if (acc == acc) acc = (x != x || x > acc) ? x : acc;   // torch.max: NaN wins, else the larger
   }
   out[i] = mode == 1 ? acc / (float)n_views : acc;
 }
@@ -345,14 +350,21 @@ extern "C" int pv_clip_transform_batch(const pv_clip_batch_desc* d, const void* 
   PV_CHECK_ARG((long long)d->C * (d->n_t > d->n_slow ? d->n_t : d->n_slow) * d->out_h * d->out_w < (1ll << 31),
                "output clip too large for 32-bit offsets");
   const bool arith = d->div255 || d->normalize;
+  // LUT instances exist only for a uint8 source with a float destination (the uint8 pass-through has no arithmetic)
+#define PV_TB_LAUNCH(ST, OT, NC, LUT)                                                                                  \
+  do {                                                                                                                 \
+    pv::clip_transform_batch_kernel<ST, OT, NC, LUT><<<grid, block, 0, s>>>(*d, (const ST*)src, idx_t, slow_pos, geom, \
+                                                                           (OT*)dst, (OT*)dst_slow);                   \
+    PV_LAUNCH_OK("clip_transform_batch_kernel<" #ST "," #OT "," #NC "," #LUT ">");                                    \
+  } while (0)
 #define PV_TB(ST, OT, NC)                                                                                              \
   do {                                                                                                                 \
-    if (std::is_same<ST, uint8_t>::value && arith)                                                                     \
-      pv::clip_transform_batch_kernel<ST, OT, NC, std::is_same<ST, uint8_t>::value><<<grid, block, 0, s>>>(            \
-          *d, (const ST*)src, idx_t, slow_pos, geom, (OT*)dst, (OT*)dst_slow);                                         \
-    else                                                                                                               \
-      pv::clip_transform_batch_kernel<ST, OT, NC, false><<<grid, block, 0, s>>>(*d, (const ST*)src, idx_t, slow_pos,   \
-                                                                               geom, (OT*)dst, (OT*)dst_slow);         \
+    if constexpr (std::is_same<ST, uint8_t>::value && !std::is_same<OT, uint8_t>::value) {                             \
+      if (arith) PV_TB_LAUNCH(ST, OT, NC, true);                                                                       \
+      else PV_TB_LAUNCH(ST, OT, NC, false);                                                                            \
+    } else {                                                                                                           \
+      PV_TB_LAUNCH(ST, OT, NC, false);                                                                                 \
+    }                                                                                                                  \
   } while (0)
 #define PV_TBC(ST, OT)                                                          \
   do {                                                                          \
@@ -380,7 +392,7 @@ extern "C" int pv_clip_transform_batch(const pv_clip_batch_desc* d, const void* 
   }
 #undef PV_TBC
 #undef PV_TB
-  PV_LAUNCH_OK("clip_transform_batch_kernel");
+#undef PV_TB_LAUNCH
   return PV_OK;
 }
 

@@ -29,7 +29,12 @@ def clip_start_frames(n_frames, clip_frames, clips_per_video):
 
 def view_reduce(preds, n_views, mode="sum"):
     """[n_videos * n_views, K] f32 CUDA predictions -> [n_videos, K]; mode: "sum" | "mean" | "max"
-    (video_classification.py:303-311; "mean" = the sum divided by the clip count of :279-282)."""
+    (video_classification.py:303-311; "mean" = the sum divided by the clip count of :279-282).
+
+    "sum" and "max" are the reference's per-video accumulators: it starts each video from zeros and adds or
+    torch.max-es the views in order, so "max" is max(0, max_i p_i) and a NaN in any view propagates.  At the end of
+    the test epoch the reference divides either accumulator by the clip count (:279-282); for "max" that division is
+    left to the caller."""
     if preds.device.type != "cuda" or preds.dtype != torch.float32 or preds.dim() != 2 or not preds.is_contiguous():
         raise RuntimeError("view_reduce expects a contiguous f32 CUDA tensor [n_videos * n_views, classes]")
     if preds.shape[0] % n_views:

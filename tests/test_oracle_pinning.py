@@ -69,7 +69,7 @@ def test_uniform_crop_goldens():
 
 def test_bilinear_table_matches_aten():
     import torch.nn.functional as F
-    for (i, o) in [(1080, 256), (1920, 455), (320, 224), (7, 13), (224, 224), (61, 30)]:
+    for (i, o) in [(1080, 256), (1920, 455), (320, 224), (7, 13), (224, 224), (61, 30), (12, 1), (700, 1), (1, 5)]:
         eye = torch.eye(i).view(1, i, 1, i)
         w = F.interpolate(eye, size=(1, o), mode="bilinear", align_corners=False)[0, :, 0, :].numpy()
         i0, i1, l1 = O.bilinear_table(i, o)
