@@ -68,13 +68,19 @@ def apply_chain(video, ops, fill=FILL):
     return video
 
 
-def augmix(video, weights, m, chains, fill=FILL):
-    """mixed = sum_k w_k * chain_k(video) (fp32, chain order), then m * video + (1 - m) * mixed (uint8: truncated)."""
+def mix_chains(video, weights, m, chain_outputs):
+    """AugMix's mix of already augmented chains: mixed = sum_k w_k * chain_k (fp32, chain order), then
+    m * video + (1 - m) * mixed (uint8: truncated)."""
     mixed = torch.zeros(video.shape, dtype=torch.float32)
-    for w, ops in zip(weights, chains):
-        mixed += w * apply_chain(video, ops, fill)
+    for w, out in zip(weights, chain_outputs):
+        mixed += w * out
     out = m * video + (1 - m) * mixed
     return out.type(torch.uint8) if video.dtype == torch.uint8 else out
+
+
+def augmix(video, weights, m, chains, fill=FILL):
+    """mix_chains over chain_k(video), each chain applied in order."""
+    return mix_chains(video, weights, m, [apply_chain(video, ops, fill) for ops in chains])
 
 
 def random_resized_crop(frames, boxes, target_h, target_w):

@@ -173,7 +173,10 @@ augment_apply_kernel(pv_augment_desc d, const T* __restrict__ src, const pv_aug_
       const pv_aug_frame_stats& s = stats[blockIdx.y];
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
-        float lo = s.mn[c], sc = __fdiv_rn(bound, __fsub_rn(s.mx[c], lo));
+        // torchvision's `bound / (maximum - minimum)` is a scalar over a tensor, which torch evaluates as
+        // reciprocal() * bound: two roundings.  One division differs in the last bit for 46 of the 255 uint8 ranges
+        // and then maps the frame's maximum to 255.00002 instead of 254.99998 (255 instead of torchvision's 254).
+        float lo = s.mn[c], sc = __fmul_rn(__frcp_rn(__fsub_rn(s.mx[c], lo)), bound);
         if (!isfinite(sc)) { lo = 0.f; sc = 1.f; }
         const float q = fminf(fmaxf(__fmul_rn(__fsub_rn(v[c], lo), sc), 0.f), bound);
         r[c] = U8 ? (float)(int)q : q;

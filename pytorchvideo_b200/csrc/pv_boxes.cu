@@ -4,7 +4,8 @@
 //
 // One thread owns one box.  Every step repeats the reference's expression with one rounding to the boxes' own type T
 // per operation, as the eager ops store it: the __*_rn intrinsics keep nvcc from contracting the scale and the crop
-// offset into an FMA the CPU does not do.  Clipping is numpy's maximum / minimum (a NaN propagates; max(0, -0) is +0).
+// offset into an FMA the CPU does not do.  Clipping is numpy's maximum / minimum (a NaN propagates; max(0, -0) is +0
+// here, while numpy leaves that zero's sign to its build).
 #include "pv_common.cuh"
 
 namespace pv {
