@@ -660,6 +660,39 @@ int pv_weights_refresh(const long long* gather_jobs, const long long* gather_chu
                        const float* const* srcs, const long long* fold_jobs, int n_fold_jobs, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Bank scans (csrc/pv_bank.cu): fp32 query rows q [N][dim] (row stride q_row_stride) against a dense fp32 bank
+ * [M][dim] with 64-bit offsets.  Similarities are q . m with the dim terms summed in ascending order by fmaf; the
+ * (N, M) matrix is never stored.  Repeated calls are bitwise identical.
+ * pv_bank_workspace : bytes of the device workspace of pv_bank_topk (op 0) or pv_queue_ce (op 1) for N queries, an
+ *                     M-row bank and k neighbours (pass k = 1 for op 1).  Host only.
+ * pv_bank_topk      : ssl_helper.py:288-311 (KnnMemory.eval_knn): per query the k largest similarities, descending,
+ *                     equal similarities by ascending bank index (-0 equals +0, NaN above +inf), into sim_out [N][k]
+ *                     and idx_out [N][k] (int64); then preds [N][n_classes] = sum_i onehot(labels[idx_i]) *
+ *                     exp(sim_i / temperature) in that order, each product and sum rounded once (a weight of +inf
+ *                     makes the other classes NaN, as 0 * inf).  labels: int64 [M]; one outside [0, n_classes) sets
+ *                     *flag (cleared by the call).  1 <= k <= min(1024, M), 1 <= dim <= 2048, M < 2^31.
+ * pv_bank_update    : ssl_helper.py:245-250 (KnnMemory.update): memory[ind[n]] = v / max(|v|, 1e-12) elementwise with
+ *                     v = x[n] * momentum + memory[ind[n]] * one_minus_momentum (two products and a sum, each rounded
+ *                     once), from the rows as they were before the call; of repeated indices the last occurrence
+ *                     wins.  An index outside [0, M) sets *flag (cleared by the call) and nothing is written.
+ * pv_queue_ce       : cross entropy against target 0 (losses.py:125-134), row_loss and with reduce_mean its mean.
+ *                     With logits == NULL, MoCo's objective (moco_v2.py:312-323): keys holds n_views blocks of N rows;
+ *                     for every block v != skip_view (-1: none), in order, row (j, n) has the logits
+ *                     [q_n . key_v,n, q_n . queue_0 .. q_n . queue_K-1] / temperature; the queue part of each query's
+ *                     logsumexp is one streamed pass over queue [K][dim].  With logits != NULL: N materialised rows
+ *                     of L logits, divided by temperature.                                                       */
+int pv_bank_workspace(int op, int N, long long M, int k, long long* bytes);
+int pv_bank_topk(const float* q, long long q_row_stride, int N, const float* memory, long long M, int dim, int k,
+                 const long long* labels, int n_classes, float temperature, void* workspace, long long workspace_bytes,
+                 float* sim_out, long long* idx_out, float* preds, int* flag, void* stream);
+int pv_bank_update(const float* x, long long x_row_stride, int N, const long long* ind, float* memory, long long M,
+                   int dim, float momentum, float one_minus_momentum, int* flag, void* stream);
+int pv_queue_ce(const float* q, long long q_row_stride, int N, int dim, const float* queue, long long K,
+                const float* keys, long long key_row_stride, int n_views, int skip_view, const float* logits,
+                long long logits_row_stride, int L, float temperature, void* workspace, long long workspace_bytes,
+                int reduce_mean, float* row_loss, float* loss, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Contrastive view colour augmentation (pytorchvideo_trainer datamodule/transforms.py ColorJitterVideoSSl): torchvision's
  * PIL ColorJitter, RandomGrayscale and Pillow's GaussianBlur on each clip stacked into one tall (n_t*H, W) RGB image,
  * in Pillow's integer and float arithmetic (blend in C float, RGB<->HSV with its double steps, 16-bit fixed-point luma,

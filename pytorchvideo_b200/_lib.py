@@ -213,6 +213,12 @@ SIGNATURES = {
     "pv_colorjitter_stats": (C.c_int, [C.POINTER(ColorJitterDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_colorjitter_apply": (C.c_int, [C.POINTER(ColorJitterDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_colorjitter_vblur": (C.c_int, [C.POINTER(ColorJitterDesc), c_vp, c_vp, c_vp]),
+    "pv_bank_workspace": (C.c_int, [C.c_int, C.c_int, c_ll, C.c_int, C.POINTER(c_ll)]),
+    "pv_bank_topk": (C.c_int, [c_vp, c_ll, C.c_int, c_vp, c_ll, C.c_int, C.c_int, c_vp, C.c_int, C.c_float, c_vp, c_ll,
+                               c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_bank_update": (C.c_int, [c_vp, c_ll, C.c_int, c_vp, c_vp, c_ll, C.c_int, C.c_float, C.c_float, c_vp, c_vp]),
+    "pv_queue_ce": (C.c_int, [c_vp, c_ll, C.c_int, C.c_int, c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_ll,
+                              C.c_int, C.c_float, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp]),
 }
 
 _lib = None

@@ -944,3 +944,88 @@ def soft_ce_case(name, seed=404):
     else:
         t = torch.randint(0, C, (N,), generator=g)
     return x, t, {"normalize_targets": norm, "reduction": red}
+
+
+# ---- MoCo v2 and the kNN memory (models/moco_v2.py, knn_memory.py; oracle/gen_golden_knn_moco.py) ---------------
+MOCO_CASES = {"moco_linear_v2": 2, "moco_linear_v3": 3, "moco_slow_r50": 2}    # name: views
+MOCO_STEPS = {"moco_linear_v2": 2, "moco_linear_v3": 2, "moco_slow_r50": 1}    # steps (the linear cases wrap the queue)
+MOCO_QUEUE_SEED = 5
+MOCO_STEP_SEED = 7
+
+
+def build_moco_case(name, ns, seed=2718):
+    """(MOCO model, views, queue size k, dim) of a MOCO_CASES entry from ``ns`` (a namespace with MOCO,
+    create_moco_resnet_50, create_mlp_util and create_resnet: this package's or the reference's).  The constructors
+    run under torch.manual_seed(seed); randomize_model then sets the online and the momentum weights apart."""
+    g = torch.Generator().manual_seed(seed + 1)
+    torch.manual_seed(seed)
+    V = MOCO_CASES[name]
+    if name == "moco_slow_r50":
+        m = ns.create_moco_resnet_50(backbone_creator=ns.create_resnet)
+        B, k, dim = 2, 65536, 128
+        views = [torch.rand((B, 3, 8, 224, 224), generator=g) for _ in range(V)]
+    else:
+        def part():
+            return nn.Linear(16, 12), ns.create_mlp_util(12, 8, 32, 3, norm=nn.BatchNorm1d)
+        (b, p), (bm, pm) = part(), part()
+        m = ns.MOCO(mmt=0.5, backbone=b, projector=p, backbone_mmt=bm, projector_mmt=pm)
+        B, k, dim = 4, 16, 8
+        views = [torch.rand((B, 16), generator=g) for _ in range(V)]
+    randomize_model(m.backbone, seed=seed + 2)
+    randomize_model(m.backbone_mmt, seed=seed + 3)
+    return m.eval(), views, k, dim
+
+
+KNN_CASES = {                  # name: (bank rows, dim, k, classes, T, queries)
+    "m1000_d8_k1": (1000, 8, 1, 10, 0.1, 5),
+    "m1000_d100_k20": (1000, 100, 20, 10, 0.1, 5),
+    "m1000_d128_kM": (1000, 128, 1000, 10, 0.1, 5),
+    "k400_n64": (239975, 128, 200, 400, 0.1, 64),
+}
+KNN_UPDATES = {                # name: (bank rows, dim, momentum, batch sizes of the update sequence)
+    "mmt1": (100, 16, 1.0, (8, 8)),
+    "mmt05": (100, 16, 0.5, (8, 8, 8)),
+    "duplicates": (10, 16, 0.5, (5000,)),
+    "n1": (100, 16, 0.5, (1, 1)),
+}
+
+
+def knn_case(name, knn_cls, seed=31):
+    """(KnnMemory on the CPU with its labels, fp32 query rows) of a KNN_CASES entry; the bank is KnnMemory's own draw
+    under torch.manual_seed(seed)."""
+    import types
+    M, dim, k, C, T, N = KNN_CASES[name]
+    torch.manual_seed(seed)
+    knn = knn_cls(M, dim, momentum=1.0, downstream_classes=C, temperature=T, knn_k=k)
+    g = torch.Generator().manual_seed(seed + 1)
+    labels = torch.randint(0, C, (M,), generator=g)
+    loader = types.SimpleNamespace(dataset=types.SimpleNamespace(
+        _labeled_videos=[(i, {"label": int(v)}) for i, v in enumerate(labels.tolist())]))
+    knn.init_knn_labels(loader)
+    q = torch.randn((N, dim), generator=g)
+    return knn, q / q.norm(dim=1, keepdim=True)
+
+
+def knn_overflow_case(knn_cls, seed=41):
+    """The trainer's overflow: update(momentum 1.0) stores +-1 rows; a unit query whose L1 norm exceeds 8.87 finds its
+    own sign row with exp(s / 0.1) = inf.  (KnnMemory after the update, queries, the update's rows and indices)."""
+    import types
+    M, dim, C = 1000, 128, 10
+    torch.manual_seed(seed)
+    knn = knn_cls(M, dim, momentum=1.0, downstream_classes=C, temperature=0.1, knn_k=20)
+    g = torch.Generator().manual_seed(seed + 1)
+    labels = torch.randint(0, C, (M,), generator=g)
+    loader = types.SimpleNamespace(dataset=types.SimpleNamespace(
+        _labeled_videos=[(i, {"label": int(v)}) for i, v in enumerate(labels.tolist())]))
+    knn.init_knn_labels(loader)
+    x = torch.randn((M, dim), generator=g)
+    ind = torch.arange(M)
+    q = x[:4] / x[:4].norm(dim=1, keepdim=True)
+    return knn, q, x, ind
+
+
+def knn_update_inputs(name, seed=51):
+    """[(rows, indices)] of a KNN_UPDATES sequence (repeated indices included)."""
+    M, dim, _, sizes = KNN_UPDATES[name]
+    g = torch.Generator().manual_seed(seed)
+    return [(torch.randn((n, dim), generator=g) * 0.1, torch.randint(0, M, (n,), generator=g)) for n in sizes]
