@@ -229,7 +229,7 @@ int attention_mma_launch(const pv_attention_desc* d, const void* q, const void* 
 #define PV_AM(DD) \
   case DD: return launch_attention_mma<DD>(d, q, k, v, o, s, "attention_mma_kernel<" #DD ">");
   switch (d->D) {
-    PV_AM(32) PV_AM(64) PV_AM(96) PV_AM(128)
+    PV_AM(128)
     default: set_error("internal: mma attention head dim %d", d->D); return PV_ERR_INVALID;
   }
 #undef PV_AM

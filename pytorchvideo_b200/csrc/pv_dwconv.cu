@@ -379,14 +379,12 @@ extern "C" int pv_dwconv3d_fwd(const pv_conv3d_desc* d, const void* x, const voi
   if (rc != PV_OK) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   if (!getenv("PVB200_DW_SIMT")) {
-    if (!getenv("PVB200_DW_NO_LANE")) {      // 3x3x3: lane-per-channel-pair register stencil (pv_dwlane.cu)
-      rc = pv::dwconv3d_lane_launch(d, x, w, scale, bias, y, se_sums, s);
-      if (rc != PV_ERR_UNSUPPORTED) return rc;
-    }
-    if (!getenv("PVB200_DW_NO_TEMPORAL")) {  // kt x 1 x 1: streaming register window
-      rc = pv::dwconv3d_temporal_launch(d, x, w, scale, bias, y, se_sums, s);
-      if (rc != PV_ERR_UNSUPPORTED) return rc;
-    }
+    // 3x3x3: lane-per-channel-pair register stencil (pv_dwlane.cu)
+    rc = pv::dwconv3d_lane_launch(d, x, w, scale, bias, y, se_sums, s);
+    if (rc != PV_ERR_UNSUPPORTED) return rc;
+    // kt x 1 x 1: streaming register window
+    rc = pv::dwconv3d_temporal_launch(d, x, w, scale, bias, y, se_sums, s);
+    if (rc != PV_ERR_UNSUPPORTED) return rc;
     rc = pv::dwconv3d_tile_launch(d, x, w, scale, bias, y, se_sums, s);
     if (rc != PV_ERR_UNSUPPORTED) return rc;
   }

@@ -17,7 +17,6 @@
 // convs (layers/attention.py:364-403).
 #include "pv_common.cuh"
 #include "pv_sm90.cuh"
-#include <stdlib.h>
 #include <string.h>
 
 namespace pv {
@@ -47,22 +46,20 @@ struct DwLaneParams {
 };
 
 
-// the two channels of a lane (Hopper has no packed fp32 FMA: two rounded FMAs, same results)
-__device__ __forceinline__ float2 fma_x2(float2 a, float2 b, float2 c) {
-  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
-}
+// Four warps and at most 50 KB of halo per CTA: four CTAs per SM, whose TMA waits stagger.
+constexpr int DWL_WARPS = 4;
+constexpr int DWL_SMEM_BUDGET = 50 * 1024;
 
-// NW warps per CTA: 8 (two 100 KB CTAs per SM) or 4 (four 50 KB CTAs per SM - more CTAs to stagger the TMA waits).
 // PRE: the pre-activation prologue runs once over the landed halo box (in-bounds positions only), before the stencil.
-template <int S, int PH, int PW, bool X2, int NW, bool PRE>
-__global__ void __launch_bounds__(NW * 32, 16 / NW)
+template <int S, int PH, int PW, bool PRE>
+__global__ void __launch_bounds__(DWL_WARPS * 32, 16 / DWL_WARPS)
 dwconv3d_lane_kernel(const __grid_constant__ DwLaneParams P, const __half* __restrict__ w,
                      const float* __restrict__ scale, const float* __restrict__ bias,
                      __half* __restrict__ y, float* __restrict__ se_sums) {
   constexpr int IH = (PH - 1) * S + 3, IW = (PW - 1) * S + 3;
   extern __shared__ __align__(128) uint8_t dwl_smem[];
   __shared__ __align__(8) uint64_t bar;
-  __shared__ float2 se_part[NW][32];
+  __shared__ float2 se_part[DWL_WARPS][32];
   const __half* xs = reinterpret_cast<const __half*>(dwl_smem);          // [tt][hh][ww][cc]
   const int cc = P.cc;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -104,7 +101,7 @@ dwconv3d_lane_kernel(const __grid_constant__ DwLaneParams P, const __half* __res
   const int total = P.bt * nph * npw;
   const int row_e = P.ww * cc;                       // elements per halo row
   float2 se = make_float2(0.f, 0.f);
-  for (int p = warp; p < total; p += NW) {
+  for (int p = warp; p < total; p += DWL_WARPS) {
     const int pwi = p % npw;
     const int r = p / npw;
     const int phi = r % nph, t = r / nph;
@@ -131,12 +128,8 @@ dwconv3d_lane_kernel(const __grid_constant__ DwLaneParams P, const __half* __res
               if (j - kw < 0 || (j - kw) % S != 0 || (j - kw) / S >= PW) continue;
               float2& a = acc[(i - kh) / S][(j - kw) / S];
               const float2 wv = wr[(kt * 3 + kh) * 3 + kw];
-              if constexpr (X2) {
-                a = fma_x2(xv, wv, a);
-              } else {
-                a.x = fmaf(xv.x, wv.x, a.x);
-                a.y = fmaf(xv.y, wv.y, a.y);
-              }
+              a.x = fmaf(xv.x, wv.x, a.x);     // the lane's two channels: Hopper has no packed fp32 FMA
+              a.y = fmaf(xv.y, wv.y, a.y);
             }
           }
         }
@@ -174,7 +167,7 @@ dwconv3d_lane_kernel(const __grid_constant__ DwLaneParams P, const __half* __res
     if (warp == 0 && live) {
       float2 tot = make_float2(0.f, 0.f);
 #pragma unroll
-      for (int k = 0; k < NW; ++k) { tot.x += se_part[k][lane].x; tot.y += se_part[k][lane].y; }
+      for (int k = 0; k < DWL_WARPS; ++k) { tot.x += se_part[k][lane].x; tot.y += se_part[k][lane].y; }
       se_sum_add(se_sums, (long long)n * P.C + ch, tot.x);
       se_sum_add(se_sums, (long long)n * P.C + ch + 1, tot.y);
     }
@@ -207,9 +200,8 @@ int dwconv3d_lane_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   // patch shape: 4x4 unless the plane is a multiple of 7 wide but not of 4 (14x14, 7x7 planes): 2x7
   const bool p27 = (d->Wo % 4 != 0) && (d->Wo % 7 == 0);
   const int PH = p27 ? 2 : 4, PW = p27 ? 7 : 4;
-  static const int nw = [] { const char* e = getenv("PVB200_DW_WARPS"); return (e && e[0] == '8') ? 8 : 4; }();
-  // ---- output box: maximise useful outputs per halo byte under a budget that keeps 16 / nw CTAs per SM
-  const int budget = (nw == 8 ? 100 : 50) * 1024;
+  // ---- output box: maximise useful outputs per halo byte under a budget that keeps 16 / DWL_WARPS CTAs per SM
+  constexpr int nw = DWL_WARPS;
   double best = -1;
   for (int bw = PW; bw <= 56; bw += PW) {
     if (bw - PW >= d->Wo) break;
@@ -220,7 +212,7 @@ int dwconv3d_lane_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
         const int ww = (bw - 1) * S + 3, hh = (bh - 1) * S + 3, tt = (bt - 1) * d->st + 3;
         if (ww > 256 || hh > 256 || tt > 256) continue;
         const long long halo = (long long)tt * hh * ww * P.cc * 2;
-        if (halo > budget) continue;
+        if (halo > DWL_SMEM_BUDGET) continue;
         const int patches = bt * (bh / PH) * (bw / PW);
         const double warp_eff = (double)patches / (double)(((patches + nw - 1) / nw) * nw);
         const double cov_w = (double)d->Wo / (((d->Wo + bw - 1) / bw) * bw);
@@ -250,23 +242,17 @@ int dwconv3d_lane_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
     if (cr != CUDA_SUCCESS) return PV_ERR_UNSUPPORTED;
   }
   const size_t smem = (size_t)P.tt * P.hh * P.ww * P.cc * 2 + 256;
-  dim3 grid((unsigned)tiles, (unsigned)chunks), block(nw * 32);
-  static const bool x2 = [] { const char* e = getenv("PVB200_DW_X2"); return !(e && e[0] == '0'); }();
-#define PV_DWL3(S_, PH_, PW_, X2_, NW_, PRE_)                                                                  \
+  dim3 grid((unsigned)tiles, (unsigned)chunks), block(DWL_WARPS * 32);
+#define PV_DWL2(S_, PH_, PW_, PRE_)                                                                            \
   do {                                                                                                        \
-    PV_OPT_IN_SMEM((dwconv3d_lane_kernel<S_, PH_, PW_, X2_, NW_, PRE_>), 110 * 1024);                         \
-    dwconv3d_lane_kernel<S_, PH_, PW_, X2_, NW_, PRE_><<<grid, block, smem, stream>>>(P, (const __half*)w,     \
-                                                                  scale, bias, (__half*)y, se_sums);          \
-    PV_LAUNCH_OK(PV_PRE_NAME("dwconv3d_lane_kernel<" #S_ "," #PH_ "," #PW_ "," #X2_ "," #NW_, PRE_));         \
-  } while (0)
-#define PV_DWL2(S_, PH_, PW_, X2_, NW_)                                                                       \
-  do {                                                                                                        \
-    if (pre) PV_DWL3(S_, PH_, PW_, X2_, NW_, true); else PV_DWL3(S_, PH_, PW_, X2_, NW_, false);              \
+    PV_OPT_IN_SMEM((dwconv3d_lane_kernel<S_, PH_, PW_, PRE_>), 110 * 1024);                                   \
+    dwconv3d_lane_kernel<S_, PH_, PW_, PRE_><<<grid, block, smem, stream>>>(P, (const __half*)w, scale, bias, \
+                                                                           (__half*)y, se_sums);             \
+    PV_LAUNCH_OK(PV_PRE_NAME("dwconv3d_lane_kernel<" #S_ "," #PH_ "," #PW_, PRE_));                           \
   } while (0)
 #define PV_DWL(S_, PH_, PW_)                                                                                  \
   do {                                                                                                        \
-    if (nw == 8) { if (x2) PV_DWL2(S_, PH_, PW_, true, 8); else PV_DWL2(S_, PH_, PW_, false, 8); }            \
-    else { if (x2) PV_DWL2(S_, PH_, PW_, true, 4); else PV_DWL2(S_, PH_, PW_, false, 4); }                    \
+    if (pre) PV_DWL2(S_, PH_, PW_, true); else PV_DWL2(S_, PH_, PW_, false);                                  \
   } while (0)
   if (S == 1 && !p27) PV_DWL(1, 4, 4);
   else if (S == 1) PV_DWL(1, 2, 7);
@@ -274,7 +260,6 @@ int dwconv3d_lane_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   else PV_DWL(2, 2, 7);
 #undef PV_DWL
 #undef PV_DWL2
-#undef PV_DWL3
   return PV_OK;
 }
 

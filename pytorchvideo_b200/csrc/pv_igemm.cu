@@ -277,8 +277,7 @@ static bool window_mode(const pv_conv3d_desc* d) { return d->x_w_pad > 0 && d->C
 // barrier rounds and no SM instructions for the A operand, which beats the cp.async gather for these
 // widths (the gather kernel keeps C_in = 4 / 8 / 24 / 40 / 48 / 56).
 bool conv3d_tma_narrow(const pv_conv3d_desc* d) {
-  static const bool off = getenv("PVB200_GATHER_ALL") != nullptr;
-  return !off && !window_mode(d) && (d->Ci == 16 || d->Ci == 32) && d->ci_pad64 == d->Ci;
+  return !window_mode(d) && (d->Ci == 16 || d->Ci == 32) && d->ci_pad64 == d->Ci;
 }
 // TMA needs a 16-byte aligned base: if the first tap of output column 0 sits at an odd pixel of a
 // 4-channel row, the window starts one pixel earlier (the packed weights carry a zero pixel there).

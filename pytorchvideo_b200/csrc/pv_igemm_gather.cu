@@ -41,7 +41,6 @@ struct GatherParams {
   long long M;
   int m_tiles, n_tiles, block_n, Co, stages;
   int nprod;   // active producer warps, <= stages (see the slot-ownership note in the kernel)
-  int depth;   // k-blocks of cp.async a producer warp keeps in flight: 2 when it owns >= 2 slots, else 1
   EpiParams epi;
   int unit_off[GG_MAX_UNITS];        // element offset of the unit relative to the row's (t0,h0,w0) corner
   unsigned int unit_d[GG_MAX_UNITS];  // packed (dt | dh<<8 | dw<<16) tap displacement (dilation applied)
@@ -120,10 +119,6 @@ conv3d_igemm_gather_kernel(const __grid_constant__ GatherParams P, const __half*
     // fill, g - nprod, already waited for g - nprod - stages >= g - 2 stages (nprod <= stages) to be released, and
     // the consumers release in order.
     // ncu source view: the producers wait on their own cp.async data and on the empty barrier about equally.
-    // Optional depth 2 (PVB200_GATHER_DEPTH2): with >= 2 slots per warp a k-block is published one iteration
-    // later (cp.async groups), i.e. two k-blocks of copies in flight per warp - measured no faster, off by default.
-    const bool deep = P.depth >= 2;
-    int pending = -1;                // stage whose copies were issued last iteration and are not yet published
     for (int g = wprod; wprod < P.nprod && g < total_g; g += P.nprod) {
       const int tile_seq = g / P.num_kb;
       const int kb = g - tile_seq * P.num_kb;
@@ -210,27 +205,10 @@ conv3d_igemm_gather_kernel(const __grid_constant__ GatherParams P, const __half*
         }
       }
       asm volatile("cp.async.commit_group;" ::: "memory");
-      if (deep) {
-        if (pending >= 0) {
-          asm volatile("cp.async.wait_group 1;" ::: "memory");     // everything but the group just committed has landed
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (elect_one()) mbar_arrive(full_bar(pending));
-          __syncwarp();
-        }
-        pending = stage;
-      } else {
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (elect_one()) mbar_arrive(full_bar(stage));
-      }
-    }
-    if (pending >= 0) {
       asm volatile("cp.async.wait_group 0;" ::: "memory");
       fence_proxy_async_smem();
       __syncwarp();
-      if (elect_one()) mbar_arrive(full_bar(pending));
+      if (elect_one()) mbar_arrive(full_bar(stage));
     }
   } else if (warp < GG_CONS_WARPS) {
     // ================================ consumers: wgmma + epilogue ===========================
@@ -360,11 +338,8 @@ int conv3d_gather_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
     int st = (227 * 1024 - 2048 - 2048 /*static tables*/ - epi_smem_bytes(P.epi.nbuf) - 512) / stage_bytes;
     if (st > 16) st = 16;
     if (st < 2) { set_error("gather: not enough smem stages"); return PV_ERR_UNSUPPORTED; }
-    static const bool shallow = getenv("PVB200_GATHER_DEPTH2") == nullptr;   // opt-in only
     P.nprod = st < GG_PROD_WARPS ? st : GG_PROD_WARPS;
     P.stages = st;
-    // two k-blocks of copies in flight per warp need two slots per warp
-    P.depth = (!shallow && P.stages >= 2 * P.nprod) ? 2 : 1;
   }
   const size_t smem_bytes = (size_t)P.stages * stage_bytes + 2048 + epi_smem_bytes(P.epi.nbuf) + 8 * (2 * P.stages) + 16;
   for (int pass = 0; pass < 2; ++pass) {     // output / residual as [Co, M, 1, 1, 1]
@@ -394,8 +369,7 @@ int conv3d_gather_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
   if (total_tiles == 0) return PV_OK;
   const int grid = (int)(total_tiles < sm_count ? total_tiles : sm_count);
   {
-    // launched with the programmatic-stream-serialization attribute (PDL); PVB200_NO_PDL=1 falls back to a plain launch
-    static const bool use_pdl = getenv("PVB200_NO_PDL") == nullptr;
+    // launched with the programmatic-stream-serialization attribute (PDL)
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3((unsigned)grid);
@@ -406,7 +380,7 @@ int conv3d_gather_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = use_pdl ? 1 : 0;
+    cfg.numAttrs = 1;
     const __half* xh = (const __half*)x;
 #define PV_GG_LAUNCH(BN)                                                                                 \
   PV_OPT_IN_SMEM(conv3d_igemm_gather_kernel<BN>, 225 * 1024);                                            \

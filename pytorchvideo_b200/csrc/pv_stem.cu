@@ -276,7 +276,6 @@ extern "C" int pv_conv3d_stem_rows_fwd(const pv_conv3d_desc* d, const void* x, c
   PV_CHECK_ARG(total_tiles < (1ll << 31), "too many tiles");
   const int grid = (int)(total_tiles < sm_count ? total_tiles : sm_count);
   {
-    static const bool use_pdl = getenv("PVB200_NO_PDL") == nullptr;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3((unsigned)grid);
@@ -287,7 +286,7 @@ extern "C" int pv_conv3d_stem_rows_fwd(const pv_conv3d_desc* d, const void* x, c
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = use_pdl ? 1 : 0;
+    cfg.numAttrs = 1;
     const unsigned char *xb = (const unsigned char*)x, *wb = (const unsigned char*)w, *zb = (const unsigned char*)zero_row;
 #define PV_ST_LAUNCH(BN, KS)                                                                              \
   if (block_n == BN && P.win == 16 * KS) {                                                                \

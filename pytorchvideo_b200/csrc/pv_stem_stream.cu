@@ -317,7 +317,6 @@ extern "C" int pv_conv3d_stem_stream_fwd(const pv_conv3d_desc* d, const void* x,
   if (units == 0) return PV_OK;
   PV_CHECK_ARG(units * d->To < (1ll << 31), "too many tiles");
   const int grid = (int)(units < sm_count ? units : sm_count);
-  static const bool use_pdl = getenv("PVB200_NO_PDL") == nullptr;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)grid);
@@ -328,7 +327,7 @@ extern "C" int pv_conv3d_stem_stream_fwd(const pv_conv3d_desc* d, const void* x,
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = use_pdl ? 1 : 0;
+  cfg.numAttrs = 1;
   const unsigned char *xb = (const unsigned char*)x, *wb = (const unsigned char*)w, *zb = (const unsigned char*)zero_row;
   const char* name = nullptr;
 #define PV_SS_LAUNCH(KT, KS)                                                                              \

@@ -115,8 +115,8 @@ class Plan:
         self.sched = None
         self.multi_lane = os.environ.get("PVB200_LANES", "1") != "0"
         # f16 engine, MViT: the residual token stream (16 blocks x 2 adds) is kept in fp32 - branch outputs stay f16, the
-        # add + LayerNorm is one kernel (pv_add_layernorm).  PVB200_TRUNK32=0 restores the all-f16 stream (A/B only).
-        self.trunk32 = dt == L.PV_F16 and os.environ.get("PVB200_TRUNK32", "1") != "0"
+        # add + LayerNorm is one kernel (pv_add_layernorm).
+        self.trunk32 = dt == L.PV_F16
         self._streams = {}
         self._events = {}
 
@@ -393,9 +393,7 @@ class Plan:
         #      tap's partial rounded to f16 and written out) + the temporal tap sum.  Only below 16 output channels:
         #      from there the direct convolution is already a full wgmma width and writes no kt-fold intermediate
         #      (CSN's 3x7x7 3->64 stem at batch 8: 0.96 ms direct, 2.10 ms factored, DESIGN.md).
-        #      PVB200_NO_STEMFACTOR: the direct stem-rows convolution for every shape, for A/B runs.
-        if (stem_candidate and co_pad < 16 and co_pad * kt <= 256 and (sw * x.Cp * 2) % 16 == 0 and kw * x.Cp <= 64 and sh <= 8
-                and not os.environ.get("PVB200_NO_STEMFACTOR")):
+        if stem_candidate and co_pad < 16 and co_pad * kt <= 256 and (sw * x.Cp * 2) % 16 == 0 and kw * x.Cp <= 64 and sh <= 8:
             w2 = torch.zeros(kt * co_pad, cig, 1, kh, kw, dtype=weight.dtype)
             wsrc = weight.detach().cpu()
             for j in range(kt):
@@ -462,8 +460,7 @@ class Plan:
                 want_tc = force_algo == L.ALGO_TCGEN05
             if window and not want_tc:
                 raise RuntimeError("internal: window-mode stem rejected by the library: " + L.last_error())
-            stem_rows = (window and want_tc and residual is None and not os.environ.get("PVB200_NO_STEMROWS")
-                         and bool(self.lib.pv_conv3d_stem_rows_supported(C.byref(d))))
+            stem_rows = window and want_tc and residual is None and bool(self.lib.pv_conv3d_stem_rows_supported(C.byref(d)))
             if stem_rows:
                 # zero-copy im2col over raw input rows (csrc/pv_stem.cu): its own weight layout and entry point
                 algo, kind = L.ALGO_TCGEN05, "tcgen05"

@@ -122,8 +122,8 @@ def test_batchnorm_pools_run_prologue_instances(gold, case):
 MVIT_B_16X4_LEDGER = {
     "add_layernorm_kernel": 33, "add_pos_cls_kernel": 1, "attention_wgmma_kernel<96>": 16,
     "conv3d_igemm_kernel<128,128>": 42, "conv3d_igemm_kernel<128,64>": 1, "conv3d_igemm_kernel<64,128>": 26,
-    "copy_rows_kernel": 3, "dwconv3d_kernel<__half>": 3, "dwconv3d_lane_kernel<1,2,7,true,4>": 2,
-    "dwconv3d_lane_kernel<2,2,7,true,4>": 13, "dwconv3d_lane_kernel<2,4,4,true,4>": 1, "head_reduce_kernel": 1,
+    "copy_rows_kernel": 3, "dwconv3d_kernel<__half>": 3, "dwconv3d_lane_kernel<1,2,7>": 2,
+    "dwconv3d_lane_kernel<2,2,7>": 13, "dwconv3d_lane_kernel<2,4,4>": 1, "head_reduce_kernel": 1,
     "layernorm_reg_kernel": 19, "ncdhw_f32_to_ndhwc4_padw_kernel": 1, "pool3d_kernel": 3,
 }
 

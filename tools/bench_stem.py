@@ -1,13 +1,13 @@
-"""Temporal stems on the H100: the streaming kernel, the factored route and the direct stem-rows kernel, per shape.
+"""Temporal stems on the H100: the streaming kernel and the factored route, per shape.
 
     python tools/bench_stem.py [--launches 50] [--rounds 7] [--out DIR]
 
-Each route of one stem shape is built in one process (the routing switches PVB200_NO_STEMSTREAM / PVB200_NO_STEMFACTOR
-are toggled between plan builds; the stream route is also taken below its one-wave threshold), its launches are captured `launches` times into a CUDA graph, and the routes' graphs
-are replayed alternately for `rounds` rounds, timed with CUDA events; the median per launch is reported.  Shapes: the
-SlowFast Fast stem (5x7x7, 3 -> 8) at batch 1, 2 and 8, and the CSN stem (3x7x7, 3 -> 64) at batch 8, on 32 frames of
-224^2.  Prints the card name, power limit and max SM clock, then per route: us, GB/s of the algorithmic bytes (input
-+ output + weights, f16) and the kernels launched.  Writes JSON to DIR/bench_stem.json when --out is given.
+Each route of one stem shape is built in one process (the routing switch PVB200_NO_STEMSTREAM is toggled between plan
+builds; the stream route is also taken below its one-wave threshold), its launches are captured `launches` times into a
+CUDA graph, and the routes' graphs are replayed alternately for `rounds` rounds, timed with CUDA events; the median per
+launch is reported.  Shapes: the SlowFast Fast stem (5x7x7, 3 -> 8) at batch 1, 2 and 8, on 32 frames of 224^2.
+Prints the card name, power limit and max SM clock, then per route: us, GB/s of the algorithmic bytes (input + output
++ weights, f16) and the kernels launched.  Writes JSON to DIR/bench_stem.json when --out is given.
 """
 import argparse
 import json
@@ -32,12 +32,10 @@ SHAPES = {
     "fast_stem_b1": (1, 8, (5, 7, 7), (1, 2, 2), (2, 3, 3)),
     "fast_stem_b2": (2, 8, (5, 7, 7), (1, 2, 2), (2, 3, 3)),
     "fast_stem_b8": (8, 8, (5, 7, 7), (1, 2, 2), (2, 3, 3)),
-    "csn_stem_b8": (8, 64, (3, 7, 7), (1, 2, 2), (1, 3, 3)),
 }
 ROUTES = {   # route: routing switches set while the plan is built
     "stream": {},
     "factored": {"PVB200_NO_STEMSTREAM": "1"},
-    "direct": {"PVB200_NO_STEMSTREAM": "1", "PVB200_NO_STEMFACTOR": "1"},
 }
 T, HW = 32, 224
 
@@ -56,7 +54,7 @@ def build(shape, route, x, w, launches, dev, stream):
     """(graph of `launches` x the route's conv launches, op names, kernels launched by one run) or None when the route
     does not apply to the shape (the stream kernel below its threshold or outside its scope)."""
     _, co, k, s, p = shape
-    saved = {key: os.environ.pop(key, None) for key in ("PVB200_NO_STEMSTREAM", "PVB200_NO_STEMFACTOR")}
+    saved = os.environ.pop("PVB200_NO_STEMSTREAM", None)
     os.environ.update(ROUTES[route])
     threshold = PL.H100_SXM_SMS
     PL.H100_SXM_SMS = 1          # the stream route at every batch, below its routing threshold too (the crossover)
@@ -66,12 +64,12 @@ def build(shape, route, x, w, launches, dev, stream):
         plan.emit_conv(xr, w, None, None, s, p, (1, 1, 1), 1, L.ACT_RELU, None, "stem")
     finally:
         PL.H100_SXM_SMS = threshold
-        for key in ROUTES["direct"]:
-            os.environ.pop(key, None)
-        os.environ.update({key: v for key, v in saved.items() if v is not None})
+        os.environ.pop("PVB200_NO_STEMSTREAM", None)
+        if saved is not None:
+            os.environ["PVB200_NO_STEMSTREAM"] = saved
     conv_ops = [(n, fn) for n, fn in plan.ops if n.startswith("stem")]
     names = [n for n, _ in conv_ops]
-    if (route == "stream") != (plan.stats.get("stem_stream") == 1) or (route == "direct") != (names == ["stem"]):
+    if (route == "stream") != (plan.stats.get("stem_stream") == 1) or names == ["stem"]:
         return None
     plan.finalize()
     with torch.cuda.stream(stream):
