@@ -97,6 +97,10 @@ class Plan:
         self.use_tcgen05 = bool(use_tcgen05) and dt == L.PV_F16
         self.ops = []          # (name, closure(stream_ptr))
         self.meta = []         # per-op {name, kind, flops, bytes} (algorithmic figures for the roofline)
+        # per op: what it computes, in torch terms ({"kind": "conv", "x": TRef, "weight": ..., "y": TRef, ...}), or None
+        # for an op that produces no value of its own (the SE-sum clear).  Tensors are TRefs, resolved when read, since
+        # concat_channels retargets them after their producer was emitted.  Kept out of meta, which is dumped as JSON.
+        self.op_spec = []
         self.attention_calls = []   # per attention op: its problem (B, H, Nq, Nk, D, scale, normalize, residual)
         self.side_outputs = []      # (weakref to module, Buf, shape): per-module results besides the output (attention weights)
         self.bufs = []
@@ -202,10 +206,11 @@ class Plan:
         return sum(b.numel * _ESIZE[b.dt] for b in self.bufs)
 
     # ---- execution -----------------------------------------------------------------------
-    def add(self, name, fn, kind="other", flops=0.0, nbytes=0.0, reads=None, writes=None):
+    def add(self, name, fn, kind="other", flops=0.0, nbytes=0.0, reads=None, writes=None, spec=None):
         """reads / writes: the TRefs (or Bufs) the launch touches; leave both None for "unknown" (the op then
-        orders against everything on the other lanes)."""
+        orders against everything on the other lanes).  spec: the op_spec record of the launch."""
         self.ops.append((name, fn))
+        self.op_spec.append(spec)
         self.meta.append({"name": name, "kind": kind, "flops": float(flops), "bytes": float(nbytes), "lane": self.lane})
         self.stats[kind] = self.stats.get(kind, 0) + 1
         self.op_lane.append(self.lane)
@@ -304,7 +309,7 @@ class Plan:
                 L.check(lib.pv_ncdhw_to_ndhwc_padw(src.data_ptr(), src_dt, x.ptr(), x.dt, N, C, T, H, W, x.Cp,
                                                   w_pad, w_phys, stream), "pv_ncdhw_to_ndhwc_padw")
             self.add("ncdhw_to_ndhwc_padw", fn, "other", 0.0, src.numel() * src.element_size() + N * T * H * w_phys * x.Cp * 2,
-                     reads=(), writes=(x,))
+                     reads=(), writes=(x,), spec={"kind": "to_ndhwc", "src": src, "y": x})
         else:
             x.buf = self.new_buf(N * T * H * W * x.Cp)
 
@@ -312,7 +317,7 @@ class Plan:
                 L.check(lib.pv_ncdhw_to_ndhwc(src.data_ptr(), src_dt, x.ptr(), x.dt, N, C, T, H, W, x.Cp,
                                               x.row_stride, stream), "pv_ncdhw_to_ndhwc")
             self.add("ncdhw_to_ndhwc", fn, "other", 0.0, src.numel() * src.element_size() + N * T * H * W * x.Cp * 2,
-                     reads=(), writes=(x,))
+                     reads=(), writes=(x,), spec={"kind": "to_ndhwc", "src": src, "y": x})
         return x
 
     def emit_conv(self, x, weight, conv_bias, bn, stride, padding, dilation, groups, act=L.ACT_NONE,
@@ -505,9 +510,12 @@ class Plan:
                                       y.ptr(), stream), "pv_conv3d_fwd(%s)" % name)
         if stem_rows:
             self.stats["stem_rows"] = self.stats.get("stem_rows", 0) + 1
+        spec = {"kind": "conv", "route": kind, "x": x, "weight": weight, "scale": scale[:co], "bias": bias[:co],
+                "stride": tuple(stride), "padding": tuple(padding), "dilation": tuple(dilation), "groups": groups,
+                "act": act, "residual": residual, "addend": addend, "y": y, "se_sums": sums}
         self.add(name, fn_stem if stem_rows else (fn_dw if (depthwise and residual is None) else fn), kind, flops, nbytes,
                  reads=(x,) + ((residual,) if residual is not None else ()) + ((a,) if addend is not None else ()),
-                 writes=(y,) + ((sums,) if sums is not None else ()))
+                 writes=(y,) + ((sums,) if sums is not None else ()), spec=spec)
         if addend is not None:
             self.meta[-1]["addend"] = (a.buf, a_off)
         return y
@@ -537,7 +545,9 @@ class Plan:
                                             scale_d.data_ptr(), bias_d.data_ptr(), act, yk.row_stride,
                                             y.row_stride, stream), "pv_temporal_tap_sum(%s)" % name)
         self.add(name + ".tapsum", fn_sum, "other", 0.0, (yk.N * Ti * hw * kt * co_pad + yk.N * To * hw * co_pad) * 2,
-                 reads=(yk,), writes=(y,))
+                 reads=(yk,), writes=(y,),
+                 spec={"kind": "tap_sum", "x": yk, "y": y, "kt": kt, "st": st, "pt": pt, "dil": dlt, "scale": scale[:co],
+                       "bias": bias[:co], "act": act})
         return y
 
     def _emit_stem_stream(self, x, d, weight, co, lead, name, flops, nbytes):
@@ -557,7 +567,11 @@ class Plan:
                                                   bias_d.data_ptr(), zero_row.data_ptr(), y.ptr(), stream),
                     "pv_conv3d_stem_stream_fwd(%s)" % name)
         self.stats["stem_stream"] = self.stats.get("stem_stream", 0) + 1
-        self.add(name, fn, "tcgen05", flops, nbytes, reads=(x,), writes=(y,))
+        self.add(name, fn, "tcgen05", flops, nbytes, reads=(x,), writes=(y,),
+                 spec={"kind": "conv", "route": "stem_stream", "x": x, "weight": weight, "scale": scale[:co],
+                       "bias": bias[:co], "stride": (d.st, d.sh, d.sw), "padding": (d.pt, d.ph, d.pw),
+                       "dilation": (d.dt, d.dh, d.dw), "groups": 1, "act": L.ACT_NONE, "residual": None, "addend": None,
+                       "y": y, "se_sums": None})
         return y
 
     def _conv_desc(self, x, out_thw, co_pad, kernel, stride, padding, dilation, groups, act, residual, y_row_stride,
@@ -600,10 +614,13 @@ class Plan:
         wb = self.const(PK.pack_rows_k16(conv_b.weight, d.Cmid, d.Cmid))
         wc = self.const(PK.pack_rows_k16(conv_c.weight, d.Cmid, d.Cout))
         ws = self.const(PK.pack_rows_k16(sc_conv.weight, x.Cp, d.Cout)) if sc_conv is not None else None
-        sa, ba = (self.const(t) for t in PK.fold_bn(conv_a.bias, bn_a, cmid, d.Cmid))
-        sbb, bbb = (self.const(t) for t in PK.fold_bn(conv_b.bias, bn_b, cmid, d.Cmid))
-        scc, bcc = (self.const(t) for t in PK.fold_bn(conv_c.bias, bn_c, cout, d.Cout))
-        ss, bs = (self.const(t) for t in PK.fold_bn(sc_conv.bias, sc_bn, cout, d.Cout)) if sc_conv is not None else (None, None)
+        folds = (PK.fold_bn(conv_a.bias, bn_a, cmid, d.Cmid), PK.fold_bn(conv_b.bias, bn_b, cmid, d.Cmid),
+                 PK.fold_bn(conv_c.bias, bn_c, cout, d.Cout),
+                 PK.fold_bn(sc_conv.bias, sc_bn, cout, d.Cout) if sc_conv is not None else (None, None))
+        sa, ba = (self.const(t) for t in folds[0])
+        sbb, bbb = (self.const(t) for t in folds[1])
+        scc, bcc = (self.const(t) for t in folds[2])
+        ss, bs = (self.const(t) for t in folds[3]) if sc_conv is not None else (None, None)
         lib = self.lib
 
         def fn(stream):
@@ -619,7 +636,12 @@ class Plan:
         flops = 2.0 * (m_in * cmid * cin * kt + m_out * cmid * cmid * 9 + m_out * cout * cmid +
                        (m_out * cout * cin if sc_conv is not None else 0))
         nbytes = (m_in * cin + m_out * cout) * 2 + sum(t.numel() for t in (wa, wb, wc)) * 2
-        self.add(name, fn, "fused_block", flops, nbytes, reads=(x,), writes=(y,))
+        widths = (cmid, cmid, cout, cout)
+        self.add(name, fn, "fused_block", flops, nbytes, reads=(x,), writes=(y,),
+                 spec={"kind": "fused_block", "x": x, "y": y, "wa": conv_a.weight, "wb": conv_b.weight,
+                       "wc": conv_c.weight, "ws": sc_conv.weight if sc_conv is not None else None, "kt": kt, "sb": sb,
+                       "act": act, "folds": tuple(None if t is None else t[:c] for f, c in zip(folds, widths) for t in f),
+                       "modules": (conv_a, conv_b, conv_c, sc_conv)})
         return y
 
     def emit_pool(self, x, mode, kernel, stride, padding, name="pool"):
@@ -641,7 +663,9 @@ class Plan:
         def fn(stream):
             d.x_row_stride, d.y_row_stride = x.row_stride, y.row_stride
             L.check(lib.pv_pool3d_fwd(C.byref(d), x.ptr(), y.ptr(), stream), "pv_pool3d_fwd(%s)" % name)
-        self.add(name, fn, reads=(x,), writes=(y,))
+        self.add(name, fn, reads=(x,), writes=(y,),
+                 spec={"kind": "pool", "x": x, "y": y, "mode": mode, "kernel": tuple(kernel), "stride": tuple(stride),
+                       "padding": tuple(padding), "cls": 0})
         return y
 
     def emit_se_scale_act(self, x, w1, b1, w2, b2, act, name="se"):
@@ -678,9 +702,10 @@ class Plan:
             L.check(lib.pv_scale_act(x.ptr(), x.ptr(), x.dt, x.row_stride, x.row_stride, x.N, npos, Cp,
                                      gate.tensor.data_ptr(), act, stream), "pv_scale_act(%s)" % name)
         if fused is None:
-            self.add(name + ".sum", fn_sum)
-        self.add(name + ".gate", fn_gate)
-        self.add(name + ".apply", fn_apply)
+            self.add(name + ".sum", fn_sum, spec={"kind": "channel_sum", "x": x, "sums": sums})
+        self.add(name + ".gate", fn_gate, spec={"kind": "se_gate", "x": x, "sums": sums, "gate": gate, "w1": w1p[:, :Cc],
+                                                "b1": b1.detach().float().cpu(), "w2": w2p[:Cc], "b2": b2p[:Cc]})
+        self.add(name + ".apply", fn_apply, spec={"kind": "scale_act", "x": x, "y": x, "gate": gate, "act": act})
         return x
 
     def raw_input(self, static_in):
@@ -713,7 +738,7 @@ class Plan:
         def fn(stream):
             L.check(lib.pv_scale_act(x.ptr(), x.ptr(), x.dt, x.row_stride, x.row_stride, x.N, x.npos, x.Cp,
                                      None, act, stream), "pv_scale_act(%s)" % name)
-        self.add(name, fn)
+        self.add(name, fn, spec={"kind": "scale_act", "x": x, "y": x, "gate": None, "act": act})
         return x
 
     def emit_head_reduce(self, x, softmax, name="head_reduce"):
@@ -723,7 +748,7 @@ class Plan:
         def fn(stream):
             L.check(lib.pv_head_reduce(x.ptr(), x.dt, x.row_stride, x.N, x.npos, x.C, 1 if softmax else 0,
                                        out.tensor.data_ptr(), stream), "pv_head_reduce(%s)" % name)
-        self.add(name, fn, reads=(x,), writes=(out,))
+        self.add(name, fn, reads=(x,), writes=(out,), spec={"kind": "head_reduce", "x": x, "out": out, "softmax": softmax})
         return out, (x.N, x.C)
 
     def emit_to_ncdhw(self, x, name="to_ncdhw"):
@@ -734,7 +759,7 @@ class Plan:
         def fn(stream):
             L.check(lib.pv_ndhwc_to_ncdhw(x.ptr(), x.dt, x.row_stride, out.tensor.data_ptr(), x.N, x.C, x.T,
                                           x.H, x.W, stream), "pv_ndhwc_to_ncdhw(%s)" % name)
-        self.add(name, fn, reads=(x,), writes=(out,))
+        self.add(name, fn, reads=(x,), writes=(out,), spec={"kind": "to_f32", "x": x, "out": out, "layout": "ncdhw"})
         return out, x.shape5()
 
     def emit_input_tokens(self, static_in):
@@ -774,7 +799,8 @@ class Plan:
             def fn_r(stream):
                 L.check(lib.pv_ndhwc_to_ncdhw(src.ptr(), src.dt, src.row_stride, out.tensor.data_ptr(), src.N, src.C, 1,
                                               1, 1, stream), "pv_ndhwc_to_ncdhw(%s)" % name)
-            self.add(name, fn_r, reads=(src,), writes=(out,))
+            self.add(name, fn_r, reads=(src,), writes=(out,),
+                     spec={"kind": "to_f32", "x": src, "out": out, "layout": "ncdhw"})
             return out, ((x.N, x.C) if squeeze else (x.N, 1, x.C))
         if x.row_stride != x.C or x.Cp != x.C:
             dense = self.new_tensor(x.N, 1, 1, x.npos, x.C, Cp=x.C, dt=x.dt)
@@ -783,7 +809,7 @@ class Plan:
             def fn_c(stream):
                 L.check(lib.pv_copy_rows(src.ptr(), dense.ptr(), src.dt, src.N * src.npos, src.C, src.row_stride,
                                          dense.row_stride, stream), "pv_copy_rows(%s)" % name)
-            self.add(name + ".dense", fn_c, reads=(src,), writes=(dense,))
+            self.add(name + ".dense", fn_c, reads=(src,), writes=(dense,), spec={"kind": "copy", "x": src, "y": dense})
             x = dense
         total = x.N * x.npos * x.C
         out = self.new_buf(total, L.PV_F32)
@@ -791,7 +817,7 @@ class Plan:
         def fn(stream):
             L.check(lib.pv_ndhwc_to_ncdhw(x.ptr(), x.dt, 1, out.tensor.data_ptr(), 1, 1, 1, 1, total, stream),
                     "pv_ndhwc_to_ncdhw(%s)" % name)
-        self.add(name, fn, reads=(x,), writes=(out,))
+        self.add(name, fn, reads=(x,), writes=(out,), spec={"kind": "to_f32", "x": x, "out": out, "layout": "ndhwc"})
         return out, ((x.N, x.C) if squeeze and x.npos == 1 else (x.N, x.npos, x.C))
 
     def concat_channels(self, parts):
@@ -834,19 +860,22 @@ def emit_layernorm(plan, x, ln, name="ln", rows_stride=None, rows=None):
     xs = x.row_stride if rows_stride is None else rows_stride
     y = plan.new_tensor(x.N, 1, 1, x.npos if rows is None else 1, C, Cp=C)
     lib = plan.lib
+    # rows: the first row of each sample (the cls rows of the MViT head)
+    spec = {"kind": "layernorm", "x": x, "y": y, "gamma": ln.weight.detach().float().cpu(),
+            "beta": ln.bias.detach().float().cpu(), "eps": eps, "first_row_only": rows is not None}
     if x.dt != plan.dt:          # fp32 trunk of the f16 engine: f32 in, f16 out
         assert x.dt == L.PV_F32 and plan.dt == L.PV_F16
 
         def fn32(stream):
             L.check(lib.pv_add_layernorm(x.ptr(), x.dt, xs, None, 0, None, 0, y.ptr(), y.row_stride, n_rows, C,
                                          g.data_ptr(), b.data_ptr(), eps, stream), "pv_add_layernorm(%s)" % name)
-        plan.add(name, fn32, "other", 0.0, n_rows * C * 6, reads=(x,), writes=(y,))
+        plan.add(name, fn32, "other", 0.0, n_rows * C * 6, reads=(x,), writes=(y,), spec=spec)
         return y
 
     def fn(stream):
         L.check(lib.pv_layernorm(x.ptr(), y.ptr(), x.dt, n_rows, 1, C, xs, y.row_stride, g.data_ptr(), b.data_ptr(),
                                  eps, stream), "pv_layernorm(%s)" % name)
-    plan.add(name, fn, "other", 0.0, n_rows * C * 4, reads=(x,), writes=(y,))
+    plan.add(name, fn, "other", 0.0, n_rows * C * 4, reads=(x,), writes=(y,), spec=spec)
     return y
 
 
@@ -875,7 +904,10 @@ def emit_add_layernorm(plan, a, br, ln, name="add_ln", want_sum=True):
                                      y.ptr() if y is not None else None, y.row_stride if y is not None else 0,
                                      n_rows, C, g.data_ptr() if g is not None else None,
                                      b.data_ptr() if b is not None else None, eps, stream), "pv_add_layernorm(%s)" % name)
-    plan.add(name, fn, "other", 0.0, n_rows * C * (_ESIZE[a.dt] + 2 + (4 if want_sum else 0) + (2 if ln is not None else 0)))
+    plan.add(name, fn, "other", 0.0, n_rows * C * (_ESIZE[a.dt] + 2 + (4 if want_sum else 0) + (2 if ln is not None else 0)),
+             spec={"kind": "add_layernorm", "a": a, "br": br, "s": s, "y": y, "eps": eps,
+                   "gamma": ln.weight.detach().float().cpu() if ln is not None else None,
+                   "beta": ln.bias.detach().float().cpu() if ln is not None else None})
     return s, y
 
 
@@ -891,7 +923,8 @@ def emit_pos_cls(plan, x, pos_table, has_cls, name="posenc", out_dt=None):
     def fn(stream):
         L.check(lib.pv_add_pos_cls_to(x.ptr(), x.dt, y.ptr(), y.dt, x.N, n_patch, C, x.row_stride, pos.data_ptr(),
                                       1 if has_cls else 0, stream), "pv_add_pos_cls_to")
-    plan.add(name, fn, "other", 0.0, x.N * n_patch * C * (_ESIZE[x.dt] + _ESIZE[y.dt]), reads=(x,), writes=(y,))
+    plan.add(name, fn, "other", 0.0, x.N * n_patch * C * (_ESIZE[x.dt] + _ESIZE[y.dt]), reads=(x,), writes=(y,),
+             spec={"kind": "pos_cls", "x": x, "y": y, "pos": pos_table.float(), "has_cls": bool(has_cls)})
     return y
 
 
@@ -1029,7 +1062,9 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool", norm_
                 L.check(lib.pv_dwconv3d_fwd(C_.byref(d), xp, w_d.data_ptr(), ones.data_ptr(), zeros.data_ptr(), yp,
                                             None, stream), "pv_dwconv3d_fwd(%s)" % name)
         plan.add(name + ".dwconv", fn, "depthwise", 2.0 * x.N * To * Ho * Wo * dim_all * k[0] * k[1] * k[2],
-                 (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz)
+                 (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz,
+                 spec={"kind": "token_conv", "x": x, "y": y, "thw": (T, H, W), "cls": cls, "weight": w_full,
+                       "stride": s, "padding": p, "dilation": dl, "prologue": norm_before_pool, "modules": pools})
     else:
         d = L.Pool3dDesc()
         d.dtype, d.mode = x.dt, L.POOL_MAX if kind == "MaxPool3d" else L.POOL_AVG
@@ -1045,7 +1080,9 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool", norm_
             L.check(lib.pv_pool3d_fwd(C_.byref(d), x.ptr() + cls * x.row_stride * esz,
                                       y.ptr() + cls * y.row_stride * esz, stream), "pv_pool3d_fwd(%s)" % name)
         plan.add(name + (".maxpool" if kind == "MaxPool3d" else ".avgpool"), fn, "other", 0.0,
-                 (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz)
+                 (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz,
+                 spec={"kind": "pool", "x": x, "y": y, "mode": d.mode, "kernel": k, "stride": s, "padding": p,
+                       "cls": cls, "thw": (T, H, W), "modules": pools})
     have_norm = [n is not None and type(n).__name__ != "Identity" and not norm_before_pool for n in norms]
     if any(have_norm) and not all(have_norm):
         raise NotImplementedError("%s: fused pooling branches need a norm on every branch" % name)
@@ -1054,7 +1091,7 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool", norm_
             def fn_cls(stream):
                 L.check(lib.pv_copy_rows(x.ptr(), y.ptr(), x.dt, x.N, dim_all, x.npos * x.row_stride, y.npos * y.row_stride,
                                          stream), "pv_copy_rows(%s)" % name)
-            plan.add(name + ".cls", fn_cls)
+            plan.add(name + ".cls", fn_cls, spec={"kind": "copy_cls", "x": x, "y": y})
         return y, (To, Ho, Wo)
     for n in norms:
         if type(n).__name__ != "LayerNorm":
@@ -1072,7 +1109,10 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool", norm_
         L.check(lib.pv_layernorm_sets(y.ptr(), y.ptr(), y.dt, y.N * y.npos, dim_all // hd, hd, y.row_stride, y.row_stride,
                                       g.data_ptr(), b.data_ptr(), dim // hd, x.ptr() if cls else None,
                                       x.npos * x.row_stride, y.npos, eps, stream), "pv_layernorm_sets(%s)" % name)
-    plan.add(name + ".norm", fn_ln, "other", 0.0, 2 * y.N * y.npos * dim_all * esz)
+    plan.add(name + ".norm", fn_ln, "other", 0.0, 2 * y.N * y.npos * dim_all * esz,
+             spec={"kind": "layernorm_sets", "x": x, "y": y, "cls": cls, "head_dim": hd, "eps": eps,
+                   "gamma": torch.cat([n.weight.detach().float().cpu() for n in norms]),
+                   "beta": torch.cat([n.bias.detach().float().cpu() for n in norms])})
     return y, (To, Ho, Wo)
 
 
@@ -1094,7 +1134,9 @@ def emit_attention(plan, q, k, v, heads, scale, residual_pool, name="attn", norm
         d.v_batch_stride, d.o_batch_stride = Nk * v.row_stride, Nq * o.row_stride
         L.check(lib.pv_attention_fwd(C_.byref(d), q.ptr(), k.ptr(), v.ptr(), o.ptr(), stream), "pv_attention_fwd(%s)" % name)
     plan.add(name, fn, "attention", 4.0 * B * heads * Nq * Nk * (dim // heads),
-             (B * Nq * dim * 2 + 2 * B * Nk * dim) * _ESIZE[plan.dt])
+             (B * Nq * dim * 2 + 2 * B * Nk * dim) * _ESIZE[plan.dt],
+             spec={"kind": "attention", "q": q, "k": k, "v": v, "o": o, "heads": heads, "scale": d.scale,
+                   "residual": bool(residual_pool), "normalize": d.normalize})
     plan.attention_calls.append({"name": name, "B": B, "H": heads, "Nq": Nq, "Nk": Nk, "D": dim // heads,
                                  "scale": d.scale, "normalize": d.normalize, "add_q_residual": d.add_q_residual})
     return o

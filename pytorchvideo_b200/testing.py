@@ -7,8 +7,11 @@ every BatchNorm random affine + running statistics (as the reference's tests/tes
 does) and re-draws conv / linear weights from a fixed seed, on the CPU generator, so the same
 state is reproduced bit-for-bit here and on the GPU box.
 """
+import math
+
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 
 
 def f16_exact(t):
@@ -376,6 +379,161 @@ def assert_close_to_f64(got, ref64, absref64, k_len, acc_eps=ACC_EPS, what="", e
         assert abs(bias) <= limit, "%s: mean signed error %.3g exceeds %.3g (biased rounding)" % (what, bias, limit)
     return float(ratio.max()), acc_ratio, extra_ratio
 
+
+
+# ---- float64 references shared by the kernel matrices and the per-launch workload audit ---------------------------
+# Bound of a run of K fp32 operations (additions, fused multiply-adds) on terms whose magnitudes sum to A:
+# |err| <= K * 2^-24 * A.  Expressed through the comparator's accumulation term acc_eps * (1 + K / 64) * A with
+# acc_eps = 2^-18 = 64 * 2^-24, i.e. (64 + K) * 2^-24 * A: the K roundings plus up to 64 further roundings of
+# intermediates of the same magnitude (divisions by the count, the final multiply-add, conversions).
+SUM_EPS = 2.0 ** -18
+# Attention error bound: the tensor-core kernels round the probabilities to f16 before P.V while the row sum l keeps
+# them in fp32, so an output may move by ~2 * 2^-11 of sum_j p_j |v_j| on top of its own rounding, independent of Nk;
+# ACC_EPS_ATTN (with k_len = 0) allows twice that (absref = p.|v| + |q|).
+ACC_EPS_ATTN = 2.0 ** -9
+# Lipschitz constants of the activations (largest slope)
+LIP = {"none": 1.0, "relu": 1.0, "swish": 1.1, "gelu": 1.13, "sigmoid": 0.25, "hswish": 1.5}
+
+
+def act64(v, act):
+    if act in (None, "none"):
+        return v
+    if act == "relu":
+        return v.clamp_min(0)
+    if act == "swish":
+        return v * torch.sigmoid(v)
+    if act == "gelu":
+        return 0.5 * v * (1 + torch.erf(v / math.sqrt(2.0)))
+    if act == "sigmoid":
+        return torch.sigmoid(v)
+    if act == "hswish":
+        return v * (v + 3).clamp(0, 6) / 6
+    raise ValueError(act)
+
+
+def act_err64(v, act):
+    """Error of apply_act (pv_common.cuh) evaluated in fp32 at the exact argument v.  __expf(x) is within
+    2 + floor(1.173 |x|) ulp (<= 2^-23 relative each) of e^x; the sigmoid factor s (1 - s) carries that relative
+    error into 1 / (1 + e).  erff is within 2 ulp.  Each further fp32 operation adds one rounding of the result."""
+    U = F32_EPS
+    a, y = v.abs(), act64(v, act).abs()
+    if act in (None, "none", "relu"):
+        return torch.zeros_like(v)
+    s = torch.sigmoid(v)
+    rel_e = (2 + 1.173 * a) * 2.0 ** -23
+    if act == "swish":
+        return a * s * (1 - s) * rel_e + 2 * U * y
+    if act == "sigmoid":
+        return s * (1 - s) * rel_e + 2 * U * s
+    if act == "gelu":
+        erf = torch.erf(v / math.sqrt(2.0))
+        return 0.5 * a * (2.0 ** -22 * erf.abs() + 0.5 * U + U * (1 + erf).abs()) + 2 * U * y
+    return U * a * (a + 3) / 6 + 2 * U * y                      # hswish: x + 3, x * clamp, / 6
+
+
+def conv_ref64(x, w, scale, bias, stride, padding, dilation, groups, act, res):
+    """(ref64, absref64) of y = act(conv(x, w) * scale + bias (+ res)) in float64 on x's device; absref is taken
+    before the activation (the magnitude the pre-activation sum is built from)."""
+    dev = x.device
+    x64, w64 = x.double(), w.double().to(dev)
+    sc, bi = scale.double().to(dev).view(1, -1, 1, 1, 1), bias.double().to(dev).view(1, -1, 1, 1, 1)
+    y = F.conv3d(x64, w64, None, stride, padding, dilation, groups) * sc + bi
+    a = F.conv3d(x64.abs(), w64.abs(), None, stride, padding, dilation, groups) * sc.abs() + bi.abs()
+    if res is not None:
+        y = y + res.double()
+        a = a + res.double().abs()
+    return act64(y, act), a
+
+
+def attn_ref64(q, k, v, scale, resid):
+    """q: [B,H,Nq,D] (f16 grid) -> (ref64, absref64) with absref = softmax . |v| (+ |q|)."""
+    q64, k64, v64 = q.double(), k.double(), v.double()
+    p = ((q64 * scale) @ k64.transpose(-2, -1)).softmax(-1)
+    ref = p @ v64
+    absref = p @ v64.abs()
+    if resid:
+        ref, absref = ref + q64, absref + q64.abs()
+    return ref, absref
+
+
+def _conv_bn(x, w, scale, bias, stride=1, padding=0):
+    return F.conv3d(x, w, None, stride, padding) * scale.view(1, -1, 1, 1, 1) + bias.view(1, -1, 1, 1, 1)
+
+
+def fused_block_ref64(x, wa, wb, wc, ws, folds, kt, sb, act):
+    """The fused bottleneck block in float64 on the f16-grid operands and the exact fp32 folded BatchNorm the kernel
+    uses.
+
+    Returns (y, A, B, Y, prop): y the result; A, B, Y the magnitude sums of a, b and y (the same sums over |x|, |w|,
+    |scale| and |bias|, plus |shortcut| for Y); prop the error of the kernel's f16 intermediates a and b propagated to
+    y.  Each intermediate may be off by one f16 rounding plus its fp32 accumulation term plus what it inherits (relu
+    is 1-Lipschitz, and a is exactly 0 outside the image where conv_b pads):
+      ea = F16_EPS |a| + ACC(Ka) A + 2^-24
+      eb = F16_EPS |b| + ACC(Kb) B + |sb| conv_b(ea, |wb|) + 2^-24
+      prop = |sc| conv_c(eb, |wc|)
+    with ACC(K) = 2^-20 (1 + K / 64).  The caller compares with assert_close_to_f64(got, y, Y, Kc + Ks, extra64=prop).
+    Runs on x's device."""
+    dev = x.device
+    f64 = [None if t is None else t.double().to(dev) for t in folds]
+    sa, ba, sbn, bbn, sc, bc, ssc, bsc = f64
+    x64 = x.double()
+    wa, wb, wc = (t.double().to(dev) for t in (wa, wb, wc))
+    pa, pb, st = (kt // 2, 0, 0), (0, 1, 1), (1, sb, sb)
+    cin, cmid = x.shape[1], wa.shape[0]
+
+    def acc(k):
+        return ACC_EPS * (1.0 + k / 64.0)
+    a = _conv_bn(x64, wa, sa, ba, 1, pa).clamp_min(0)
+    A = _conv_bn(x64.abs(), wa.abs(), sa.abs(), ba.abs(), 1, pa)
+    b = _conv_bn(a, wb, sbn, bbn, st, pb).clamp_min(0)
+    B = _conv_bn(a, wb.abs(), sbn.abs(), bbn.abs(), st, pb)
+    ea = F16_EPS * a + acc(kt * cin) * A + 2.0 ** -24
+    eb = (F16_EPS * b + acc(9 * cmid) * B + sbn.abs().view(1, -1, 1, 1, 1) * F.conv3d(ea, wb.abs(), None, st, pb)
+          + 2.0 ** -24)
+    del ea
+    if ws is None:
+        short = x64[:, :, :, ::sb, ::sb]
+        S = short.abs()
+    else:
+        ws = ws.double().to(dev)
+        short = _conv_bn(x64, ws, ssc, bsc, st)
+        S = _conv_bn(x64.abs(), ws.abs(), ssc.abs(), bsc.abs(), st)
+    y = act64(_conv_bn(b, wc, sc, bc) + short, act)
+    Y = _conv_bn(b, wc.abs(), sc.abs(), bc.abs()) + S
+    prop = sc.abs().view(1, -1, 1, 1, 1) * F.conv3d(eb, wc.abs())
+    return y, A, B, Y, prop
+
+
+def ln_ref64(v, gamma, beta, gps, depth, eps):
+    """(ref, absref, K, extra) of LayerNorm over the last dim of v [rows, groups, C]; group j uses set j // gps of
+    gamma / beta [sets, C].  The kernel sums a row at depth ``depth`` (see the LayerNorm rows of the CUDA-core
+    matrix); the mean is off by (depth + 1) 2^-24 mean|x|, rsqrtf by 2 ulp; the output takes <= 4 roundings."""
+    v = v.double()
+    G = v.shape[1]
+    idx = torch.arange(G, device=v.device) // gps
+    g64, b64 = gamma.double().to(v.device)[idx], beta.double().to(v.device)[idx]
+    mu = v.mean(-1, keepdim=True)
+    var = ((v - mu) ** 2).mean(-1, keepdim=True)
+    rstd = 1 / torch.sqrt(var + float(torch.tensor(eps, dtype=torch.float32)))
+    xh = (v - mu) * rstd
+    ref = xh * g64 + b64
+    m_abs = v.abs().mean(-1, keepdim=True)
+    absref = g64.abs() * (rstd * m_abs + xh.abs()) + b64.abs()
+    dmu = (depth + 1) * F32_EPS * m_abs * rstd
+    extra = (g64 * xh).abs() * (2.0 ** -22 + 0.5 * dmu ** 2)
+    return ref, absref, depth + 5, extra
+
+
+def ln_dispatch(C, aligned=True):
+    """(launch, lanes per row, chunks per lane) pv_layernorm_sets picks."""
+    chunks = -(-C // 8)
+    lg = 2
+    while (1 << lg) < chunks and lg < 5:
+        lg += 1
+    nch = -(-chunks // (1 << lg))
+    if nch <= 3 and aligned:
+        return "layernorm_reg_kernel", 1 << lg, nch
+    return "layernorm_kernel", 32, -(-chunks // 32)
 
 # ---- Non-local block cases (tests/golden/nonlocal.pt): name -> (create_nonlocal kwargs, input shape) ---------------
 NONLOCAL_CASES = {

@@ -30,26 +30,13 @@ import torch
 import torch.nn.functional as F
 
 from pytorchvideo_b200 import testing as TS
+from pytorchvideo_b200.testing import ACC_EPS_ATTN, attn_ref64, conv_ref64, fused_block_ref64
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "pytorchvideo_b200", "csrc")
 
 def _dev():
     return torch.device("cuda:0")
-
-
-def _act64(y, act):
-    if act in (None, "none"):
-        return y
-    if act == "relu":
-        return y.clamp_min(0)
-    if act == "swish":
-        return y * torch.sigmoid(y)
-    if act == "gelu":
-        return 0.5 * y * (1 + torch.erf(y / math.sqrt(2.0)))
-    if act == "sigmoid":
-        return torch.sigmoid(y)
-    raise ValueError(act)
 
 
 def _bn(c, seed):
@@ -61,19 +48,6 @@ def _bn(c, seed):
         bn.running_mean.copy_(torch.rand(c, generator=g) - 0.5)
         bn.running_var.copy_(torch.rand(c, generator=g) + 0.5)
     return bn
-
-
-def conv_ref64(x, w, scale, bias, stride, padding, dilation, groups, act, res):
-    """(ref64, absref64) of y = act(conv(x, w) * scale + bias (+ res)) in float64; absref is taken before the
-    activation (the magnitude the pre-activation sum is built from)."""
-    x64, w64 = x.double(), w.double()
-    sc, bi = scale.double().view(1, -1, 1, 1, 1), bias.double().view(1, -1, 1, 1, 1)
-    y = F.conv3d(x64, w64, None, stride, padding, dilation, groups) * sc + bi
-    a = F.conv3d(x64.abs(), w64.abs(), None, stride, padding, dilation, groups) * sc.abs() + bi.abs()
-    if res is not None:
-        y = y + res.double()
-        a = a + res.double().abs()
-    return _act64(y, act), a
 
 
 # ---- convolution rows --------------------------------------------------------------------------------------------
@@ -279,17 +253,6 @@ def test_depthwise_instance(row):
 
 
 # ---- attention -----------------------------------------------------------------------------------------------------
-def attn_ref64(q, k, v, scale, resid):
-    """q: [B,H,Nq,D] (f16 grid) -> (ref64, absref64) with absref = softmax . |v| (+ |q|)."""
-    q64, k64, v64 = q.double(), k.double(), v.double()
-    p = ((q64 * scale) @ k64.transpose(-2, -1)).softmax(-1)
-    ref = p @ v64
-    absref = p @ v64.abs()
-    if resid:
-        ref, absref = ref + q64, absref + q64.abs()
-    return ref, absref
-
-
 ATTN_NK = [1, 63, 64, 65, 393, 1569]
 
 
@@ -307,12 +270,6 @@ def _attn_rows():
 
 
 ATTN_ROWS = _attn_rows()
-
-# Attention error bound: the tensor-core kernels round the probabilities to f16 before P.V while the row sum l keeps
-# them in fp32, so an output may move by ~2 * 2^-11 of sum_j p_j |v_j| on top of its own rounding, independent of Nk;
-# ACC_EPS_ATTN (with k_len = 0) allows twice that (absref = p.|v| + |q|).
-ACC_EPS_ATTN = 2.0 ** -9
-
 
 def _attention_call(q, k, v, scale, resid, mode):
     from pytorchvideo_b200 import ops
@@ -742,53 +699,6 @@ def _fused_operands(inst, N, T, H, W, seed):
     for i, c in enumerate((cmid, cmid, cout, cout if proj else 0)):
         folds += list(_scale_bias(_bn(c, seed + i), c)) if c else [None, None]
     return x, wa, wb, wc, ws, tuple(folds)
-
-
-def _conv_bn(x, w, scale, bias, stride=1, padding=0):
-    return F.conv3d(x, w, None, stride, padding) * scale.view(1, -1, 1, 1, 1) + bias.view(1, -1, 1, 1, 1)
-
-
-def fused_block_ref64(x, wa, wb, wc, ws, folds, kt, sb, act):
-    """The fused block in float64 on the f16-grid operands and the exact fp32 folded BatchNorm the kernel uses.
-
-    Returns (y, A, B, Y, prop): y the result; A, B, Y the magnitude sums of a, b and y (the same sums over |x|, |w|,
-    |scale| and |bias|, plus |shortcut| for Y); prop the error of the kernel's f16 intermediates a and b propagated to
-    y.  Each intermediate may be off by one f16 rounding plus its fp32 accumulation term plus what it inherits (relu
-    is 1-Lipschitz, and a is exactly 0 outside the image where conv_b pads):
-      ea = F16_EPS |a| + ACC(Ka) A + 2^-24
-      eb = F16_EPS |b| + ACC(Kb) B + |sb| conv_b(ea, |wb|) + 2^-24
-      prop = |sc| conv_c(eb, |wc|)
-    with ACC(K) = 2^-20 (1 + K / 64).  The caller compares with assert_close_to_f64(got, y, Y, Kc + Ks, extra64=prop).
-    Runs on x's device."""
-    dev = x.device
-    f64 = [None if t is None else t.double().to(dev) for t in folds]
-    sa, ba, sbn, bbn, sc, bc, ssc, bsc = f64
-    x64 = x.double()
-    wa, wb, wc = (t.double().to(dev) for t in (wa, wb, wc))
-    pa, pb, st = (kt // 2, 0, 0), (0, 1, 1), (1, sb, sb)
-    cin, cmid = x.shape[1], wa.shape[0]
-
-    def acc(k):
-        return TS.ACC_EPS * (1.0 + k / 64.0)
-    a = _conv_bn(x64, wa, sa, ba, 1, pa).clamp_min(0)
-    A = _conv_bn(x64.abs(), wa.abs(), sa.abs(), ba.abs(), 1, pa)
-    b = _conv_bn(a, wb, sbn, bbn, st, pb).clamp_min(0)
-    B = _conv_bn(a, wb.abs(), sbn.abs(), bbn.abs(), st, pb)
-    ea = TS.F16_EPS * a + acc(kt * cin) * A + 2.0 ** -24
-    eb = (TS.F16_EPS * b + acc(9 * cmid) * B + sbn.abs().view(1, -1, 1, 1, 1) * F.conv3d(ea, wb.abs(), None, st, pb)
-          + 2.0 ** -24)
-    del ea
-    if ws is None:
-        short = x64[:, :, :, ::sb, ::sb]
-        S = short.abs()
-    else:
-        ws = ws.double().to(dev)
-        short = _conv_bn(x64, ws, ssc, bsc, st)
-        S = _conv_bn(x64.abs(), ws.abs(), ssc.abs(), bsc.abs(), st)
-    y = _act64(_conv_bn(b, wc, sc, bc) + short, act)
-    Y = _conv_bn(b, wc.abs(), sc.abs(), bc.abs()) + S
-    prop = sc.abs().view(1, -1, 1, 1, 1) * F.conv3d(eb, wc.abs())
-    return y, A, B, Y, prop
 
 
 def _fused_k(inst):

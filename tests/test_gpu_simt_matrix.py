@@ -35,17 +35,13 @@ import torch
 import torch.nn.functional as F
 
 from pytorchvideo_b200 import testing as TS
+from pytorchvideo_b200.testing import LIP, SUM_EPS, act64, act_err64
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "pytorchvideo_b200", "csrc")
 TESTS = os.path.dirname(os.path.abspath(__file__))
 
 U = TS.F32_EPS                  # fp32 unit roundoff
-# Bound of a run of K fp32 operations (additions, fused multiply-adds) on terms whose magnitudes sum to A:
-# |err| <= K * 2^-24 * A.  Expressed through the comparator's accumulation term acc_eps * (1 + K / 64) * A with
-# acc_eps = 2^-18 = 64 * 2^-24, i.e. (64 + K) * 2^-24 * A: the K roundings plus up to 64 further roundings of
-# intermediates of the same magnitude (divisions by the count, the final multiply-add, conversions).
-SUM_EPS = 2.0 ** -18
 TAIL = 64                       # sentinel elements after every output buffer
 SENT = {torch.float16: 0x5A5A, torch.float32: 0x5A5A5A5A, torch.int64: 0x5A5A5A5A5A5A5A5A}
 TDT = {"f16": torch.float16, "f32": torch.float32}
@@ -165,48 +161,12 @@ def _written(R, stride, C, off=0):
 
 # ---- activations: float64 reference, Lipschitz constant, error of the kernel's own fp32 evaluation ------------------
 ACTS = ("none", "relu", "swish", "gelu", "sigmoid", "hswish")
-LIP = {"none": 1.0, "relu": 1.0, "swish": 1.1, "gelu": 1.13, "sigmoid": 0.25, "hswish": 1.5}
 
 
 def _act_code(act):
     L = _L()
     return {"none": L.ACT_NONE, "relu": L.ACT_RELU, "swish": L.ACT_SWISH, "gelu": L.ACT_GELU,
             "sigmoid": L.ACT_SIGMOID, "hswish": L.ACT_HSWISH}[act]
-
-
-def act64(v, act):
-    if act == "none":
-        return v
-    if act == "relu":
-        return v.clamp_min(0)
-    if act == "swish":
-        return v * torch.sigmoid(v)
-    if act == "gelu":
-        return 0.5 * v * (1 + torch.erf(v / math.sqrt(2.0)))
-    if act == "sigmoid":
-        return torch.sigmoid(v)
-    if act == "hswish":
-        return v * (v + 3).clamp(0, 6) / 6
-    raise ValueError(act)
-
-
-def act_err64(v, act):
-    """Error of apply_act (pv_common.cuh) evaluated in fp32 at the exact argument v.  __expf(x) is within
-    2 + floor(1.173 |x|) ulp (<= 2^-23 relative each) of e^x; the sigmoid factor s (1 - s) carries that relative
-    error into 1 / (1 + e).  erff is within 2 ulp.  Each further fp32 operation adds one rounding of the result."""
-    a, y = v.abs(), act64(v, act).abs()
-    if act in ("none", "relu"):
-        return torch.zeros_like(v)
-    s = torch.sigmoid(v)
-    rel_e = (2 + 1.173 * a) * 2.0 ** -23
-    if act == "swish":
-        return a * s * (1 - s) * rel_e + 2 * U * y
-    if act == "sigmoid":
-        return s * (1 - s) * rel_e + 2 * U * s
-    if act == "gelu":
-        erf = torch.erf(v / math.sqrt(2.0))
-        return 0.5 * a * (2.0 ** -22 * erf.abs() + 0.5 * U + U * (1 + erf).abs()) + 2 * U * y
-    return U * a * (a + 3) / 6 + 2 * U * y                      # hswish: x + 3, x * clamp, / 6
 
 
 def act32(v, act):
@@ -910,18 +870,6 @@ LN_ROWS = [
 LN_EPS = 1e-6
 
 
-def ln_dispatch(C, aligned=True):
-    """(launch, lanes per row, chunks per lane) pv_layernorm_sets picks."""
-    chunks = -(-C // 8)
-    lg = 2
-    while (1 << lg) < chunks and lg < 5:
-        lg += 1
-    nch = -(-chunks // (1 << lg))
-    if nch <= 3 and aligned:
-        return REG, 1 << lg, nch
-    return GEN, 32, -(-chunks // 32)
-
-
 def ln_inputs(row):
     """(x [rows, groups * C] fp32 on the storage grid, cls source [B, src_npos, src_rs] or None, gamma, beta [sets, C])."""
     name, entry, dt, rows, groups, gps, C, xrs, yrs, cnpos, inplace, kind, goff = row
@@ -955,24 +903,6 @@ def _ln_eff(x, cls, row):
     if cls is not None:
         v.view(rows // cnpos, cnpos, -1)[:, 0] = cls[:, 0, groups * C:2 * groups * C]
     return v.view(rows, groups, C)
-
-
-def ln_ref64(v, gamma, beta, gps, depth, eps=LN_EPS):
-    """(ref, absref, K, extra) of LayerNorm over the last dim of v [rows, groups, C]; group j uses set j // gps."""
-    v = v.double()
-    G = v.shape[1]
-    idx = torch.arange(G) // gps
-    g64, b64 = gamma.double()[idx], beta.double()[idx]
-    mu = v.mean(-1, keepdim=True)
-    var = ((v - mu) ** 2).mean(-1, keepdim=True)
-    rstd = 1 / torch.sqrt(var + float(torch.tensor(eps, dtype=torch.float32)))
-    xh = (v - mu) * rstd
-    ref = xh * g64 + b64
-    m_abs = v.abs().mean(-1, keepdim=True)
-    absref = g64.abs() * (rstd * m_abs + xh.abs()) + b64.abs()
-    dmu = (depth + 1) * U * m_abs * rstd
-    extra = (g64 * xh).abs() * (2.0 ** -22 + 0.5 * dmu ** 2)
-    return ref, absref, depth + 5, extra
 
 
 def ln_emulate(v, gamma, beta, gps, lpr, nch, eps=LN_EPS, mutation=None):
@@ -1266,6 +1196,15 @@ def test_add_pos_cls_row(row):
     want[:R * C] = pos_emulate(x, pos, row).reshape(-1)
     _assert_bits(yb, want, name)
     _exact("add-pos-cls", row, launched)
+
+
+def ln_dispatch(C, aligned=True):
+    """(launch, lanes per row, chunks per lane) pv_layernorm_sets picks."""
+    return TS.ln_dispatch(C, aligned)
+
+
+def ln_ref64(v, gamma, beta, gps, depth, eps=LN_EPS):
+    return TS.ln_ref64(v, gamma, beta, gps, depth, eps)
 
 
 # =====================================================================================================================
