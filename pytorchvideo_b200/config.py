@@ -1,5 +1,5 @@
 """Process-wide defaults for the engine."""
-_state = {"precision": "f16", "use_tcgen05": True, "use_graph": True}
+_state = {"precision": "f16", "use_graph": True}
 
 
 def set_precision(p):
@@ -10,14 +10,6 @@ def set_precision(p):
 
 def get_precision():
     return _state["precision"]
-
-
-def set_use_tcgen05(flag):
-    _state["use_tcgen05"] = bool(flag)
-
-
-def get_use_tcgen05():
-    return _state["use_tcgen05"]
 
 
 def set_use_graph(flag):

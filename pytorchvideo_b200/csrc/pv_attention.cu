@@ -5,7 +5,6 @@
 // A CTA owns ATT_BQ query rows of one (batch, head); K/V stream through shared memory in tiles
 // of 32 keys; online softmax state (running max / sum / output) stays in registers.
 #include "pv_common.cuh"
-#include <stdlib.h>
 
 namespace pv {
 
@@ -228,7 +227,7 @@ extern "C" int pv_attention_kernel_for(const pv_attention_desc* d, const void* q
     pv::set_error("linear attention (normalize = 1) head dim %d unsupported (64/128/256/512)", d->D);
     return PV_ERR_UNSUPPORTED;
   }
-  const bool tc = d->dtype == PV_F16 && !getenv("PVB200_ATTN_SIMT") && pv::tensor_core_aligned(d, q, k, v, o);
+  const bool tc = d->dtype == PV_F16 && pv::tensor_core_aligned(d, q, k, v, o);
   if (pv::wide_family(d)) return tc ? PV_ATTN_WIDE : PV_ATTN_SIMT;
   if (tc) return d->D == 128 ? PV_ATTN_MMA : PV_ATTN_WGMMA;
   return PV_ATTN_SIMT;

@@ -11,7 +11,6 @@
 // and the MViT pooling convs (layers/attention.py:364-403).
 #include "pv_common.cuh"
 #include "pv_sm90.cuh"
-#include <stdlib.h>
 #include <string.h>
 
 namespace pv {
@@ -378,16 +377,14 @@ extern "C" int pv_dwconv3d_fwd(const pv_conv3d_desc* d, const void* x, const voi
   int rc = pv::conv3d_check(d);
   if (rc != PV_OK) return rc;
   cudaStream_t s = (cudaStream_t)stream;
-  if (!getenv("PVB200_DW_SIMT")) {
-    // 3x3x3: lane-per-channel-pair register stencil (pv_dwlane.cu)
-    rc = pv::dwconv3d_lane_launch(d, x, w, scale, bias, y, se_sums, s);
-    if (rc != PV_ERR_UNSUPPORTED) return rc;
-    // kt x 1 x 1: streaming register window
-    rc = pv::dwconv3d_temporal_launch(d, x, w, scale, bias, y, se_sums, s);
-    if (rc != PV_ERR_UNSUPPORTED) return rc;
-    rc = pv::dwconv3d_tile_launch(d, x, w, scale, bias, y, se_sums, s);
-    if (rc != PV_ERR_UNSUPPORTED) return rc;
-  }
+  // 3x3x3: lane-per-channel-pair register stencil (pv_dwlane.cu)
+  rc = pv::dwconv3d_lane_launch(d, x, w, scale, bias, y, se_sums, s);
+  if (rc != PV_ERR_UNSUPPORTED) return rc;
+  // kt x 1 x 1: streaming register window
+  rc = pv::dwconv3d_temporal_launch(d, x, w, scale, bias, y, se_sums, s);
+  if (rc != PV_ERR_UNSUPPORTED) return rc;
+  rc = pv::dwconv3d_tile_launch(d, x, w, scale, bias, y, se_sums, s);
+  if (rc != PV_ERR_UNSUPPORTED) return rc;
   // generic path: stencil kernel, then (if requested) a separate channel-sum pass
   int rc2 = pv::conv3d_direct_launch(d, x, w, scale, bias, nullptr, y, s);
   if (rc2 != PV_OK || !se_sums) return rc2;

@@ -2,7 +2,6 @@
 // pooling, squeeze-excitation, head reduction, LayerNorm.  All are HBM-bound or serve shapes the
 // tensor-core implicit-GEMM path does not take (3-channel stems, fp32 "parity" storage).
 #include "pv_common.cuh"
-#include <stdlib.h>
 
 namespace pv {
 
@@ -1092,7 +1091,7 @@ int conv3d_direct_launch(const pv_conv3d_desc* d, const void* x, const void* w, 
     const bool pre = d->pre_scale != nullptr;
     PV_CHECK_ARG(d->x_row_stride % 8 == 0 && d->y_row_stride % 8 == 0, "row strides must be multiples of 8");
     // TMA-fed shared-memory stencil (pv_dwconv.cu) whenever it applies
-    if (!d->has_residual && d->dtype == PV_F16 && !getenv("PVB200_DW_SIMT")) {
+    if (!d->has_residual && d->dtype == PV_F16) {
       const int rc = dwconv3d_tile_launch(d, x, w, scale, bias, y, nullptr, s);
       if (rc != PV_ERR_UNSUPPORTED) return rc;
     }

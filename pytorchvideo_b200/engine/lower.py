@@ -279,9 +279,8 @@ class Lowering:
         plain Conv3d / BatchNorm / ReLU bottleneck with a (kt,1,1) conv_a, a dense (1,3,3) conv_b of stride
         (1,s,s) and an inner width of 8 / 16 / 32 channels (the SlowFast Fast pathway, res2-res4)."""
         import ctypes as C_
-        import os
         p = self.p
-        if not p.use_tcgen05 or os.environ.get("PVB200_NO_FUSED"):
+        if p.dt != L.PV_F16:
             return False
         b = m.branch2
         if type(b).__name__ != "BottleneckBlock" or not isinstance(x, TRef):
@@ -661,7 +660,7 @@ class CompiledModel:
     ``extra`` carries non-tensor forward arguments (the ``thw_shape`` of MultiScaleBlock / MultiScaleAttention);
     a lowering handler may leave a second, host-side result in ``Lowering.aux_out`` (the pooled thw)."""
 
-    def __init__(self, model, example_inputs, dtype="f16", use_tcgen05=True, use_graph=True, extra=()):
+    def __init__(self, model, example_inputs, dtype="f16", use_graph=True, extra=()):
         L.require_device()
         multi = isinstance(example_inputs, (list, tuple))
         ins = list(example_inputs) if multi else [example_inputs]
@@ -676,7 +675,7 @@ class CompiledModel:
             raise RuntimeError("pytorchvideo_b200 has no CPU path: inputs must be CUDA tensors")
         dt = {"f16": L.PV_F16, "f32": L.PV_F32}[dtype]
         self.multi = multi
-        self.plan = Plan(device, dt, use_tcgen05)
+        self.plan = Plan(device, dt)
         self.static_in = [torch.empty(t.shape, dtype=torch.uint8 if i in self.mask_slots else
                                       t.dtype if (t.dtype in (torch.float16, torch.float32) and i not in raw)
                                       else torch.float32, device=device) for i, t in enumerate(ins)]
@@ -830,17 +829,17 @@ def _emit_output(plan, out, tokens):
     return out
 
 
-def compile_model(model, example_inputs, dtype="f16", use_tcgen05=True, use_graph=True, extra=()):
-    return CompiledModel(model, example_inputs, dtype, use_tcgen05, use_graph, extra)
+def compile_model(model, example_inputs, dtype="f16", use_graph=True, extra=()):
+    return CompiledModel(model, example_inputs, dtype, use_graph, extra)
 
 
-def lower_only(model, example_inputs, dtype="f16", use_tcgen05=True, extra=()):
+def lower_only(model, example_inputs, dtype="f16", extra=()):
     """Host-side dry run (works without a GPU): build the plan on the CPU and return
     (plan, output_shape).  Nothing can be executed; used by the CPU test-suite to check the
     lowering, shape inference, channel padding, concat fusion and algorithm selection."""
     multi = isinstance(example_inputs, (list, tuple))
     ins = list(example_inputs) if multi else [example_inputs]
-    plan = Plan("cpu", {"f16": L.PV_F16, "f32": L.PV_F32}[dtype], use_tcgen05)
+    plan = Plan("cpu", {"f16": L.PV_F16, "f32": L.PV_F32}[dtype])
     raw = _raw_inputs(model, ins)
     masks = _mask_slots(ins, extra)
     _image_root(model, ins)

@@ -8,7 +8,6 @@ buffer after it was produced - that is how ``torch.cat([slow, fuse], dim=1)``
 buffer.
 """
 import ctypes as C
-import os
 
 import torch
 
@@ -90,11 +89,10 @@ def _conv_out(i, k, s, p, d):
 class Plan:
     """Collects launches; ``finalize`` allocates, ``run`` replays (eagerly or as a CUDA graph)."""
 
-    def __init__(self, device, dt=L.PV_F16, use_tcgen05=True):
+    def __init__(self, device, dt=L.PV_F16):
         self.lib = L.load()
         self.device = torch.device(device)
         self.dt = dt
-        self.use_tcgen05 = bool(use_tcgen05) and dt == L.PV_F16
         self.ops = []          # (name, closure(stream_ptr))
         self.meta = []         # per-op {name, kind, flops, bytes} (algorithmic figures for the roofline)
         # per op: what it computes, in torch terms ({"kind": "conv", "x": TRef, "weight": ..., "y": TRef, ...}), or None
@@ -117,7 +115,6 @@ class Plan:
         self.op_lane = []
         self.op_io = []        # (reads, writes) as lists of TRef / Buf, or None = unknown (acts as a full barrier)
         self.sched = None
-        self.multi_lane = os.environ.get("PVB200_LANES", "1") != "0"
         # f16 engine, MViT: the residual token stream (16 blocks x 2 adds) is kept in fp32 - branch outputs stay f16, the
         # add + LayerNorm is one kernel (pv_add_layernorm).
         self.trunk32 = dt == L.PV_F16
@@ -243,7 +240,7 @@ class Plan:
         parallel branches (and an eager call overlaps them the same way)."""
         assert self.finalized
         lanes = self.sched["lanes"]
-        if single_stream or not self.multi_lane or len(lanes) <= 1:
+        if single_stream or len(lanes) <= 1:
             for _, fn in self.ops:
                 fn(stream_ptr)
             return
@@ -357,7 +354,7 @@ class Plan:
             # grouped conv (ResNeXt-style group counts, CSN with several channels per group): the grouped mode of the
             # TMA-fed kernel when the library takes the shape, else the dense convolution with block-diagonal weights
             # (one group span, C % 8 != 0, non-square groups, f32, forced CUDA-core algorithm)
-            if self.use_tcgen05 and force_algo in (None, L.ALGO_TCGEN05) and x.Cp == ci and co_pad == co:
+            if self.dt == L.PV_F16 and force_algo in (None, L.ALGO_TCGEN05) and x.Cp == ci and co_pad == co:
                 probe = self._conv_desc(x, (To, Ho, Wo), co_pad, (kt, kh, kw), stride, padding, dilation, groups, act,
                                         residual, co_pad, 0)
                 if addend is not None:
@@ -375,7 +372,7 @@ class Plan:
         m_out = x.N * To * Ho * Wo
         flops = 2.0 * m_out * co * cig * kt * kh * kw
         nbytes = (x.N * x.npos * ci + m_out * co * (2 if residual is not None else 1)) * esz + weight.numel() * esz
-        stem_candidate = (x.lazy_src is not None and self.use_tcgen05 and force_algo in (None, L.ALGO_TCGEN05)
+        stem_candidate = (x.lazy_src is not None and self.dt == L.PV_F16 and force_algo in (None, L.ALGO_TCGEN05)
                           and groups == 1 and x.Cp == 4 and kt > 1 and residual is None and addend is None and dlw == 1
                           and pw > 0)
         # Narrow stems with a temporal extent run as two launches, `.taps` (the convolution's tensor-core pass) and
@@ -384,9 +381,8 @@ class Plan:
         #      row over all input frames and sums the kt temporal taps in fp32 registers, so `.taps` writes the Co
         #      channels of the pre-BN sum once (rounded to f16 once); `.tapsum` is then the BN / activation pass over
         #      it (one tap).  With fewer rows than SMs the factored route fills the machine better (its taps pass has
-        #      kt times more tiles).  PVB200_NO_STEMSTREAM: the factored route at every size, for A/B runs.
-        if (stem_candidate and x.N * Ho * -(-Wo // 128) >= H100_SXM_SMS
-                and not os.environ.get("PVB200_NO_STEMSTREAM")):
+        #      kt times more tiles).
+        if stem_candidate and x.N * Ho * -(-Wo // 128) >= H100_SXM_SMS:
             wp, w_phys, lead, win = self._stem_window(x, kw, sw, pw, Wo)
             d = self._conv_desc(x, (To, Ho, Wo), co_pad, (kt, kh, kw), stride, padding, dilation, 1, L.ACT_NONE, None,
                                 co_pad, win)
@@ -409,7 +405,7 @@ class Plan:
         # ---- network input: pick the layout its first consumer wants
         window = False
         if x.lazy_src is not None:
-            window = (self.use_tcgen05 and force_algo in (None, L.ALGO_TCGEN05) and groups == 1 and x.Cp == 4
+            window = (self.dt == L.PV_F16 and force_algo in (None, L.ALGO_TCGEN05) and groups == 1 and x.Cp == 4
                       and dlw == 1 and (sw * x.Cp * 2) % 16 == 0 and (kw + 1) * x.Cp <= 64 and kt * kh <= 64
                       and st * sh <= 8 and pw > 0)
             if window:
@@ -460,7 +456,7 @@ class Plan:
             algo, kind = L.ALGO_TCGEN05, "grouped"
             w_d = self.const(PK.pack_grouped_tcgen05(weight, groups, span[0], span[1]))
         else:
-            want_tc = self.use_tcgen05 and bool(self.lib.pv_conv3d_tcgen05_supported(C.byref(d)))
+            want_tc = self.dt == L.PV_F16 and bool(self.lib.pv_conv3d_tcgen05_supported(C.byref(d)))
             if force_algo is not None:
                 want_tc = force_algo == L.ALGO_TCGEN05
             if window and not want_tc:

@@ -29,10 +29,10 @@ CHUNK = 4096            # elements per block of pv_weights_refresh (csrc/pv_cont
 _BASE = 1024
 
 
-def _lower_consts(model, shapes, dtype, use_tcgen05, extra):
+def _lower_consts(model, shapes, dtype, extra):
     from .lower import lower_only
     plan, _ = lower_only(model, [torch.empty(s) for s in shapes] if len(shapes) > 1 else torch.empty(shapes[0]),
-                         dtype, use_tcgen05, extra)
+                         dtype, extra)
     return [t.double() for t in plan.consts], plan.const_folds
 
 
@@ -62,7 +62,7 @@ class WeightsRefresh:
         self.device = dev
 
     @classmethod
-    def build(cls, cm, model, example_inputs, dtype, use_tcgen05=True, extra=()):
+    def build(cls, cm, model, example_inputs, dtype, extra=()):
         """The refresh of the compiled plan ``cm`` of ``model``, or None when the plan is not refreshable."""
         ins = list(example_inputs) if isinstance(example_inputs, (list, tuple)) else [example_inputs]
         shapes = [tuple(t.shape) for t in ins]
@@ -82,7 +82,7 @@ class WeightsRefresh:
             with torch.no_grad():
                 for k, p in enumerate(wparams):
                     p.copy_(fill(k, p))
-            return _lower_consts(work, shapes, dtype, use_tcgen05, extra)
+            return _lower_consts(work, shapes, dtype, extra)
 
         a, fa = encoded(lambda k, p: torch.full(p.shape, float(k + 1)))
         b, _ = encoded(lambda k, p: torch.full(p.shape, float(2 * (k + 1))))

@@ -88,13 +88,11 @@ class BYOL(nn.Module):
         if st["fp"] != fp:                                 # backbone_mmt changed from outside: compile again
             st["plans"].clear()
             st["fp"] = fp
-        key = (tuple(x.shape), x.dtype, x.device.index, config.get_precision(), config.get_use_tcgen05(),
-               config.get_use_graph())
+        key = (tuple(x.shape), x.dtype, x.device.index, config.get_precision(), config.get_use_graph())
         entry = st["plans"].get(key)
         if entry is None:
-            cm = _lower.compile_model(ch, x, config.get_precision(), config.get_use_tcgen05(), config.get_use_graph())
-            entry = st["plans"][key] = (cm, WeightsRefresh.build(cm, ch, x, config.get_precision(),
-                                                                 config.get_use_tcgen05()))
+            cm = _lower.compile_model(ch, x, config.get_precision(), config.get_use_graph())
+            entry = st["plans"][key] = (cm, WeightsRefresh.build(cm, ch, x, config.get_precision()))
         return entry[0]
 
     @torch.no_grad()

@@ -35,7 +35,7 @@ class B200Module(nn.Module):
         if self.training:
             raise RuntimeError("pytorchvideo_b200 is an eval-mode forward engine: call model.eval() first")
         key = (tuple((tuple(t.shape), t.dtype, t.device.index) for t in ins), config.get_precision(),
-               config.get_use_tcgen05(), config.get_use_graph(), tuple(extra), self._pv_fingerprint())
+               config.get_use_graph(), tuple(extra), self._pv_fingerprint())
         cache = self.__dict__.setdefault("_pv_cache", {})
         cm = cache.pop(key, None)
         if cm is None:
@@ -45,7 +45,7 @@ class B200Module(nn.Module):
             while len(cache) >= self._PV_CACHE_PLANS:
                 del cache[next(iter(cache))]       # least recently used
             cm = compile_model(self, list(ins) if isinstance(x, (list, tuple)) else x, config.get_precision(),
-                               config.get_use_tcgen05(), config.get_use_graph(), extra=extra)
+                               config.get_use_graph(), extra=extra)
         cache[key] = cm                            # (re)insert at the most-recently-used end
         return cm
 

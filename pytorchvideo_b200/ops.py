@@ -28,7 +28,7 @@ def conv3d_bn_act(x, weight, bias=None, bn=None, stride=(1, 1, 1), padding=(0, 0
     """y = act(BN(conv3d(x)) + residual); x, residual: [N,C,T,H,W] CUDA tensors; returns f32 NCDHW.
     se_sums=True (depthwise): stats additionally carries "se_sums" = per-(n, c) output sums [N, C]."""
     _require_cuda(x, residual)
-    plan = Plan(x.device, _DT[dtype], use_tcgen05=True)
+    plan = Plan(x.device, _DT[dtype])
     xin = x.contiguous().float()
     xr = plan.emit_input_ncdhw(xin, x.shape[1], 4 if x.shape[1] <= 4 else (x.shape[1] + 7) // 8 * 8)
     rr = None

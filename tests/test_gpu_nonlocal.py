@@ -211,7 +211,8 @@ def _wide_rows():
         for mode in modes:
             for i, (nq, nk) in enumerate(SIMT_NQ_NK):
                 rows.append(("attention_wide_simt_kernel<float,%d>" % D, "f32", D, mode, nq, nk, 1 + 2 * (i % 2)))
-                rows.append(("attention_wide_simt_kernel<__half,%d>" % D, "simt", D, mode, nq, nk, 3 - 2 * (i % 2)))
+                rows.append(("attention_wide_simt_kernel<__half,%d>" % D, "unaligned", D, mode, nq, nk,
+                             3 - 2 * (i % 2)))
     return rows
 
 
@@ -256,7 +257,8 @@ def _dev():
 def _run_attention(q, k, v, scale, normalize, mode, layout="slices", resid=False):
     """pv_attention_fwd with q / k / v as channel slices: with Nq == Nk of ONE theta|phi|g buffer [B][N][3D] (the
     un-pooled Non-local block), else q from a theta buffer and k / v from a phi|g buffer [B][Nk][2D] (pooled).  mode:
-    f16, f32, or simt (f16 storage, CUDA-core kernel forced)."""
+    f16, f32, or unaligned (f16 storage with o 2 bytes off the 4-byte alignment the tensor-core kernels store with: the
+    CUDA-core kernel)."""
     L = _lib()
     B, Nq, D = q.shape
     Nk = k.shape[1]
@@ -272,17 +274,13 @@ def _run_attention(q, k, v, scale, normalize, mode, layout="slices", resid=False
         buf = torch.cat([k, v], -1).to(tdt).to(_dev()).contiguous()
         qp, kp, vp = qb.data_ptr(), buf.data_ptr(), buf.data_ptr() + D * buf.element_size()
         q_rs, kv_rs, q_bs, kv_bs = D, 2 * D, Nq * D, Nk * 2 * D
-    o = torch.empty(B, Nq, D, dtype=tdt, device=_dev())
+    off = 1 if mode == "unaligned" else 0
+    o = torch.empty(off + B * Nq * D, dtype=tdt, device=_dev())
     d = _desc(dt, B, Nq, Nk, D, q_rs, kv_rs, q_bs, kv_bs, D, Nq * D, normalize, 1 if resid else 0, scale)
-    if mode == "simt":
-        os.environ["PVB200_ATTN_SIMT"] = "1"
-    try:
-        L.check(L.load().pv_attention_fwd(C.byref(d), qp, kp, vp, o.data_ptr(), torch.cuda.current_stream().cuda_stream),
-                "pv_attention_fwd")
-        torch.cuda.synchronize()
-    finally:
-        os.environ.pop("PVB200_ATTN_SIMT", None)
-    return o.float().cpu()
+    L.check(L.load().pv_attention_fwd(C.byref(d), qp, kp, vp, o.data_ptr() + off * o.element_size(),
+                                      torch.cuda.current_stream().cuda_stream), "pv_attention_fwd")
+    torch.cuda.synchronize()
+    return o[off:].view(B, Nq, D).float().cpu()
 
 
 def _qkv(B, Nq, Nk, D, seed, mag=1.0):
@@ -358,7 +356,7 @@ def test_wide_linear_large_magnitude(D):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("D,normalize,mode", [(64, 1, "f16"), (128, 1, "f16"), (256, 0, "f16"), (256, 1, "f16"),
-                                              (512, 0, "f16"), (512, 1, "f16"), (512, 0, "f32"), (256, 1, "simt")])
+                                              (512, 0, "f16"), (512, 1, "f16"), (512, 0, "f32"), (256, 1, "unaligned")])
 def test_wide_batch_invariance(D, normalize, mode):
     """B = 3 gives bit for bit the three B = 1 results."""
     q, k, v = _qkv(3, 196, 784, D, seed=D + normalize)

@@ -144,18 +144,10 @@ def test_stem_stream_through_the_plan():
 
 
 # ---- CPU: routing -------------------------------------------------------------------------------------------------
-def _fast_stem_ops(batch, env=None):
+def _fast_stem_ops(batch):
     import pytorchvideo_b200.models.hub as PH
     from pytorchvideo_b200.engine.lower import lower_only
-    old = os.environ.pop("PVB200_NO_STEMSTREAM", None)
-    if env:
-        os.environ["PVB200_NO_STEMSTREAM"] = env
-    try:
-        plan, _ = lower_only(PH.slowfast_r50().eval(), TS.slowfast_inputs(torch.zeros(batch, 3, 32, 224, 224)))
-    finally:
-        os.environ.pop("PVB200_NO_STEMSTREAM", None)
-        if old is not None:
-            os.environ["PVB200_NO_STEMSTREAM"] = old
+    plan, _ = lower_only(PH.slowfast_r50().eval(), TS.slowfast_inputs(torch.zeros(batch, 3, 32, 224, 224)))
     stem = "blocks.0.multipathway_blocks.1.conv"
     return [m for m in plan.meta if m["name"].startswith(stem)], plan.stats
 
@@ -163,7 +155,7 @@ def _fast_stem_ops(batch, env=None):
 PAIR = [("blocks.0.multipathway_blocks.1.conv.taps", "tcgen05"), ("blocks.0.multipathway_blocks.1.conv.tapsum", "other")]
 
 
-def test_slowfast_batch8_fast_stem_streams():
+def test_slowfast_fast_stem_route_by_batch(monkeypatch):
     """Batch 8: the stream kernel as `.taps`; `.tapsum` then reads one tap (its Co = 8 channels of the pre-BN sum),
     not the kt * Co channels of the factored partials.  The op list is the factored route's either way."""
     ops8, stats = _fast_stem_ops(8)
@@ -171,7 +163,10 @@ def test_slowfast_batch8_fast_stem_streams():
     assert stats["stem_stream"] == 1
     n_out = 8 * 32 * 112 * 112 * 8
     assert ops8[1]["bytes"] == 2 * n_out * 2
-    off, stats_off = _fast_stem_ops(8, env="1")
+    from pytorchvideo_b200.engine import plan as PL
+    monkeypatch.setattr(PL, "H100_SXM_SMS", 1 << 30)      # no batch fills the machine: the factored route
+    off, stats_off = _fast_stem_ops(8)
+    monkeypatch.undo()
     assert [(m["name"], m["kind"]) for m in off] == PAIR, off
     assert "stem_stream" not in stats_off
     assert off[1]["bytes"] == (5 + 1) * n_out * 2

@@ -74,7 +74,7 @@ def main():
     print("byol momentum plan refresh (pv_weights_refresh): %.3f ms" % timed(refresh, a.iters, a.warmup))
 
     def recompile():
-        c = _lower.compile_model(st["mmt"], x1, config.get_precision(), config.get_use_tcgen05(), config.get_use_graph())
+        c = _lower.compile_model(st["mmt"], x1, config.get_precision(), config.get_use_graph())
         c(x1)
     print("byol momentum plan compiled again instead: %.3f ms" % timed(recompile, max(3, a.iters // 4), 1))
     print("byol momentum plan, replay:         %.3f ms" % timed(lambda: m._mmt_embed(x1), a.iters, a.warmup))

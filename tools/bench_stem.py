@@ -2,10 +2,10 @@
 
     python tools/bench_stem.py [--launches 50] [--rounds 7] [--out DIR]
 
-Each route of one stem shape is built in one process (the routing switch PVB200_NO_STEMSTREAM is toggled between plan
-builds; the stream route is also taken below its one-wave threshold), its launches are captured `launches` times into a
-CUDA graph, and the routes' graphs are replayed alternately for `rounds` rounds, timed with CUDA events; the median per
-launch is reported.  Shapes: the SlowFast Fast stem (5x7x7, 3 -> 8) at batch 1, 2 and 8, on 32 frames of 224^2.
+Each route of one stem shape is built in one process (the SM count the planner routes by, plan.H100_SXM_SMS, is patched
+per plan build: down to 1, so the stream route is also taken below its one-wave threshold, or up past any batch, so the
+factored route is taken above it), its launches are captured `launches` times into a CUDA graph, and the routes'
+graphs are replayed alternately for `rounds` rounds, timed with CUDA events; the median per launch is reported.  Shapes: the SlowFast Fast stem (5x7x7, 3 -> 8) at batch 1, 2 and 8, on 32 frames of 224^2.
 Prints the card name, power limit and max SM clock, then per route: us, GB/s of the algorithmic bytes (input + output
 + weights, f16) and the kernels launched.  Writes JSON to DIR/bench_stem.json when --out is given.
 """
@@ -33,9 +33,9 @@ SHAPES = {
     "fast_stem_b2": (2, 8, (5, 7, 7), (1, 2, 2), (2, 3, 3)),
     "fast_stem_b8": (8, 8, (5, 7, 7), (1, 2, 2), (2, 3, 3)),
 }
-ROUTES = {   # route: routing switches set while the plan is built
-    "stream": {},
-    "factored": {"PVB200_NO_STEMSTREAM": "1"},
+ROUTES = {   # route: the SM count (plan.H100_SXM_SMS) the plan is built with
+    "stream": 1,
+    "factored": 1 << 30,
 }
 T, HW = 32, 224
 
@@ -54,19 +54,14 @@ def build(shape, route, x, w, launches, dev, stream):
     """(graph of `launches` x the route's conv launches, op names, kernels launched by one run) or None when the route
     does not apply to the shape (the stream kernel below its threshold or outside its scope)."""
     _, co, k, s, p = shape
-    saved = os.environ.pop("PVB200_NO_STEMSTREAM", None)
-    os.environ.update(ROUTES[route])
     threshold = PL.H100_SXM_SMS
-    PL.H100_SXM_SMS = 1          # the stream route at every batch, below its routing threshold too (the crossover)
+    PL.H100_SXM_SMS = ROUTES[route]
     try:
         plan = Plan(dev, L.PV_F16)
         xr = plan.emit_input_ncdhw(x, 3, 4)
         plan.emit_conv(xr, w, None, None, s, p, (1, 1, 1), 1, L.ACT_RELU, None, "stem")
     finally:
         PL.H100_SXM_SMS = threshold
-        os.environ.pop("PVB200_NO_STEMSTREAM", None)
-        if saved is not None:
-            os.environ["PVB200_NO_STEMSTREAM"] = saved
     conv_ops = [(n, fn) for n, fn in plan.ops if n.startswith("stem")]
     names = [n for n, _ in conv_ops]
     if (route == "stream") != (plan.stats.get("stem_stream") == 1) or names == ["stem"]:

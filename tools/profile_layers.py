@@ -59,7 +59,7 @@ def device_info():
 
 def build(dev, xs, co, k, s, p, use_res, name):
     g = torch.Generator().manual_seed(0)
-    plan = Plan(dev, L.PV_F16, True)
+    plan = Plan(dev, L.PV_F16)
     x = torch.randn(xs, generator=g).to(dev)
     xr = plan.emit_input_ncdhw(x, xs[1], 4 if xs[1] <= 4 else xs[1])
     w = torch.randn(co, xs[1], *k, generator=g) * (2.0 / (xs[1] * k[0] * k[1] * k[2])) ** 0.5
