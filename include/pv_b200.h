@@ -734,6 +734,89 @@ int pv_colorjitter_apply(const pv_colorjitter_desc* d, const void* src, const in
                          const pv_cj_view* views, const unsigned long long* sums, uint8_t* dst, void* stream);
 int pv_colorjitter_vblur(const pv_colorjitter_desc* d, const pv_cj_view* views, uint8_t* dst, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Baseline JPEG decode (csrc/pv_jpeg.cu), data/frame_video.py:242-245 (cv2.imdecode(IMREAD_COLOR) + BGR2RGB): the
+ * bytes libjpeg's default decode gives - ISLOW integer IDCT with its range-limit table and 10-bit wrap, fancy
+ * (triangle) upsampling with replicated edge rows / columns (plain replication when the chroma plane is at most 2
+ * samples wide, as libjpeg does), integer YCbCr->RGB tables, grayscale replicated to three channels.
+ *
+ * pv_jpeg_parse  : host only.  Parses one stream (SOI, DQT, SOF0/SOF1 8-bit, DHT, SOS, DRI; APPn/COM and fill bytes
+ *                  skipped), builds its Huffman lookup tables and appends it to *batch: frame->data_off is where the
+ *                  caller must place the stream in the batch's data buffer, frame->out_off where its (H, W, 3) output
+ *                  goes in out (elements), and the byte ranges [begin, end) of its sequential segments (restart
+ *                  intervals, or the whole scan) are written as uint32 pairs, stream-relative, to
+ *                  segs[2 * batch->n_segments ...] (capacity seg_cap pairs).  On error nothing of *batch changes.
+ *                  Rejects with its own code each class below; malformed or truncated headers and a scan that runs
+ *                  off the buffer are PV_ERR_INVALID.  PV_ERR_UNSUPPORTED: Huffman table slots 2 and 3 (SOF1 allows
+ *                  four; baseline files use 0 and 1), and frames of more than 2^31 - 1 pixels.
+ * pv_jpeg_decode : three launches on `stream` for every frame of the batch: entropy decode (one single-warp CTA per
+ *                  segment, int16 coefficients in natural order), dequantise + ISLOW IDCT into per-component uint8 planes,
+ *                  and upsample + YCbCr->RGB into out (uint8 or fp32, (H, W, 3) per frame at frames[i].out_off), one
+ *                  launch per sampling mode present.  frames, segs, data and status are DEVICE arrays (frames and
+ *                  segs as parse wrote them, data holding each stream at its data_off); batch is the host struct.
+ *                  status[i] is zeroed by the call and set to PV_JPEG_BAD_* bits when frame i's entropy data is
+ *                  corrupt (its output is then unspecified, but every read and write stays inside its ranges).
+ *                  workspace: batch->ws_bytes bytes, 16-byte aligned.                                            */
+typedef enum pv_jpeg_error {
+  PV_JPEG_ERR_PROGRESSIVE = -20,
+  PV_JPEG_ERR_ARITHMETIC = -21,
+  PV_JPEG_ERR_LOSSLESS = -22,
+  PV_JPEG_ERR_HIERARCHICAL = -23,
+  PV_JPEG_ERR_PRECISION = -24,     /* sample precision other than 8 bits                                       */
+  PV_JPEG_ERR_COMPONENTS = -25,    /* 2 or more than 4 components                                               */
+  PV_JPEG_ERR_COLORSPACE = -26,    /* CMYK / YCCK (4 components), an Adobe transform other than YCbCr, RGB ids */
+  PV_JPEG_ERR_ORIENTATION = -27,   /* EXIF orientation other than 1 (IMREAD_COLOR would rotate)                */
+  PV_JPEG_ERR_MULTISCAN = -28,     /* more than one scan                                                       */
+  PV_JPEG_ERR_DNL = -29,           /* height given by a DNL marker                                             */
+  PV_JPEG_ERR_SAMPLING = -30       /* chroma sampling other than 1x1, 2x1, 1x2, 2x2 of the luma grid           */
+} pv_jpeg_error;
+
+#define PV_JPEG_BAD_CODE 1       /* status bit: a Huffman code absent from its table, or an AC run past 63     */
+#define PV_JPEG_BAD_OVERRUN 2    /* status bit: a segment's codes need more bits than it holds                */
+#define PV_JPEG_BAD_RESTART 4    /* status bit: RSTn out of sequence                                          */
+
+typedef enum pv_jpeg_mode { PV_JPEG_GRAY = 0, PV_JPEG_H1V1 = 1, PV_JPEG_H2V1 = 2, PV_JPEG_H1V2 = 3, PV_JPEG_H2V2 = 4 } pv_jpeg_mode;
+
+typedef struct pv_jpeg_huff {
+  uint16_t look[512];                /* (length << 8) | symbol of every code of <= 9 bits by its 9-bit prefix, else 0 */
+  int32_t maxcode[18];               /* largest code of each length, -1 if none; [17] is a sentinel                  */
+  int32_t valoff[18];                /* symbol index minus code, per length                                          */
+  uint8_t val[256];
+} pv_jpeg_huff;
+
+typedef struct pv_jpeg_frame {
+  int width, height, ncomp, mode;    /* mode: pv_jpeg_mode                                                       */
+  int mcus_x, mcus_y, restart_interval, n_segments;
+  int n_blocks;                      /* 8x8 blocks of all components (padded to whole MCUs)                      */
+  int scan_comp[3];                  /* SOF index of the scan's components, in scan order                         */
+  int h[3], v[3];                    /* sampling factors, SOF order (1 for a grayscale frame)                      */
+  int bw[3], bh[3];                  /* block grid of each component                                               */
+  int dw[3], dh[3];                  /* real sample width / height of each component                               */
+  int block_off[3];                  /* first block of each component within the frame                             */
+  int dc_tbl[3], ac_tbl[3];          /* Huffman table slot of each component (0 | 1)                               */
+  long long data_off;                /* the stream's first byte in the batch data buffer                          */
+  long long seg_base;                /* first segment pair in segs                                                 */
+  long long block_base;              /* first block in the workspace                                               */
+  long long out_off;                 /* first output element                                                       */
+  uint16_t qt[3][64];                /* quantisation table of each component, natural order                        */
+  pv_jpeg_huff dc[2], ac[2];
+} pv_jpeg_frame;
+
+typedef struct pv_jpeg_batch {
+  int n_frames;
+  int mode_mask;                     /* 1 << pv_jpeg_mode of every frame                                         */
+  int max_blocks, max_pixels;        /* largest n_blocks, largest width * height                                   */
+  long long n_segments, n_blocks;
+  long long data_bytes;              /* bytes of all streams                                                       */
+  long long out_elems;               /* 3 * sum of width * height                                                  */
+  long long ws_bytes;                /* workspace of pv_jpeg_decode: 192 bytes per block                           */
+} pv_jpeg_batch;
+
+int pv_jpeg_parse(const uint8_t* data, long long len, pv_jpeg_batch* batch, pv_jpeg_frame* frame, uint32_t* segs,
+                  long long seg_cap);
+int pv_jpeg_decode(const pv_jpeg_batch* batch, const pv_jpeg_frame* frames, const uint32_t* segs, const uint8_t* data,
+                   void* workspace, long long workspace_bytes, void* out, int out_dtype, int* status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

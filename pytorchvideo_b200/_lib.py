@@ -85,6 +85,34 @@ class ColorJitterDesc(C.Structure):
                 ("src_dtype", C.c_int), ("src_scale", C.c_int)]
 
 
+JPEG_GRAY, JPEG_H1V1, JPEG_H2V1, JPEG_H1V2, JPEG_H2V2 = 0, 1, 2, 3, 4     # pv_jpeg_mode
+JPEG_BAD_CODE, JPEG_BAD_OVERRUN, JPEG_BAD_RESTART = 1, 2, 4             # pv_jpeg_decode status bits
+# pv_jpeg_parse's rejections, by code
+JPEG_ERRORS = {-20: "progressive", -21: "arithmetic", -22: "lossless", -23: "hierarchical", -24: "precision",
+               -25: "components", -26: "colorspace", -27: "orientation", -28: "multiscan", -29: "dnl", -30: "sampling"}
+
+
+class JpegHuff(C.Structure):
+    _fields_ = [("look", C.c_uint16 * 512), ("maxcode", C.c_int32 * 18), ("valoff", C.c_int32 * 18),
+                ("val", C.c_uint8 * 256)]
+
+
+class JpegFrame(C.Structure):
+    _fields_ = [("width", C.c_int), ("height", C.c_int), ("ncomp", C.c_int), ("mode", C.c_int),
+                ("mcus_x", C.c_int), ("mcus_y", C.c_int), ("restart_interval", C.c_int), ("n_segments", C.c_int),
+                ("n_blocks", C.c_int), ("scan_comp", C.c_int * 3), ("h", C.c_int * 3), ("v", C.c_int * 3),
+                ("bw", C.c_int * 3), ("bh", C.c_int * 3), ("dw", C.c_int * 3), ("dh", C.c_int * 3),
+                ("block_off", C.c_int * 3), ("dc_tbl", C.c_int * 3), ("ac_tbl", C.c_int * 3),
+                ("data_off", c_ll), ("seg_base", c_ll), ("block_base", c_ll), ("out_off", c_ll),
+                ("qt", (C.c_uint16 * 64) * 3), ("dc", JpegHuff * 2), ("ac", JpegHuff * 2)]
+
+
+class JpegBatch(C.Structure):
+    _fields_ = [("n_frames", C.c_int), ("mode_mask", C.c_int), ("max_blocks", C.c_int), ("max_pixels", C.c_int),
+                ("n_segments", c_ll), ("n_blocks", c_ll), ("data_bytes", c_ll), ("out_elems", c_ll),
+                ("ws_bytes", c_ll)]
+
+
 class BottleneckDesc(C.Structure):
     _fields_ = [("N", C.c_int), ("T", C.c_int), ("H", C.c_int), ("W", C.c_int),
                 ("Cin", C.c_int), ("Cmid", C.c_int), ("Cout", C.c_int), ("kt", C.c_int), ("sb", C.c_int),
@@ -219,6 +247,8 @@ SIGNATURES = {
     "pv_bank_update": (C.c_int, [c_vp, c_ll, C.c_int, c_vp, c_vp, c_ll, C.c_int, C.c_float, C.c_float, c_vp, c_vp]),
     "pv_queue_ce": (C.c_int, [c_vp, c_ll, C.c_int, C.c_int, c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_ll,
                               C.c_int, C.c_float, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp]),
+    "pv_jpeg_parse": (C.c_int, [c_vp, c_ll, C.POINTER(JpegBatch), C.POINTER(JpegFrame), c_vp, c_ll]),
+    "pv_jpeg_decode": (C.c_int, [C.POINTER(JpegBatch), c_vp, c_vp, c_vp, c_vp, c_ll, c_vp, C.c_int, c_vp, c_vp]),
 }
 
 _lib = None
