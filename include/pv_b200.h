@@ -141,6 +141,20 @@ int pv_clip_transform_batch(const pv_clip_batch_desc* d, const void* src, const 
 int pv_clip_transform_rrc(const pv_clip_batch_desc* d, const void* src, const int32_t* idx_t, const int32_t* boxes,
                           void* dst, void* stream);
 
+/* Ragged mode of the batched chain: the output of pv_clip_transform_batch, but every clip reads its own frames, of
+ * its own size (a batch of frame-folder videos of mixed resolutions, decoded by pv_jpeg_decode into one buffer).
+ * Kept frame j of clip b is a packed HWC frame of C channels, in_h[b] x in_w[b], starting at element
+ * frame_off[b * n_t + j] of src (temporal selection is done in frame_off; an entry may repeat).  geom is a DEVICE int32
+ * array of {in_h, in_w, new_h, new_w, top, left, hflip} per clip and geom_host the same table in host memory, which the
+ * call validates; frame_off is a DEVICE int64 array whose frames the caller keeps inside src.  slow_pos / dst_slow,
+ * mean / stdv / div255 / normalize, out_h / out_w, n_slow, d_clip and d_slow_clip are read as pv_clip_transform_batch
+ * reads them; in_h / in_w / new_h / new_w / top / left / hflip and the source strides of the descriptor are ignored.
+ * C must be 3; src PV_U8 or PV_F32, dst PV_F16 or PV_F32.  PV_ERR_INVALID for an empty batch, a frame of
+ * in_h * in_w * C >= 2^31 elements, or a window outside its resized frame.  One launch.                        */
+int pv_clip_transform_ragged(const pv_clip_batch_desc* d, const void* src, const long long* frame_off,
+                             const int32_t* geom, const int32_t* geom_host, const int32_t* slow_pos, void* dst,
+                             void* dst_slow, void* stream);
+
 /* Detection boxes of the batched chain (transforms/functional.py:195-445: short_side_scale_with_boxes,
  * random_crop_with_boxes, uniform_crop_with_boxes, horizontal_flip_with_boxes, clip_boxes_to_image, crop_boxes).
  * Clip b owns boxes box_start[b] .. box_start[b+1]-1 of the (n_boxes, 4) array of (x1, y1, x2, y2); box_start is a

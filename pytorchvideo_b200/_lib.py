@@ -168,6 +168,7 @@ SIGNATURES = {
                                         c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_clip_transform_batch": (C.c_int, [C.POINTER(ClipBatchDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_clip_transform_rrc": (C.c_int, [C.POINTER(ClipBatchDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_clip_transform_ragged": (C.c_int, [C.POINTER(ClipBatchDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_clip_boxes_transform": (C.c_int, [C.POINTER(BoxesDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_augment_stats": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, c_vp]),
     "pv_augment_apply": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),

@@ -122,11 +122,13 @@ constexpr int TB_THREADS = 256;
 
 // RRC (RandomResizedCrop mode, pv_clip_transform_rrc): geom holds one {top, left, h, w, hflip} source window per
 // (clip, kept frame); the taps are ATen's for an h x w -> out_h x out_w resize, offset by the window origin.
+// Ragged mode (pv_clip_transform_ragged), selected at run time by a non-null frame_off: kept frame j of clip b is a
+// packed HWC frame at src + frame_off[b * n_t + j], and geom holds {in_h, in_w, new_h, new_w, top, left, hflip} per clip.
 template <typename SrcT, typename OutT, int NC, bool LUT, bool RRC>
 __device__ __forceinline__ void
 clip_transform_batch_body(const pv_clip_batch_desc& d, const SrcT* __restrict__ src, const int32_t* __restrict__ idx_t,
                           const int32_t* __restrict__ slow_pos, const int32_t* __restrict__ geom,
-                          OutT* __restrict__ dst, OutT* __restrict__ dst_slow) {
+                          const long long* __restrict__ frame_off, OutT* __restrict__ dst, OutT* __restrict__ dst_slow) {
   constexpr int PX = 2;
   __shared__ float lut[LUT ? NC * 256 : 1];
   if constexpr (LUT) {
@@ -143,29 +145,36 @@ clip_transform_batch_body(const pv_clip_batch_desc& d, const SrcT* __restrict__ 
   int new_h = d.new_h, new_w = d.new_w, top = d.top, left = d.left, flip = d.hflip;
   int t_off = 0;
   int win_h = 0, win_w = 0;                 // RRC source window size
+  int in_h = d.in_h, in_w = d.in_w;
+  unsigned sh = (unsigned)d.sh, sw = (unsigned)d.sw;
   if constexpr (RRC) {          // per-(clip, frame) source window
     const int32_t* g = geom + 5 * blockIdx.z;
     top = __ldg(g); left = __ldg(g + 1); win_h = __ldg(g + 2); win_w = __ldg(g + 3); flip = __ldg(g + 4);
     new_h = d.out_h; new_w = d.out_w;
+  } else if (frame_off != nullptr) {   // ragged: per-clip source size and geometry, packed HWC frames
+    const int32_t* g = geom + 7 * clip;
+    in_h = __ldg(g); in_w = __ldg(g + 1); new_h = __ldg(g + 2); new_w = __ldg(g + 3);
+    top = __ldg(g + 4); left = __ldg(g + 5); flip = __ldg(g + 6);
+    sw = NC; sh = (unsigned)(NC * in_w);
   } else if (geom != nullptr) {        // per-clip (new_h, new_w, top, left, hflip, first frame)
     const int32_t* g = geom + 6 * clip;
     new_h = __ldg(g); new_w = __ldg(g + 1); top = __ldg(g + 2); left = __ldg(g + 3); flip = __ldg(g + 4);
     t_off = __ldg(g + 5);
   }
   // block-uniform channel planes of this (clip, frame); everything per thread below is a 32-bit offset into them
-  // (the host checks in_h*|sh| + in_w*|sw| < 2^31)
+  // (the host checks in_h*|sh| + in_w*|sw| < 2^31, and in_h*in_w*NC < 2^31 for a ragged frame)
   const SrcT* cbase[NC];
+  const SrcT* fbase = frame_off != nullptr ? src + __ldg(frame_off + blockIdx.z)
+                                           : src + (long long)clip * d.s_clip + (long long)(__ldg(idx_t + j) + t_off) * d.st;
 #pragma unroll
-  for (int c = 0; c < NC; ++c)
-    cbase[c] = src + (long long)clip * d.s_clip + (long long)(__ldg(idx_t + j) + t_off) * d.st + (long long)c * d.sc;
+  for (int c = 0; c < NC; ++c) cbase[c] = fbase + (frame_off != nullptr ? (long long)c : (long long)c * d.sc);
   const int sp = slow_pos != nullptr ? __ldg(slow_pos + j) : -1;
   const int half_w = (d.out_w + PX - 1) / PX;
   const int y_base = blockIdx.y * TB_ROWS;
   const int n_rows = min(TB_ROWS, d.out_h - y_base);
   const int plane = d.out_h * d.out_w;                 // host checks C*n_t*plane < 2^31
-  const unsigned sh = (unsigned)d.sh, sw = (unsigned)d.sw;
-  const float scale_y = RRC ? bilinear_scale(win_h, new_h) : bilinear_scale(d.in_h, new_h);
-  const float scale_x = RRC ? bilinear_scale(win_w, new_w) : bilinear_scale(d.in_w, new_w);
+  const float scale_y = RRC ? bilinear_scale(win_h, new_h) : bilinear_scale(in_h, new_h);
+  const float scale_x = RRC ? bilinear_scale(win_w, new_w) : bilinear_scale(in_w, new_w);
   OutT* const dclip = dst + (long long)clip * d.d_clip + (long long)j * plane;
   OutT* const sclip = sp >= 0 ? dst_slow + (long long)clip * d.d_slow_clip + (long long)sp * plane : nullptr;
   const int cstep = d.n_t * plane, cstep_slow = d.n_slow * plane;
@@ -185,14 +194,14 @@ clip_transform_batch_body(const pv_clip_batch_desc& d, const SrcT* __restrict__ 
         lx1[i] = t.l1; lx0[i] = 1.f - t.l1;
         continue;
       }
-      const TapXY t = bilinear_tap(left + (flip ? d.out_w - 1 - xo : xo), d.in_w, scale_x);
+      const TapXY t = bilinear_tap(left + (flip ? d.out_w - 1 - xo : xo), in_w, scale_x);
       xo0[i] = t.i0 * sw; xo1[i] = t.i1 * sw;
       lx1[i] = t.l1; lx0[i] = 1.f - t.l1;
     }
     const bool two = (xb + 1 < d.out_w);
     for (int r = threadIdx.y; r < n_rows; r += blockDim.y) {
       const int y = y_base + r;
-      const TapXY ty = RRC ? bilinear_tap(y, win_h, scale_y) : bilinear_tap(top + y, d.in_h, scale_y);
+      const TapXY ty = RRC ? bilinear_tap(y, win_h, scale_y) : bilinear_tap(top + y, in_h, scale_y);
       const float ly1 = ty.l1, ly0 = 1.f - ly1;
       const unsigned ro0 = ((RRC ? top : 0) + ty.i0) * sh, ro1 = ((RRC ? top : 0) + ty.i1) * sh;
       unsigned off[PX][4];
@@ -250,15 +259,15 @@ template <typename SrcT, typename OutT, int NC, bool LUT>
 __global__ void __launch_bounds__(TB_THREADS)
 clip_transform_batch_kernel(pv_clip_batch_desc d, const SrcT* __restrict__ src, const int32_t* __restrict__ idx_t,
                             const int32_t* __restrict__ slow_pos, const int32_t* __restrict__ geom,
-                            OutT* __restrict__ dst, OutT* __restrict__ dst_slow) {
-  clip_transform_batch_body<SrcT, OutT, NC, LUT, false>(d, src, idx_t, slow_pos, geom, dst, dst_slow);
+                            const long long* __restrict__ frame_off, OutT* __restrict__ dst, OutT* __restrict__ dst_slow) {
+  clip_transform_batch_body<SrcT, OutT, NC, LUT, false>(d, src, idx_t, slow_pos, geom, frame_off, dst, dst_slow);
 }
 
 template <typename SrcT, typename OutT, bool LUT>
 __global__ void __launch_bounds__(TB_THREADS)
 clip_transform_rrc_kernel(pv_clip_batch_desc d, const SrcT* __restrict__ src, const int32_t* __restrict__ idx_t,
                           const int32_t* __restrict__ boxes, OutT* __restrict__ dst) {
-  clip_transform_batch_body<SrcT, OutT, 3, LUT, true>(d, src, idx_t, nullptr, boxes, dst, nullptr);
+  clip_transform_batch_body<SrcT, OutT, 3, LUT, true>(d, src, idx_t, nullptr, boxes, nullptr, dst, nullptr);
 }
 
 }  // namespace pv
@@ -324,6 +333,11 @@ extern "C" int pv_view_reduce(const float* preds, float* out, int n_videos, int 
   return PV_OK;
 }
 
+namespace pv {
+static int launch_clip_batch(const pv_clip_batch_desc* d, const void* src, const int32_t* idx_t, const int32_t* slow_pos,
+                             const int32_t* geom, const long long* frame_off, void* dst, void* dst_slow, cudaStream_t s);
+}  // namespace pv
+
 extern "C" int pv_clip_transform_batch(const pv_clip_batch_desc* d, const void* src, const int32_t* idx_t,
                                        const int32_t* slow_pos, const int32_t* geom, void* dst, void* dst_slow,
                                        void* stream) {
@@ -338,23 +352,29 @@ extern "C" int pv_clip_transform_batch(const pv_clip_batch_desc* d, const void* 
   const bool pass = d->dst_dtype == PV_U8;
   PV_CHECK_ARG(!pass || (d->src_dtype == PV_U8 && !d->div255 && !d->normalize && geom == nullptr && d->new_h == d->in_h && d->new_w == d->in_w),
                "uint8 output is a pure frame selection / crop (no resize, no arithmetic)");
-  cudaStream_t s = (cudaStream_t)stream;
-  const int half_w = (d->out_w + 1) / 2;
-  const unsigned bx = (unsigned)(half_w >= pv::TB_THREADS ? pv::TB_THREADS : half_w);
-  const unsigned by = (unsigned)(pv::TB_THREADS / bx >= pv::TB_ROWS ? pv::TB_ROWS : (pv::TB_THREADS / bx < 1 ? 1 : pv::TB_THREADS / bx));
-  dim3 grid(1, (unsigned)pv::cdiv(d->out_h, pv::TB_ROWS), d->n_clips * d->n_t), block(bx, by);
-  PV_CHECK_ARG(grid.y <= 65535, "grid too large");
   auto absll = [](long long v) { return v < 0 ? -v : v; };
   PV_CHECK_ARG((long long)d->in_h * absll(d->sh) + (long long)d->in_w * absll(d->sw) < (1ll << 31) && d->sh >= 0 && d->sw >= 0,
                "frame too large for 32-bit in-plane offsets");
   PV_CHECK_ARG((long long)d->C * (d->n_t > d->n_slow ? d->n_t : d->n_slow) * d->out_h * d->out_w < (1ll << 31),
                "output clip too large for 32-bit offsets");
+  return pv::launch_clip_batch(d, src, idx_t, slow_pos, geom, nullptr, dst, dst_slow, (cudaStream_t)stream);
+}
+
+namespace pv {
+// grid and instance selection shared by the per-batch and ragged entry points; frame_off selects the ragged mode
+static int launch_clip_batch(const pv_clip_batch_desc* d, const void* src, const int32_t* idx_t, const int32_t* slow_pos,
+                             const int32_t* geom, const long long* frame_off, void* dst, void* dst_slow, cudaStream_t s) {
+  const int half_w = (d->out_w + 1) / 2;
+  const unsigned bx = (unsigned)(half_w >= pv::TB_THREADS ? pv::TB_THREADS : half_w);
+  const unsigned by = (unsigned)(pv::TB_THREADS / bx >= pv::TB_ROWS ? pv::TB_ROWS : (pv::TB_THREADS / bx < 1 ? 1 : pv::TB_THREADS / bx));
+  dim3 grid(1, (unsigned)pv::cdiv(d->out_h, pv::TB_ROWS), d->n_clips * d->n_t), block(bx, by);
+  PV_CHECK_ARG(grid.y <= 65535, "grid too large");
   const bool arith = d->div255 || d->normalize;
   // LUT instances exist only for a uint8 source with a float destination (the uint8 pass-through has no arithmetic)
 #define PV_TB_LAUNCH(ST, OT, NC, LUT)                                                                                  \
   do {                                                                                                                 \
     pv::clip_transform_batch_kernel<ST, OT, NC, LUT><<<grid, block, 0, s>>>(*d, (const ST*)src, idx_t, slow_pos, geom, \
-                                                                           (OT*)dst, (OT*)dst_slow);                   \
+                                                                           frame_off, (OT*)dst, (OT*)dst_slow);        \
     PV_LAUNCH_OK("clip_transform_batch_kernel<" #ST "," #OT "," #NC "," #LUT ">");                                    \
   } while (0)
 #define PV_TB(ST, OT, NC)                                                                                              \
@@ -394,6 +414,30 @@ extern "C" int pv_clip_transform_batch(const pv_clip_batch_desc* d, const void* 
 #undef PV_TB
 #undef PV_TB_LAUNCH
   return PV_OK;
+}
+}  // namespace pv
+
+extern "C" int pv_clip_transform_ragged(const pv_clip_batch_desc* d, const void* src, const long long* frame_off,
+                                        const int32_t* geom, const int32_t* geom_host, const int32_t* slow_pos,
+                                        void* dst, void* dst_slow, void* stream) {
+  PV_CHECK_ARG(d && src && frame_off && geom && geom_host && dst, "null argument");
+  PV_CHECK_ARG(d->C == 3, "ragged mode needs 3 channels (got %d)", d->C);
+  PV_CHECK_ARG(d->n_clips >= 1 && d->n_t >= 1 && d->out_h >= 1 && d->out_w >= 1, "empty batch");
+  PV_CHECK_ARG((long long)d->n_clips * d->n_t <= 65535, "grid too large");
+  PV_CHECK_ARG(d->src_dtype == PV_U8 || d->src_dtype == PV_F32, "ragged mode reads uint8 or f32 frames");
+  PV_CHECK_ARG(d->dst_dtype == PV_F16 || d->dst_dtype == PV_F32, "ragged mode writes f16 or f32");
+  PV_CHECK_ARG((slow_pos == nullptr) == (dst_slow == nullptr) && (slow_pos == nullptr || d->n_slow >= 1), "slow pathway arguments");
+  PV_CHECK_ARG((long long)d->C * (d->n_t > d->n_slow ? d->n_t : d->n_slow) * d->out_h * d->out_w < (1ll << 31),
+               "output clip too large for 32-bit offsets");
+  for (int b = 0; b < d->n_clips; ++b) {
+    const int32_t* g = geom_host + 7 * b;
+    PV_CHECK_ARG(g[0] >= 1 && g[1] >= 1 && g[2] >= 1 && g[3] >= 1, "clip %d: bad frame size", b);
+    PV_CHECK_ARG((long long)g[0] * g[1] * d->C < (1ll << 31), "clip %d: %dx%d frame too large for 32-bit in-frame offsets",
+                 b, g[1], g[0]);
+    PV_CHECK_ARG(g[4] >= 0 && g[5] >= 0 && (long long)g[4] + d->out_h <= g[2] && (long long)g[5] + d->out_w <= g[3],
+                 "clip %d: crop window outside the resized frame", b);
+  }
+  return pv::launch_clip_batch(d, src, nullptr, slow_pos, geom, frame_off, dst, dst_slow, (cudaStream_t)stream);
 }
 
 extern "C" int pv_clip_transform_rrc(const pv_clip_batch_desc* d, const void* src, const int32_t* idx_t,

@@ -14,7 +14,7 @@ import math
 import os
 import re
 from concurrent.futures import ThreadPoolExecutor
-from typing import Callable, Dict, List, Optional
+from typing import Callable, Dict, List, NamedTuple, Optional
 
 import torch
 
@@ -37,6 +37,15 @@ def clip_frame_indices(fps: float, duration: float, n_frames: int, start_sec: fl
     first = math.ceil(fps * start_sec)
     stop = min(math.ceil(fps * min(end_sec, duration)), n_frames)
     return list(range(first, stop))
+
+
+class ClipFrames(NamedTuple):
+    """A clip's frames as file bytes, not decoded: what a DataLoader worker can produce without the GPU."""
+
+    data: List[bytes]            # file bytes of each kept frame, in clip order (a repeated frame repeats its bytes)
+    paths: List[str]             # file of each kept frame
+    frame_indices: List[int]     # the clip's frame indices, as get_clip returns them
+    kept: List[int]              # the positions in frame_indices that data and paths hold
 
 
 class FrameVideo:
@@ -122,6 +131,27 @@ class FrameVideo:
         files = _read_all([self._frame_path(i) for i in indices], self._multithreaded_io)
         thwc = decode_jpeg_frames(files, out_dtype=torch.float32)
         return {"video": thwc.permute(3, 0, 1, 2), "frame_indices": indices, "audio": None}
+
+    def get_clip_frames(self, start_sec: float, end_sec: float, frame_filter: Optional[FrameFilter] = None,
+                        keep: Optional[Callable[[int], List[int]]] = None) -> Optional[ClipFrames]:
+        """The clip get_clip would load, as the files' bytes: reads, never decodes, so it runs on any host process.
+
+        ``keep`` maps the clip's frame count to the positions to read (a temporal subsample), so frames a transform
+        would drop are not read; by default every frame is.  Returns None, or raises ValueError, where get_clip does.
+        """
+        indices = self.frame_indices(start_sec, end_sec, frame_filter)
+        if indices is None:
+            return None
+        if not indices:
+            raise ValueError("FrameVideo %s: no frame to load for [%s, %s) s" % (self._name, start_sec, end_sec))
+        kept = list(range(len(indices))) if keep is None else [int(k) for k in keep(len(indices))]
+        paths = [self._frame_path(indices[k]) for k in kept]
+        unique = list(dict.fromkeys(paths))
+        read = dict(zip(unique, _read_all(unique, self._multithreaded_io)))
+        return ClipFrames([read[p] for p in paths], paths, indices, kept)
+
+    def close(self) -> None:
+        """Nothing to release: a frame video holds no open file."""
 
     def _frame_path(self, index: int) -> str:
         if self._path_fn is not None:

@@ -24,9 +24,9 @@ def _as_bytes(frame):
     raise RuntimeError("a frame must be bytes or a 1-D uint8 tensor, got %s" % type(frame).__name__)
 
 
-def _parse_error(i, rc):
+def _parse_error(name, rc):
     kind = L.JPEG_ERRORS.get(rc, "invalid" if rc == -1 else "unsupported" if rc == -3 else "status %d" % rc)
-    return RuntimeError("frame %d: JPEG rejected (%s): %s" % (i, kind, L.last_error()))
+    return RuntimeError("%s: JPEG rejected (%s): %s" % (name, kind, L.last_error()))
 
 
 def parse_jpeg(data):
@@ -41,13 +41,14 @@ def parse_jpeg(data):
     return rc, frame, batch, [(int(segs[2 * k]), int(segs[2 * k + 1])) for k in range(n)]
 
 
-def decode_batch(frames, out=None, out_dtype=torch.uint8, same_size=False, out_shape=None):
+def decode_batch(frames, out=None, out_dtype=torch.uint8, same_size=False, out_shape=None, names=None):
     """Decode JPEG streams of any sizes with one host-to-device copy and one launch sequence.
 
     Returns (out, [(H, W) per frame]); out is flat and holds frame i's (H, W, 3) pixels right after frame i-1's.
     ``out`` may be given as a contiguous CUDA tensor of out_dtype with exactly that many elements.  same_size
     raises on the first frame whose size differs from frame 0's; with it, out_shape (the caller's view of out) must be
-    (N, H, W, 3) of the parsed frames, checked before anything is written.
+    (N, H, W, 3) of the parsed frames, checked before anything is written.  Errors name frame i as names[i] when
+    ``names`` is given (e.g. the file paths), else as "frame i".
     """
     if out_dtype not in (torch.uint8, torch.float32):
         raise RuntimeError("out_dtype must be torch.uint8 or torch.float32")
@@ -81,7 +82,7 @@ def decode_batch(frames, out=None, out_dtype=torch.uint8, same_size=False, out_s
             rc = lib.pv_jpeg_parse(base + batch.data_bytes, b.size, C.byref(batch), C.byref(farr[i]),
                                    base + segs_off, cap)
             if rc != 0:
-                raise _parse_error(i, rc)
+                raise _parse_error(names[i] if names is not None else "frame %d" % i, rc)
             sizes.append((farr[i].height, farr[i].width))
             if same_size and sizes[i] != sizes[0]:
                 raise RuntimeError("frame %d is %dx%d, frame 0 is %dx%d: all frames must share one size"
@@ -109,7 +110,8 @@ def decode_batch(frames, out=None, out_dtype=torch.uint8, same_size=False, out_s
         s = int(status[bad[0]])
         why = [w for bit, w in ((L.JPEG_BAD_CODE, "bad Huffman code"), (L.JPEG_BAD_OVERRUN, "entropy data overrun"),
                                 (L.JPEG_BAD_RESTART, "restart marker out of sequence")) if s & bit]
-        raise RuntimeError("frame %d: corrupt JPEG entropy data (%s)" % (bad[0], ", ".join(why)))
+        name = names[bad[0]] if names is not None else "frame %d" % bad[0]
+        raise RuntimeError("%s: corrupt JPEG entropy data (%s)" % (name, ", ".join(why)))
     return out, sizes
 
 

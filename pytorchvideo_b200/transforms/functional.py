@@ -193,6 +193,33 @@ def slow_pathway_indices(n_frames, alpha):
     return torch.linspace(0, n_frames - 1, n_frames // alpha).long()
 
 
+def _set_arith(d, Cc, mean, std, div255):
+    """The /255 and normalisation fields of a ClipBatchDesc; one mean / std value stands for every channel."""
+    normalize = mean is not None or std is not None
+    mean_l = [float(m) for m in (mean if mean is not None else [0.0] * Cc)]
+    std_l = [float(v) for v in (std if std is not None else [1.0] * Cc)]
+    mean_l = mean_l * Cc if len(mean_l) == 1 else mean_l
+    std_l = std_l * Cc if len(std_l) == 1 else std_l
+    for i in range(4):
+        d.mean[i] = mean_l[i] if i < len(mean_l) else 0.0
+        d.stdv[i] = std_l[i] if i < len(std_l) else 1.0
+    d.div255, d.normalize = 1 if div255 else 0, 1 if normalize else 0
+
+
+def _slow_table(n_t, slow_alpha, dev):
+    """(device slot of each kept frame in the slow pathway or -1, slow frame count)."""
+    sidx = slow_pathway_indices(n_t, int(slow_alpha)).tolist()
+    n_slow = len(sidx)
+    if n_slow < 1:
+        raise RuntimeError("slow pathway would be empty (n_t=%d, alpha=%d)" % (n_t, slow_alpha))
+    pos = [-1] * n_t
+    for k, j in enumerate(sidx):
+        pos[j] = k           # linspace().long() is strictly increasing for alpha >= 1: every slot is unique
+    if len(set(sidx)) != n_slow:
+        raise RuntimeError("slow pathway indices repeat (alpha < 1?)")
+    return _dev_i32(pos, dev), n_slow
+
+
 def clip_transform_batch(x, frame_idx=None, resize_hw=None, window=None, mean=None, std=None, div255=False,
                          out_dtype=torch.float16, hflip=False, geom=None, slow_alpha=None, out=None, out_slow=None):
     """The fused chain on a BATCH of clips in one launch (pv_clip_transform_batch; taps computed in the kernel).
@@ -251,15 +278,7 @@ def clip_transform_batch(x, frame_idx=None, resize_hw=None, window=None, mean=No
     d.in_h, d.in_w, d.new_h, d.new_w = H, W, nh, nw
     d.top, d.left, d.out_h, d.out_w, d.hflip = top, left, oh, ow, 1 if hflip else 0
     d.s_clip, d.sc, d.st, d.sh, d.sw = x.stride(0), x.stride(1), x.stride(2), x.stride(3), x.stride(4)
-    normalize = mean is not None or std is not None
-    mean_l = [float(m) for m in (mean if mean is not None else [0.0] * Cc)]
-    std_l = [float(v) for v in (std if std is not None else [1.0] * Cc)]
-    mean_l = mean_l * Cc if len(mean_l) == 1 else mean_l
-    std_l = std_l * Cc if len(std_l) == 1 else std_l
-    for i in range(4):
-        d.mean[i] = mean_l[i] if i < len(mean_l) else 0.0
-        d.stdv[i] = std_l[i] if i < len(std_l) else 1.0
-    d.div255, d.normalize = 1 if div255 else 0, 1 if normalize else 0
+    _set_arith(d, Cc, mean, std, div255)
     d.src_dtype = _DT[x.dtype]
     if out_dtype not in _DT:
         raise RuntimeError("unsupported output dtype %s" % out_dtype)
@@ -272,16 +291,7 @@ def clip_transform_batch(x, frame_idx=None, resize_hw=None, window=None, mean=No
     idx_d = _dev_i32(idx.tolist(), dev)
     slow_d, n_slow = None, 0
     if slow_alpha is not None:
-        sidx = slow_pathway_indices(n_t, int(slow_alpha)).tolist()
-        n_slow = len(sidx)
-        if n_slow < 1:
-            raise RuntimeError("slow pathway would be empty (n_t=%d, alpha=%d)" % (n_t, slow_alpha))
-        pos = [-1] * n_t
-        for k, j in enumerate(sidx):
-            pos[j] = k           # linspace().long() is strictly increasing for alpha >= 1: every slot is unique
-        if len(set(sidx)) != n_slow:
-            raise RuntimeError("slow pathway indices repeat (alpha < 1?)")
-        slow_d = _dev_i32(pos, dev)
+        slow_d, n_slow = _slow_table(n_t, slow_alpha, dev)
         if out_slow is None:
             out_slow = torch.empty((B, Cc, n_slow, oh, ow), dtype=out_dtype, device=dev)
         elif tuple(out_slow.shape) != (B, Cc, n_slow, oh, ow) or not out_slow.is_contiguous() or out_slow.dtype != out_dtype:
@@ -297,6 +307,69 @@ def clip_transform_batch(x, frame_idx=None, resize_hw=None, window=None, mean=No
     if squeeze:
         out = out[0]
         out_slow = out_slow[0] if out_slow is not None else None
+    return [out_slow, out] if slow_alpha is not None else out
+
+
+def ragged_tables(frame_off, geom, out_hw):
+    """Host checks and the flat tables of a ragged launch: (int64 frame offsets, int32 geometry rows).
+
+    frame_off : (B, n_t) element offsets of each clip's kept frames in the source buffer
+    geom      : per clip (in_hw, resize_hw, window (top, left, out_h, out_w), hflip); every window is out_hw
+    """
+    offs = torch.as_tensor(frame_off, dtype=torch.int64)
+    if offs.dim() != 2 or offs.shape[0] == 0 or offs.shape[1] == 0:
+        raise RuntimeError("frame_off must be a non-empty (B, n_t) table")
+    if len(geom) != offs.shape[0]:
+        raise RuntimeError("geom needs one entry per clip (%d clips)" % offs.shape[0])
+    rows = []
+    for (ih, iw), (nh, nw), (top, left, oh, ow), flip in geom:
+        if (oh, ow) != tuple(out_hw):
+            raise RuntimeError("every crop window must be %s (got %s)" % (tuple(out_hw), (oh, ow)))
+        rows += [int(ih), int(iw), int(nh), int(nw), int(top), int(left), 1 if flip else 0]
+    return offs.contiguous().view(-1), torch.tensor(rows, dtype=torch.int32)
+
+
+def clip_transform_ragged(src, frame_off, geom, out_hw, mean=None, std=None, div255=False, out_dtype=torch.float16,
+                          slow_alpha=None):
+    """The fused chain on a batch whose clips read frames of their own sizes, in one launch (pv_clip_transform_ragged).
+
+    src       : flat uint8 or float32 CUDA tensor of packed (H, W, 3) frames, as ``decode_batch`` writes them
+    frame_off : (B, n_t) element offsets of each clip's kept frames in src (an offset may repeat)
+    geom      : per clip ((in_h, in_w), (new_h, new_w), (top, left, out_h, out_w), hflip)
+    Returns (B, 3, n_t, out_h, out_w) of out_dtype, or [slow, fast] with ``slow_alpha``.
+    """
+    if not torch.is_tensor(src) or src.device.type != "cuda":
+        raise RuntimeError("pytorchvideo_b200 transforms run on the GPU only (no CPU path)")
+    if src.dtype not in (torch.uint8, torch.float32) or not src.is_contiguous():
+        raise RuntimeError("the ragged source must be a contiguous uint8 or float32 tensor")
+    if out_dtype not in (torch.float16, torch.float32):
+        raise RuntimeError("the ragged mode writes float16 or float32")
+    offs, rows = ragged_tables(frame_off, geom, out_hw)
+    B, n_t = len(geom), offs.numel() // len(geom)
+    sizes = torch.tensor([g[0][0] * g[0][1] * 3 for g in geom], dtype=torch.int64).repeat_interleave(n_t)
+    if int(offs.min()) < 0 or int((offs + sizes).max()) > src.numel():
+        raise RuntimeError("a frame offset lies outside the source buffer")
+    lib = L.load()
+    dev = src.device
+    oh, ow = (int(v) for v in out_hw)
+    d = L.ClipBatchDesc()
+    d.C, d.n_clips, d.n_t, d.out_h, d.out_w = 3, B, n_t, oh, ow
+    _set_arith(d, 3, mean, std, div255)
+    d.src_dtype, d.dst_dtype = _DT[src.dtype], _DT[out_dtype]
+    out = torch.empty((B, 3, n_t, oh, ow), dtype=out_dtype, device=dev)
+    d.d_clip = out.stride(0)
+    slow_d, out_slow = None, None
+    if slow_alpha is not None:
+        slow_d, d.n_slow = _slow_table(n_t, slow_alpha, dev)
+        out_slow = torch.empty((B, 3, d.n_slow, oh, ow), dtype=out_dtype, device=dev)
+        d.d_slow_clip = out_slow.stride(0)
+    offs_d = offs.to(dev)
+    rows_d = rows.to(dev)
+    L.check(lib.pv_clip_transform_ragged(C.byref(d), src.data_ptr(), offs_d.data_ptr(), rows_d.data_ptr(),
+                                         rows.data_ptr(), slow_d.data_ptr() if slow_d is not None else None,
+                                         out.data_ptr(), out_slow.data_ptr() if out_slow is not None else None,
+                                         torch.cuda.current_stream(dev).cuda_stream), "pv_clip_transform_ragged")
+    out._pv_keepalive = (offs_d, rows_d, slow_d)     # device tables must outlive the asynchronous launch
     return [out_slow, out] if slow_alpha is not None else out
 
 
