@@ -1364,7 +1364,8 @@ def _lstm(low, m, x, mask, name):
     if r.bias:
         bias = torch.cat([par("bias_ih", s_) + par("bias_hh", s_) for s_ in sfx], 0)
     g = PL.emit_linear(p, x, w_ih, bias, L.ACT_NONE, None, name + ".lstm.input_proj")
-    w_hh_t = p.const(torch.stack([par("weight_hh", s_).t().contiguous() for s_ in sfx], 0))   # [dir][H][4H]
+    w_hh = torch.stack([par("weight_hh", s_).t().contiguous() for s_ in sfx], 0)                # [dir][H][4H]
+    w_hh_t = p.const(w_hh)
     y = PL._tok(p, x.N, 1, nd * H)
     lib = p.lib
     B, T = x.N, x.npos
@@ -1373,7 +1374,8 @@ def _lstm(low, m, x, mask, name):
         L.check(lib.pv_lstm_recurrence(g.ptr(), g.dt, g.row_stride, w_hh_t.data_ptr(), PL._mask_ptr(mask), B, T, H, nd,
                                        y.ptr(), y.row_stride, stream), "pv_lstm_recurrence(%s)" % name)
     p.add(name + ".lstm.recurrence", fn, "other", 2.0 * nd * B * T * 4 * H * H, nd * 4 * H * H * 4 * T,
-          reads=(g,) + PL._mask_io(mask), writes=(y,))
+          reads=(g,) + PL._mask_io(mask), writes=(y,),
+          spec={"kind": "lstm", "g": g, "mask": mask, "y": y, "w_hh_t": w_hh, "hidden": H, "dirs": nd})
     return _mark(y, squeeze=True, retargetable=True), mask
 
 

@@ -725,7 +725,8 @@ class Plan:
             L.check(lib.pv_roi_align_fwd(x.ptr(), x.dt, x.row_stride, N, H, W, Cp, rois.tensor.data_ptr(), K, rh, rw,
                                          float(spatial_scale), int(sampling_ratio), y.ptr(), y.row_stride, stream),
                     "pv_roi_align_fwd(%s)" % name)
-        self.add(name, fn, reads=(x,), writes=(y,))
+        self.add(name, fn, reads=(x,), writes=(y,), spec={"kind": "roi_align", "x": x, "rois": rois, "y": y,
+                                                          "geom": (rh, rw, float(spatial_scale), int(sampling_ratio))})
         return y
 
     def emit_act(self, x, act, name="act"):
@@ -778,7 +779,8 @@ class Plan:
             # a [1, 1, 1, 1, total] "clip" with one channel: the layout conversion degenerates to a cast
             L.check(lib.pv_ncdhw_to_ndhwc(static_in.data_ptr(), src_dt, x.ptr(), x.dt, 1, 1, 1, 1, total, 1, 1, stream),
                     "pv_ncdhw_to_ndhwc(tokens)")
-        self.add("tokens_in", fn, "other", 0.0, total * (static_in.element_size() + _ESIZE[self.dt]), reads=(), writes=(x,))
+        self.add("tokens_in", fn, "other", 0.0, total * (static_in.element_size() + _ESIZE[self.dt]), reads=(), writes=(x,),
+                 spec={"kind": "tokens_in", "src": static_in, "y": x})
         return x
 
     def emit_to_tokens(self, x, name="to_tokens", squeeze=False):
@@ -1033,10 +1035,11 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool", norm_
         d.groups, d.act, d.has_residual = dim_all, L.ACT_NONE, 0
         d.x_row_stride, d.y_row_stride = x.row_stride, y.row_stride
         d.x_batch_stride, d.y_batch_stride = x.npos * x.row_stride, y.npos * y.row_stride
+        pre_vec = None
         if norm_before_pool:
             vec = [_prologue_vectors(n, pool_ch) for n in norms]
-            pre_s = plan.const(torch.cat([s_.repeat(reps) for s_, _ in vec]).contiguous())
-            pre_b = plan.const(torch.cat([b_.repeat(reps) for _, b_ in vec]).contiguous())
+            pre_vec = [torch.cat([v_[j].repeat(reps) for v_ in vec]).float().contiguous() for j in (0, 1)]
+            pre_s, pre_b = plan.const(pre_vec[0]), plan.const(pre_vec[1])
             d.pre_scale, d.pre_bias, d.pre_act = pre_s.data_ptr(), pre_b.data_ptr(), L.ACT_GELU
             plan.stats["pool_prologue"] = plan.stats.get("pool_prologue", 0) + 1
         # a one-frame token grid (image MViT) pooled by a (1,kh,kw) conv: the plane kernel (csrc/pv_dwplane.cu) when it
@@ -1060,7 +1063,8 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool", norm_
         plan.add(name + ".dwconv", fn, "depthwise", 2.0 * x.N * To * Ho * Wo * dim_all * k[0] * k[1] * k[2],
                  (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz,
                  spec={"kind": "token_conv", "x": x, "y": y, "thw": (T, H, W), "cls": cls, "weight": w_full,
-                       "stride": s, "padding": p, "dilation": dl, "prologue": norm_before_pool, "modules": pools})
+                       "stride": s, "padding": p, "dilation": dl, "prologue": norm_before_pool, "modules": pools,
+                       "pre_scale": pre_vec[0] if pre_vec else None, "pre_bias": pre_vec[1] if pre_vec else None})
     else:
         d = L.Pool3dDesc()
         d.dtype, d.mode = x.dt, L.POOL_MAX if kind == "MaxPool3d" else L.POOL_AVG
@@ -1160,7 +1164,9 @@ def emit_channel_affine(plan, x, scale, shift, name="affine"):
         d.x_batch_stride, d.y_batch_stride = x.npos * x.row_stride, y.npos * y.row_stride
         L.check(lib.pv_dwconv3d_fwd(C_.byref(d), x.ptr(), w_d.data_ptr(), sc.data_ptr(), sh.data_ptr(), y.ptr(), None,
                                     stream), "pv_dwconv3d_fwd(%s)" % name)
-    plan.add(name, fn, "depthwise", 2.0 * x.N * x.npos * C, 2 * x.N * x.npos * C * _ESIZE[x.dt], reads=(x,), writes=(y,))
+    plan.add(name, fn, "depthwise", 2.0 * x.N * x.npos * C, 2 * x.N * x.npos * C * _ESIZE[x.dt], reads=(x,), writes=(y,),
+             spec={"kind": "channel_affine", "x": x, "y": y, "scale": scale.float().cpu(),
+                   "shift": shift.float().cpu()})
     return y
 
 
@@ -1194,7 +1200,8 @@ def emit_mask_force_first(plan, mask, name="mask_force_first"):
 
     def fn(stream):
         L.check(lib.pv_mask_force_first(mask.ptr(), out.ptr(), mask.B, mask.T, stream), "pv_mask_force_first(%s)" % name)
-    plan.add(name, fn, "other", 0.0, 2 * mask.B * mask.T, reads=mask.io(), writes=out.io())
+    plan.add(name, fn, "other", 0.0, 2 * mask.B * mask.T, reads=mask.io(), writes=out.io(),
+             spec={"kind": "mask_force_first", "mask": mask, "out": out})
     return out
 
 
@@ -1208,7 +1215,8 @@ def emit_masked_pool(plan, x, mask, mode, name="masked_pool"):
     def fn(stream):
         L.check(lib.pv_masked_pool(x.ptr(), x.dt, x.row_stride, B, T, Cc, _mask_ptr(mask), mode, y.ptr(), y.row_stride,
                                    stream), "pv_masked_pool(%s)" % name)
-    plan.add(name, fn, "other", 0.0, (B * T + B) * Cc * _ESIZE[x.dt], reads=(x,) + _mask_io(mask), writes=(y,))
+    plan.add(name, fn, "other", 0.0, (B * T + B) * Cc * _ESIZE[x.dt], reads=(x,) + _mask_io(mask), writes=(y,),
+             spec={"kind": "masked_pool", "x": x, "mask": mask, "mode": mode, "y": y})
     return y
 
 
@@ -1228,7 +1236,9 @@ def emit_masked_default(plan, x, mask, default, name="learned_default"):
     def fn(stream):
         L.check(lib.pv_masked_default(x.ptr(), x.dt, x.row_stride, x.N, x.C, mask.ptr(), mask.T, d.data_ptr(), y.ptr(),
                                       y.row_stride, stream), "pv_masked_default(%s)" % name)
-    plan.add(name, fn, "other", 0.0, 2 * x.N * x.C * _ESIZE[x.dt], reads=(x,) + mask.io(), writes=(y,))
+    plan.add(name, fn, "other", 0.0, 2 * x.N * x.C * _ESIZE[x.dt], reads=(x,) + mask.io(), writes=(y,),
+             spec={"kind": "masked_default", "x": x, "mask": mask, "y": y,
+                   "default": default.detach().float().cpu().reshape(-1)})
     return y
 
 
@@ -1251,7 +1261,8 @@ def emit_reduce_fusion(plan, parts, op, name="reduce_fusion"):
             ptrs[i], strides[i] = p.ptr(), p.row_stride
         L.check(lib.pv_reduce_fusion(ptrs, strides, P, p0.dt, p0.N * p0.npos, p0.C, op, y.ptr(), y.row_stride, stream),
                 "pv_reduce_fusion(%s)" % name)
-    plan.add(name, fn, "other", 0.0, (P + 1) * p0.N * p0.npos * p0.C * _ESIZE[p0.dt], reads=tuple(parts), writes=(y,))
+    plan.add(name, fn, "other", 0.0, (P + 1) * p0.N * p0.npos * p0.C * _ESIZE[p0.dt], reads=tuple(parts), writes=(y,),
+             spec={"kind": "reduce_fusion", "parts": list(parts), "op": op, "y": y})
     return y
 
 
@@ -1270,7 +1281,8 @@ def emit_copy_tokens(plan, x, y, row0, name="copy_tokens"):
             L.check(lib.pv_copy_rows(x.ptr() + b * x.npos * x.row_stride * esz,
                                      y.ptr() + (b * y.npos + row0) * y.row_stride * esz, x.dt, x.npos, x.C,
                                      x.row_stride, y.row_stride, stream), "pv_copy_rows(%s)" % name)
-    plan.add(name, fn, "other", 0.0, 2 * x.N * x.npos * x.C * _ESIZE[x.dt], reads=(x,), writes=(y,))
+    plan.add(name, fn, "other", 0.0, 2 * x.N * x.npos * x.C * _ESIZE[x.dt], reads=(x,), writes=(y,),
+             spec={"kind": "copy_tokens", "x": x, "y": y, "row0": int(row0)})
 
 
 def emit_attention_masked(plan, q, k, v, heads, scale, mask, name="attn", weights=False):
@@ -1298,7 +1310,9 @@ def emit_attention_masked(plan, q, k, v, heads, scale, mask, name="attn", weight
                 "pv_attention_masked_fwd(%s)" % name)
     plan.add(name, fn, "attention", 4.0 * B * heads * Nq * Nk * (dim // heads),
              (B * Nq * dim * 2 + 2 * B * Nk * dim) * _ESIZE[plan.dt], reads=(q, k, v) + mask.io(),
-             writes=(o,) + ((lse,) if lse is not None else ()))
+             writes=(o,) + ((lse,) if lse is not None else ()),
+             spec={"kind": "attention_masked", "q": q, "k": k, "v": v, "o": o, "heads": heads, "scale": d.scale,
+                   "mask": mask, "lse": lse})
     plan.attention_calls.append({"name": name, "B": B, "H": heads, "Nq": Nq, "Nk": Nk, "D": dim // heads,
                                  "scale": d.scale, "normalize": 0, "add_q_residual": 0, "masked": True})
     if weights:
@@ -1306,5 +1320,7 @@ def emit_attention_masked(plan, q, k, v, heads, scale, mask, name="attn", weight
             L.check(lib.pv_attention_weights(C_.byref(d), q.ptr(), k.ptr(), mask.ptr(), lse.tensor.data_ptr(),
                                              w.tensor.data_ptr(), stream), "pv_attention_weights(%s)" % name)
         plan.add(name + ".weights", fn_w, "other", 2.0 * B * heads * Nq * Nk * (dim // heads), B * Nq * Nk * 4,
-                 reads=(q, k, lse) + mask.io(), writes=(w,))
+                 reads=(q, k, lse) + mask.io(), writes=(w,),
+                 spec={"kind": "attention_weights", "q": q, "k": k, "mask": mask, "lse": lse, "w": w, "heads": heads,
+                       "scale": d.scale})
     return o, w

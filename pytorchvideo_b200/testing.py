@@ -8,7 +8,9 @@ does) and re-draws conv / linear weights from a fixed seed, on the CPU generator
 state is reproduced bit-for-bit here and on the GPU box.
 """
 import math
+from fractions import Fraction
 
+import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -389,8 +391,22 @@ def assert_close_to_f64(got, ref64, absref64, k_len, acc_eps=ACC_EPS, what="", e
 SUM_EPS = 2.0 ** -18
 # Attention error bound: the tensor-core kernels round the probabilities to f16 before P.V while the row sum l keeps
 # them in fp32, so an output may move by ~2 * 2^-11 of sum_j p_j |v_j| on top of its own rounding, independent of Nk;
-# ACC_EPS_ATTN (with k_len = 0) allows twice that (absref = p.|v| + |q|).
+# ACC_EPS_ATTN (with k_len = 0) allows twice that (absref = p.|v| + |q|).  A probability below 2^-14 of its row's
+# running maximum is an f16 subnormal, rounded to the absolute step 2^-24 instead: attn_p16_floor64 charges half that
+# step for every key (a sharp softmax whose winning key has v ~ 0 leaves o made of such probabilities).
 ACC_EPS_ATTN = 2.0 ** -9
+# fp32 attention (attention_kernel<float, D>, attention_wide_simt_kernel<float, D>: fp32 storage, fp32 maths, P never
+# rounded to f16).  Per query the kernel forms o = (sum_j p_j v_j) / l, l = sum_j p_j, online over key tiles of 32:
+#   s_j = sum_c fmaf(q_c * scale, k_c, .)         D + 1 roundings of terms of magnitude S_j = |scale| |q|.|k_j|
+#   p_j = __expf(s_j - m)                         the subtraction (one rounding of |x_j|, x_j = s_j - m) and __expf,
+#                                                 within (2 + 1.173 |x_j|) ulp (as act_err64 charges it)
+#   l, acc rescaled by __expf(m_old - m_new) once per tile (the same factor on both: it cancels in acc / l), summed
+#   by fmaf over Nk keys (acc) and a 32-lane shuffle tree plus one add per tile (l), then acc * (1 / l) (+ q).
+# The relative errors e_j of p_j move o as attn_score_extra64 bounds (to first order: sum_j p_j e_j |v_j| +
+# (sum_j p_j e_j) sum_j p_j |v_j|).  The tensor-core kernels form the same fp32 scores, so their bound carries it too.
+# The sums, rescales and the final division take at most Nk + 3 ceil(Nk / 32) + 10 roundings of p.|v| + |q|; with
+# k_len = Nk the comparator's accumulation term acc_eps (1 + Nk / 64) = (128 + 2 Nk) 2^-24 covers them.
+ACC_EPS_ATTN_F32 = 2.0 ** -17
 # Lipschitz constants of the activations (largest slope)
 LIP = {"none": 1.0, "relu": 1.0, "swish": 1.1, "gelu": 1.13, "sigmoid": 0.25, "hswish": 1.5}
 
@@ -445,15 +461,144 @@ def conv_ref64(x, w, scale, bias, stride, padding, dilation, groups, act, res):
     return act64(y, act), a
 
 
-def attn_ref64(q, k, v, scale, resid):
-    """q: [B,H,Nq,D] (f16 grid) -> (ref64, absref64) with absref = softmax . |v| (+ |q|)."""
+def attn_probs64(q, k, scale, mask=None):
+    """Float64 softmax(scale q k^T) over the keys, q [B, H, Nq, D], k [B, H, Nk, D]; mask (bool [B, Nk]): keys where
+    it is False take no weight, and a query without a valid key has all-zero probabilities."""
+    s = (q.double() * scale) @ k.double().transpose(-2, -1)
+    if mask is None:
+        return s.softmax(-1)
+    s = s.masked_fill(~mask.to(s.device)[:, None, None, :], float("-inf"))
+    return s.softmax(-1).nan_to_num(0.0)
+
+
+def attn_ref64(q, k, v, scale, resid, normalize=0, mask=None):
+    """q: [..., Nq, D], k / v: [..., Nk, D] (the operands the kernel read) -> (ref64, absref64) with
+    absref = P . |v| (+ |q|).  normalize = 0: P = softmax(scale q k^T) (masked keys as attn_probs64); 1: the linear mode
+    P = scale q k^T / Nk, whose magnitude is |P| = |scale| |q| |k|^T / Nk."""
     q64, k64, v64 = q.double(), k.double(), v.double()
-    p = ((q64 * scale) @ k64.transpose(-2, -1)).softmax(-1)
+    if normalize:
+        nk = k.shape[-2]
+        p = ((q64 * scale) @ k64.transpose(-2, -1)) / nk
+        absp = (q64.abs() @ k64.abs().transpose(-2, -1)) * abs(scale) / nk
+    else:
+        p = absp = attn_probs64(q64, k64, scale, mask)
     ref = p @ v64
-    absref = p @ v64.abs()
+    absref = absp @ v64.abs()
     if resid:
         ref, absref = ref + q64, absref + q64.abs()
     return ref, absref
+
+
+def _score_err64(q, k, scale, mask):
+    """(p, e): the float64 probabilities and a bound on the relative error of the kernel's fp32 probability of every
+    key: D + 2 roundings of |scale| |q|.|k_j| in the score, one of |x_j| = |s_j - m| in the subtraction and the
+    __expf error at x_j (masked keys and queries without a valid key: 0)."""
+    q64, k64 = q.double(), k.double()
+    s = (q64 * scale) @ k64.transpose(-2, -1)
+    S = (q64.abs() * abs(scale)) @ k64.abs().transpose(-2, -1)
+    p = attn_probs64(q64, k64, scale, mask)
+    valid = p > 0
+    x = torch.where(valid, s - s.masked_fill(~valid, float("-inf")).max(-1, keepdim=True).values, torch.zeros_like(s))
+    x = x.abs()
+    e = (q.shape[-1] + 2) * F32_EPS * S + F32_EPS * x + (2 + 1.173 * x) * 2.0 ** -23
+    return p, torch.where(valid, e, torch.zeros_like(e))
+
+
+def attn_score_extra64(q, k, v, scale, mask=None):
+    """extra64 of softmax attention: the error of the kernel's fp32 scores and __expf probabilities (_score_err64)
+    carried to o, for q [..., Nq, D], k / v [..., Nk, D].  With p_j off by a factor within exp(+-e_j),
+    |o' - o| <= (sum_j p_j E_j |v_j| + (sum_j p_j E_j) |o|) / sum_j p_j exp(-e_j), E_j = exp(e_j) - 1, and
+    |o| <= sum_j p_j |v_j|.  Where the logits are so large that e_j reaches 1 (fp32 cannot resolve which key wins)
+    the bound grows accordingly."""
+    p, e = _score_err64(q, k, scale, mask)
+    pE = p * torch.expm1(e)
+    av = v.double().abs()
+    den = (p * torch.exp(-e)).sum(-1, keepdim=True)
+    den = torch.where(den > 0, den, torch.ones_like(den))         # queries without a valid key: o = 0 exactly
+    return (pE @ av + pE.sum(-1, keepdim=True) * (p @ av)) / den
+
+
+def attn_weights_err64(q, k, scale, mask=None):
+    """(ref, err) of the head-averaged attention weights [B, Nq, Nk] pv_attention_weights writes in fp32 from the
+    row log-sum-exp of the attention launch: w_j = sum_h __expf(s_hj - lse_h) / H.  Each term carries the relative
+    error of its score and __expf (_score_err64), the score error of the row maximum inside lse, and lse's own error:
+    log of a row sum with at most Nk + 3 ceil(Nk / 32) + 10 roundings, logf and the add (4 roundings of |lse|).  The
+    sum over heads and the division take H + 1 roundings of w."""
+    p, e = _score_err64(q, k, scale, mask)
+    H, Nk = q.shape[1], k.shape[-2]
+    s = (q.double() * scale) @ k.double().transpose(-2, -1)
+    lse = torch.logsumexp(s if mask is None else s.masked_fill(~mask.to(s.device)[:, None, None, :], float("-inf")), -1,
+                          keepdim=True).nan_to_num(0.0, neginf=0.0)
+    S = (q.double().abs() * abs(scale)) @ k.double().abs().transpose(-2, -1)
+    Smax = torch.where(p > 0, S, torch.zeros_like(S)).max(-1, keepdim=True).values
+    e_lse = (q.shape[-1] + 2) * F32_EPS * Smax + (Nk + 3 * -(-Nk // 32) + 10) * F32_EPS + 4 * F32_EPS * lse.abs()
+    w = p.mean(1)
+    return w, (p * (e + e_lse)).mean(1) + (H + 1) * F32_EPS * w
+
+
+def lstm_ref64(G, W, lengths, H, nd, h16=False):
+    """float64 restatement of the LSTM recurrence on the operands the kernel received: G [B][T][nd*4H] (input
+    projection plus biases), W^T [nd][H][4H]; the first lengths[b] steps of row b, walked forward (and backward by the
+    second direction).  h16: h enters the product rounded to f16 (the tensor-core operand of the cluster kernel).
+    Returns (h_n [B, nd*H], err): err bounds the kernel's fp32 error, propagated to first order step by step:
+      z = G + h W        H + 2 roundings of |G| + |h| |W|, the carried error of h through |W| (and h's f16 rounding)
+      sigmoid = 1 / (1 + expf(-z)), tanhf    each within 2 ulp, and the slope s (1 - s) or 1 - t^2 times z's error
+      c = f c + i g, h = o tanhf(c)          the carried errors of f, c, i, g, o and 3 / 2 roundings."""
+    G, W = G.double().cpu(), W.double().cpu()
+    U = F32_EPS
+    B = G.shape[0]
+    out = torch.zeros(B, nd * H, dtype=torch.float64)
+    err = torch.zeros(B, nd * H, dtype=torch.float64)
+    for b in range(B):
+        n = int(lengths[b])
+        for d in range(nd):
+            h, c, eh, ec = (torch.zeros(H, dtype=torch.float64) for _ in range(4))
+            Wd = W[d]
+            for s_ in range(n):
+                t = s_ if d == 0 else n - 1 - s_
+                g_t = G[b, t, d * 4 * H:(d + 1) * 4 * H]
+                hop = h.half().double() if h16 else h
+                z = g_t + hop @ Wd
+                ez = (H + 2) * U * (g_t.abs() + h.abs() @ Wd.abs()) + eh @ Wd.abs()
+                if h16:
+                    ez = ez + F16_EPS * (h.abs() @ Wd.abs())
+                sg = z.sigmoid()
+                es = sg * (1 - sg) * (ez + 4 * U) + 3 * U * sg
+                tg = z.tanh()
+                et = (1 - tg * tg) * ez + 4 * U * tg.abs()
+                i, f, gg, o = sg[:H], sg[H:2 * H], tg[2 * H:3 * H], sg[3 * H:]
+                ei, ef, eg, eo = es[:H], es[H:2 * H], et[2 * H:3 * H], es[3 * H:]
+                c_new = f * c + i * gg
+                ec = (f.abs() * ec + c.abs() * ef + i.abs() * eg + gg.abs() * ei
+                      + 3 * U * ((f * c).abs() + (i * gg).abs()))
+                c = c_new
+                tc = c.tanh()
+                h = o * tc
+                eh = tc.abs() * eo + o.abs() * ((1 - tc * tc) * ec + 4 * U * tc.abs()) + 2 * U * h.abs()
+            out[b, d * H:(d + 1) * H] = h
+            err[b, d * H:(d + 1) * H] = eh
+    return out, err
+
+
+def attn_p16_floor64(v, Nq, mask=None):
+    """extra64 of the f16 rounding of subnormal probabilities (see ACC_EPS_ATTN): 2^-25 sum_j |v_j| over the valid keys
+    for every query (the probabilities are relative to the row maximum, so the row sum l >= 1), v [B, H, Nk, D]."""
+    av = v.double().abs()
+    if mask is not None:
+        av = av * mask.to(av.device)[:, None, :, None]
+    return (2.0 ** -25 * av.sum(-2, keepdim=True)).expand(*v.shape[:2], Nq, v.shape[-1])
+
+
+def prologue_conv_ref64(x, pre_s, pre_b, w, scale, bias, stride, padding, dilation=(1, 1, 1)):
+    """The depthwise pooling conv with the BatchNorm + GELU prologue (pv_conv3d_desc.pre_*): conv(GELU(x * pre_s +
+    pre_b), w) * scale + bias in float64 on x's device, the prologue applied to in-bounds inputs before the zero
+    padding.  Returns (ref, absref, u, pre): u = GELU(pre) is what the stencil reads, pre its argument."""
+    C = x.shape[1]
+    view = (1, C, 1, 1, 1)
+    pre = x.double() * pre_s.double().to(x.device).view(view) + pre_b.double().to(x.device).view(view)
+    u = act64(pre, "gelu")
+    ref, absref = conv_ref64(u, w, scale, bias, stride, padding, dilation, C, "none", None)
+    return ref, absref, u, pre
 
 
 def _conv_bn(x, w, scale, bias, stride=1, padding=0):
@@ -535,6 +680,835 @@ def ln_dispatch(C, aligned=True):
         return "layernorm_reg_kernel", 1 << lg, nch
     return "layernorm_kernel", 32, -(-chunks // 32)
 
+
+# ---- RoIAlign (pv_roi_align_fwd): torchvision's fp32 sampling geometry and the float64 reference ------------------
+def round32(q):
+    """A Fraction rounded to the nearest float32 (ties to even), without double rounding through float64."""
+    r = np.float32(float(q))
+    best = r
+    for cand in (np.nextafter(r, np.float32(-np.inf)), np.nextafter(r, np.float32(np.inf))):
+        d0, d1 = abs(Fraction(float(best)) - q), abs(Fraction(float(cand)) - q)
+        if d1 < d0 or (d1 == d0 and int(np.array(cand).view(np.int32)) % 2 == 0):
+            best = cand
+    return best
+
+
+def fma32(a, b, c):
+    return round32(Fraction(float(a)) * Fraction(float(b)) + Fraction(float(c)))
+
+
+def roi_geometry(box, H, W, ph_n, pw_n, scale, sr, contract=False, mutation=None):
+    """torchvision's fp32 sampling geometry of one RoI (oracle.interp.roi_align_ref's arithmetic): per bin, the list
+    of kept samples (y_low, x_low, y_high, x_high, w1, w2, w3, w4), the count, and (grid_h, grid_w).
+    contract=True evaluates `end * scale - start` and `start + ph * bin` as single-rounding FMAs, as nvcc contracts
+    them unless told not to; mutation injects a known bug."""
+    s = np.float32(scale)
+    x1, y1, x2, y2 = (np.float32(v) for v in box[1:5])
+    sw, sh = x1 * s, y1 * s
+    if contract:
+        rw, rh = fma32(x2, s, -sw), fma32(y2, s, -sh)
+    else:
+        rw, rh = x2 * s - sw, y2 * s - sh
+    rw, rh = max(rw, np.float32(1)), max(rh, np.float32(1))
+    bh, bw = rh / np.float32(ph_n), rw / np.float32(pw_n)
+    rnd = np.floor if mutation == "floor" else np.ceil
+    gh = sr if sr > 0 else int(rnd(rh / np.float32(ph_n)))
+    gw = sr if sr > 0 else int(rnd(rw / np.float32(pw_n)))
+    count = max(gh * gw, 1)
+    half = np.float32(0) if mutation == "iy" else np.float32(0.5)
+    bins = []
+    for ph in range(ph_n):
+        st_y = fma32(np.float32(ph), bh, sh) if contract else sh + np.float32(ph) * bh
+        for pw in range(pw_n):
+            st_x = fma32(np.float32(pw), bw, sw) if contract else sw + np.float32(pw) * bw
+            samples = []
+            for iy in range(gh):
+                yy0 = st_y + (np.float32(iy) + half) * bh / np.float32(gh)
+                for ix in range(gw):
+                    xx = st_x + (np.float32(ix) + half) * bw / np.float32(gw)
+                    yy = yy0
+                    y_out = (yy >= H) if mutation == "ge_H" else (yy > H)
+                    if yy < -1 or y_out or xx < -1 or xx > W:
+                        continue
+                    yy, xx = max(yy, np.float32(0)), max(xx, np.float32(0))
+                    yl, xl = int(yy), int(xx)
+                    if yl >= H - 1:
+                        yh = yl = H - 1
+                        yy = np.float32(yl)
+                    else:
+                        yh = yl + 1
+                    if xl >= W - 1:
+                        xh = xl = W - 1
+                        xx = np.float32(xl)
+                    else:
+                        xh = xl + 1
+                    ly, lx = yy - np.float32(yl), xx - np.float32(xl)
+                    hy, hx = np.float32(1) - ly, np.float32(1) - lx
+                    samples.append((yl, xl, yh, xh, hy * hx, hy * lx, ly * hx, ly * lx))
+            bins.append(samples)
+    return bins, count, (gh, gw)
+
+
+def roi_ref64(x, rois, geom, mutation=None, emulate=False, contract=False):
+    """x [N, H, W, C], geom (pooled h, pooled w, spatial scale, sampling ratio); returns (ref, absref) [K, ph, pw, C]
+    in float64 (weights from the fp32 geometry), or the fp32 emulation in the kernel's order (acc += w1 v1 + w2 v2 +
+    w3 v3 + w4 v4 per sample, then / count).  Invalid batch indices give zeros.  contract: the geometry as nvcc
+    contracts it (see roi_geometry)."""
+    N, H, W, C = x.shape
+    ph_n, pw_n, scale, sr = geom
+    dt = torch.float32 if emulate else torch.float64
+    X = x.to(dt)
+    out = torch.zeros(len(rois), ph_n * pw_n, C, dtype=dt)
+    absout = torch.zeros(len(rois), ph_n * pw_n, C, dtype=torch.float64)
+    for k, box in enumerate(rois):
+        n = int(box[0])
+        if not 0 <= n < N:
+            continue
+        bins, count, _ = roi_geometry(box, H, W, ph_n, pw_n, scale, sr, contract=contract, mutation=mutation)
+        Xn = X[n]
+        for b, samples in enumerate(bins):
+            acc = torch.zeros(C, dtype=dt)
+            mag = torch.zeros(C, dtype=torch.float64)
+            for (yl, xl, yh, xh, w1, w2, w3, w4) in samples:
+                v = (Xn[yl, xl], Xn[yl, xh], Xn[yh, xl], Xn[yh, xh])
+                acc = acc + (float(w1) * v[0] + float(w2) * v[1] + float(w3) * v[2] + float(w4) * v[3])
+                if not emulate:
+                    mag = mag + sum(float(w) * t.abs() for w, t in zip((w1, w2, w3, w4), v))
+            out[k, b] = acc / float(count)
+            absout[k, b] = mag / float(count)
+    shape = (len(rois), ph_n, pw_n, C)
+    return out.view(shape), absout.view(shape)
+
+
+def roi_acc_eps(rois, geom, H, W):
+    """About 4 roundings per sample (the four products summed, the accumulation) plus one for the division."""
+    grids = [roi_geometry(b, H, W, *geom)[2] for b in rois]
+    return (4 * max(gh * gw for gh, gw in grids) + 1) * F32_EPS
+
+
+
+# ---- per-launch audit of a compiled plan (tests/test_gpu_workload_audit.py, tests/test_gpu_model_audit.py) --------
+# Each op of a plan carries a record of what it computes (Plan.op_spec).  audit_plan walks the plan on one stream,
+# reads each op's inputs just before it runs, runs it, asserts the launched instances belong to the family the record
+# implies, and compares the output with the same operation in float64 under the kernel-matrix bounds; the stored
+# dtype of each output sets its rounding term (f16 or fp32), and the reference multiplies the operands the kernel read
+# (the weights in the plan's storage dtype, as engine/packing.py packs them).
+NO_VALUE_SUFFIXES = (".se_zero",)        # ops that produce no value of their own: the clear of an SE-sum accumulator
+
+_TC = ("conv3d_igemm_kernel<", "conv3d_igemm_gather_kernel<", "conv3d_igemm_grouped_kernel<",
+       "conv3d_stem_rows_kernel<", "conv3d_stem_stream_kernel<")
+_DW = ("dwconv3d_lane_kernel<", "dwconv_temporal_kernel<", "dwconv3d_tile_kernel<", "dwconv_plane_kernel<",
+       "dwconv3d_kernel<", "dwconv3d_w4_kernel<")
+_LN = ("layernorm_reg_kernel", "layernorm_kernel")
+_ATTN = ("attention_wgmma_kernel<", "attention_mma_kernel<", "attention_kernel<", "attention_wide_kernel<",
+         "attention_wide_simt_kernel<")
+_CVT = ("ncdhw_to_ndhwc_kernel", "ncdhw_to_ndhwc_padw_kernel", "ncdhw_f32_to_ndhwc4_padw_kernel")
+# instance families a record's launch may take, by record kind (conv: by route).  The prefixes cover the f16 and the
+# fp32 instances (conv3d_direct_kernel<float>, dwconv3d_kernel<float>, dwconv3d_w4_kernel<float,..>,
+# attention_kernel<float,..>, attention_wide_simt_kernel<float,..>); FAMILY_F32 lists the fp32 ones an f32 plan takes.
+FAMILY = {
+    "tcgen05": _TC, "grouped": _TC, "stem_stream": _TC, "direct": ("conv3d_direct_kernel<",),
+    "depthwise": _DW + ("channel_sum_kernel",), "token_conv": _DW, "channel_affine": _DW,
+    "to_ndhwc": _CVT, "tokens_in": _CVT, "to_f32": ("ndhwc_to_ncdhw_kernel",), "copy": ("copy_rows_kernel",),
+    "tap_sum": ("temporal_tap_sum_kernel",), "fused_block": ("bottleneck_fused_kernel<",),
+    "pool": ("pool3d_kernel", "global_pool_kernel"), "head_reduce": ("head_reduce_kernel",),
+    "se_gate": ("se_gate_kernel",), "scale_act": ("scale_act_kernel",), "pos_cls": ("add_pos_cls_kernel",),
+    "layernorm": _LN + ("add_layernorm_kernel",), "layernorm_sets": _LN, "add_layernorm": ("add_layernorm_kernel",),
+    "attention": _ATTN, "copy_cls": ("copy_rows_kernel",), "roi_align": ("roi_align_kernel<",),
+    "mask_force_first": ("mask_force_first_kernel",), "masked_pool": ("masked_pool_kernel<",),
+    "masked_default": ("masked_default_kernel<",), "reduce_fusion": ("reduce_fusion_kernel<",),
+    "copy_tokens": ("copy_rows_kernel",),
+    "attention_masked": ("attention_wgmma_masked_kernel<", "attention_mma_masked_kernel<", "attention_masked_kernel<"),
+    "attention_weights": ("attention_weights_kernel<",),
+    "lstm": ("lstm_recurrence_kernel<", "lstm_cluster_kernel"),
+}
+_DW32 = ("dwconv3d_kernel<float", "dwconv3d_w4_kernel<float,")       # <float>, <float,pre>, <float,kt,sw>(,pre)
+FAMILY_F32 = {"direct": ("conv3d_direct_kernel<float>",), "depthwise": _DW32 + ("channel_sum_kernel",),
+              "token_conv": _DW32, "channel_affine": _DW32,
+              "attention": ("attention_kernel<float,", "attention_wide_simt_kernel<float,"),
+              "attention_masked": ("attention_masked_kernel<float,",),
+              "attention_weights": ("attention_weights_kernel<float>",),
+              "masked_pool": ("masked_pool_kernel<float,",), "masked_default": ("masked_default_kernel<float>",),
+              "reduce_fusion": ("reduce_fusion_kernel<float,",), "lstm": ("lstm_recurrence_kernel<float>",)}
+
+_ACT_NAMES = ("none", "relu", "swish", "gelu", "sigmoid", "hswish")       # by the library's ACT_* value
+
+
+def supported(spec):
+    """True when the audit has a reference for this record."""
+    return spec is not None and (spec["route"] if spec["kind"] == "conv" else spec["kind"]) in FAMILY
+
+
+def family_of(spec, f32=False):
+    key = spec["route"] if spec["kind"] == "conv" else spec["kind"]
+    return FAMILY_F32.get(key, FAMILY[key]) if f32 else FAMILY[key]
+
+
+def record_io(spec):
+    """(plan tensors the op reads, plan tensors it writes) according to its record."""
+    k = spec["kind"]
+    if k == "conv":
+        ins = [spec["x"]] + [t for t in (spec["residual"],) if t is not None]
+        if spec["addend"] is not None:
+            ins.append(spec["addend"][0])
+        return ins, [spec["y"]] + ([spec["se_sums"]] if spec["se_sums"] is not None else [])
+    if k in ("to_ndhwc", "tokens_in"):
+        return [], [spec["y"]]
+    if k in ("head_reduce", "to_f32"):
+        return [spec["x"]], [spec["out"]]
+    if k == "se_gate":
+        return [spec["sums"]], [spec["gate"]]
+    if k == "channel_sum":
+        return [spec["x"]], [spec["sums"]]
+    if k == "scale_act":
+        return [spec["x"]] + ([spec["gate"]] if spec["gate"] is not None else []), [spec["y"]]
+    if k == "add_layernorm":
+        return [spec["a"], spec["br"]], [t for t in (spec["s"], spec["y"]) if t is not None]
+    if k == "layernorm_sets":
+        return [spec["x"], spec["y"]], [spec["y"]]
+    if k == "attention":
+        return [spec["q"], spec["k"], spec["v"]], [spec["o"]]
+    if k == "mask_force_first":
+        return list(spec["mask"].io()), list(spec["out"].io())
+    if k in ("masked_pool", "masked_default"):
+        return [spec["x"]] + list(_mask_io(spec["mask"])), [spec["y"]]
+    if k == "reduce_fusion":
+        return list(spec["parts"]), [spec["y"]]
+    if k == "attention_masked":
+        return [spec["q"], spec["k"], spec["v"]] + list(spec["mask"].io()), \
+            [spec["o"]] + ([spec["lse"]] if spec["lse"] is not None else [])
+    if k == "attention_weights":
+        return [spec["q"], spec["k"], spec["lse"]] + list(spec["mask"].io()), [spec["w"]]
+    if k == "lstm":
+        return [spec["g"]] + list(_mask_io(spec["mask"])), [spec["y"]]
+    return [spec["x"]], [spec["y"]]
+
+
+def _mask_io(mask):
+    return mask.io() if mask is not None else ()
+
+
+def mask_bool(mask, clips):
+    """The (n, T) bool mask a MaskRef holds for the selected clips (None: every step valid)."""
+    if mask is None:
+        return None
+    t = mask.tensor if mask.tensor is not None else mask.buf.tensor[:mask.B * mask.T].view(mask.B, mask.T)
+    return t.view(mask.B, mask.T)[clips] != 0
+
+
+def io_buffers(items):
+    """ids of the plan buffers behind a list of TRefs / Bufs."""
+    from .engine.plan import Buf
+    return {id(t if isinstance(t, Buf) else t.buf) for t in items if t is not None and
+            (isinstance(t, Buf) or t.buf is not None)}
+
+
+def io_problems(plan):
+    """[(op name, "reads" | "writes")] where a record reads or writes a buffer its declared I/O (which orders the
+    lanes) does not list."""
+    bad = []
+    for (n, _), s, io in zip(plan.ops, plan.op_spec, plan.op_io):
+        if io is None or s is None:
+            continue
+        ins, outs = record_io(s)
+        if not io_buffers(ins) <= io_buffers(io[0]):
+            bad.append((n, "reads"))
+        if not io_buffers(outs) <= io_buffers(io[1]):
+            bad.append((n, "writes"))
+    return bad
+
+
+# ---- reading plan tensors
+def full_rows(t):
+    """[N, T, H, W, row_stride] view of the whole rows a TRef lives in (W-padded stem inputs: their visible columns)."""
+    b = t.buf.tensor
+    if t.padw is not None:
+        wp, wphys = t.padw
+        return b[:t.N * t.T * t.H * wphys * t.Cp].view(t.N, t.T, t.H, wphys, t.Cp)[:, :, :, wp:wp + t.W]
+    return b[:t.N * t.npos * t.row_stride].view(t.N, t.T, t.H, t.W, t.row_stride)
+
+
+def ndhwc(t, clips):
+    """The C valid channels of TRef t as [n, T, H, W, C] for the selected clips (a copy)."""
+    return full_rows(t)[clips][..., t.ch_off:t.ch_off + t.C].clone()
+
+
+def ncdhw64(t, clips):
+    return ndhwc(t, clips).permute(0, 4, 1, 2, 3).double()
+
+
+def rows64(t, clips):
+    """[n, npos, C] float64 (token tensors and pooled rows)."""
+    return ndhwc(t, clips).reshape(len(clips), t.npos, t.C).double()
+
+
+def buf_view(b, shape):
+    n = math.prod(shape)
+    return b.tensor[:n].view(*shape)
+
+
+def se_sums64(b, N, Cp, C, clips):
+    """The int64 fixed-point (2^-24) per-(sample, channel) sums an SE accumulator holds, as float64."""
+    return b.tensor[:2 * N * Cp].view(torch.int64).view(N, Cp)[clips, :C].double() * 2.0 ** -24
+
+
+def _grid(rows, cls, thw):
+    """[n, cls + THW, C] token rows -> the patch grid [n, C, T, H, W]."""
+    n, _, C = rows.shape
+    return rows[:, cls:].reshape(n, *thw, C).permute(0, 4, 1, 2, 3)
+
+
+def _rows_of(grid):
+    n, C = grid.shape[:2]
+    return grid.permute(0, 2, 3, 4, 1).reshape(n, -1, C)
+
+
+def _tdt(t):
+    """torch dtype a TRef / Buf is stored in."""
+    from .engine.plan import _TORCH_DT
+    return _TORCH_DT[t.dt]
+
+
+def _is32(t):
+    return _tdt(t) == torch.float32
+
+
+def _rnd(t):
+    """Unit roundoff of the stored result."""
+    return F32_EPS if _is32(t) else F16_EPS
+
+
+def _wq(w, t):
+    """The weights as the kernel writing TRef t read them: packed in t's storage dtype (engine/packing.py)."""
+    return w.detach().to(_tdt(t)).double()
+
+
+# ---- per kind: inputs (read before the op runs), output (after) and the comparison
+def gather_inputs(spec, clips):
+    k = spec["kind"]
+    if k in ("to_ndhwc", "tokens_in"):
+        return {"src": spec["src"][clips].clone()}
+    if k == "conv":
+        d = {"x": ncdhw64(spec["x"], clips)}
+        d["res"] = ncdhw64(spec["residual"], clips) if spec["residual"] is not None else None
+        if spec["addend"] is not None:
+            a, off = spec["addend"]
+            co = spec["weight"].shape[0]
+            full = full_rows(a)[clips][..., a.ch_off + off:a.ch_off + off + co]
+            d["addend"] = full.permute(0, 4, 1, 2, 3).double()
+        return d
+    if k == "tap_sum":
+        return {"x": ndhwc(spec["x"], clips).double()}
+    if k == "fused_block":
+        return {"x": ncdhw64(spec["x"], clips)}
+    if k in ("pool", "token_conv", "copy_cls", "pos_cls", "head_reduce", "layernorm", "to_f32", "copy",
+             "channel_affine"):
+        return {"x": rows64(spec["x"], clips), "x_raw": ndhwc(spec["x"], clips)}
+    if k == "se_gate":
+        x = spec["x"]
+        return {"sums": se_sums64(spec["sums"], x.N, x.Cp, x.C, clips)}
+    if k == "scale_act":
+        x = spec["x"]
+        g = buf_view(spec["gate"], (x.N, x.Cp))[clips, :x.C].double() if spec["gate"] is not None else None
+        return {"x": rows64(x, clips), "gate": g}
+    if k == "add_layernorm":
+        return {"a": rows64(spec["a"], clips).float(), "br": rows64(spec["br"], clips).float()}
+    if k == "layernorm_sets":
+        return {"x": rows64(spec["x"], clips), "y": rows64(spec["y"], clips)}
+    if k == "attention":
+        return {n: rows64(spec[n], clips) for n in ("q", "k", "v")}
+    if k == "mask_force_first":
+        m = spec["mask"]
+        src = m.tensor if m.tensor is not None else m.buf.tensor[:m.B * m.T]
+        return {"src": src.view(m.B, m.T)[clips].clone()}
+    if k in ("masked_pool", "masked_default", "copy_tokens"):
+        return {"x": rows64(spec["x"], clips), "x_raw": ndhwc(spec["x"], clips),
+                "mask": mask_bool(spec.get("mask"), clips)}
+    if k == "reduce_fusion":
+        return {"parts": [rows64(t, clips) for t in spec["parts"]],
+                "parts_raw": [ndhwc(t, clips).reshape(len(clips), t.npos, t.C) for t in spec["parts"]]}
+    if k in ("attention_masked", "attention_weights"):
+        d = {n: rows64(spec[n], clips) for n in ("q", "k", "v") if n in spec}
+        d["mask"] = mask_bool(spec["mask"], clips)
+        return d
+    if k == "lstm":
+        return {"g": rows64(spec["g"], clips), "mask": mask_bool(spec["mask"], clips)}
+    if k == "roi_align":
+        # the boxes may sample any clip: the whole feature map, and every box
+        x = spec["x"]
+        return {"x": ndhwc(x, list(range(x.N)))[:, 0].double().cpu(), "rois": spec["rois"].tensor.float().cpu()}
+    raise AssertionError("no reference for %s" % k)
+
+
+def _heads(r, H):
+    n, N, C = r.shape
+    return r.view(n, N, H, C // H).permute(0, 2, 1, 3)
+
+
+def compare(spec, inp, clips, launched, cpu_ref=False):
+    """Run the comparison of one op; returns [(what, err / tol)] (0.0 for bit-exact checks).  cpu_ref: compute the
+    float64 reference on the CPU instead (self-check of the GPU path) and return it instead of comparing."""
+    from . import _lib as L
+    from .engine import packing as PK
+    k = spec["kind"]
+    if cpu_ref is not False:
+        inp = {n: (v.to(cpu_ref) if torch.is_tensor(v) else v) for n, v in inp.items()}
+    n = len(clips)
+    out = []
+    live = cpu_ref is False
+
+    def bound(got, ref, absref, K, acc_eps=ACC_EPS, extra=None, rnd=F16_EPS, what=k):
+        if not live:
+            out.append((what, ref))
+            return
+        r = assert_close_to_f64(got, ref, absref, K, acc_eps=acc_eps, what=what, extra64=extra, rnd_eps=rnd)
+        out.append((what, r[0]))
+
+    def exact(got, want, what=k):
+        if not live:
+            out.append((what, want.double()))
+            return
+        g, w = got.contiguous(), want.to(got.dtype).contiguous()
+        bits = {torch.float16: torch.int16, torch.float32: torch.int32}[g.dtype]
+        diff = g.view(bits) != w.view(bits)
+        assert not bool(diff.any()), "%s: %d elements differ from the bit-exact reference" % (what, int(diff.sum()))
+        out.append((what, 0.0))
+
+    if k in ("to_ndhwc", "tokens_in"):
+        y = spec["y"]
+        src = inp["src"]
+        if k == "to_ndhwc":
+            want, got = src.permute(0, 2, 3, 4, 1), ndhwc(y, clips) if live else None
+        else:
+            want, got = src.reshape(n, -1, y.C), ndhwc(y, clips).reshape(n, -1, y.C) if live else None
+        exact(got, want.to(_tdt(y)))
+    elif k == "to_f32":
+        x, o = spec["x"], spec["out"]
+        if spec["layout"] == "ncdhw":
+            want = inp["x_raw"].permute(0, 4, 1, 2, 3)
+            got = buf_view(o, (x.N, x.C, x.T, x.H, x.W))[clips] if live else None
+        else:
+            want = inp["x_raw"].reshape(n, x.npos, x.C)
+            got = buf_view(o, (x.N, x.npos, x.C))[clips] if live else None
+        exact(got, want.float())
+    elif k == "copy":
+        exact(ndhwc(spec["y"], clips) if live else None, inp["x_raw"])
+    elif k == "conv":
+        y = spec["y"]
+        w = _wq(spec["weight"], y)
+        x = inp["x"]
+        ref, absref = conv_ref64(x, w, spec["scale"], spec["bias"], spec["stride"], spec["padding"],
+                                 spec["dilation"], spec["groups"], _ACT_NAMES[spec["act"]], inp["res"])
+        extra = None
+        if spec["addend"] is not None:
+            # the tensor-core epilogue adds the addend to the stored-precision result: one more rounding of |act(.)|
+            extra = _rnd(y) * ref.abs()
+            ref, absref = ref + inp["addend"], absref + inp["addend"].abs()
+        K = w.shape[1] * math.prod(w.shape[2:])
+        got = ncdhw64(y, clips) if live else None
+        bound(got, ref, absref, K, extra=extra, rnd=_rnd(y))
+        if spec["se_sums"] is not None:
+            ntaps = math.prod(w.shape[2:])
+            ref_s, npos = ref.sum(dim=(2, 3, 4)), ref[0, 0].numel()
+            if not live:
+                out.append(("se_sums", ref_s))
+            else:
+                # the SE-sum bound of test_depthwise_instance (fp32 sums of the pre-rounding outputs, fixed point)
+                sums = se_sums64(spec["se_sums"], y.N, y.Cp, y.C, clips).cpu()
+                ref_s, absref_s = ref_s.cpu(), absref.sum(dim=(2, 3, 4)).cpu()
+                tol = 2.0 ** -20 * (1 + ntaps / 64.0) * absref_s + npos * 2.0 ** -23 + 2.0 ** -22 * ref_s.abs()
+                if any(i.startswith(("dwconv3d_kernel<", "dwconv3d_w4_kernel<")) for i in launched):
+                    # the generic path sums the stored outputs (pv_channel_sum after the stencil): their rounding, and
+                    # the fp32 partial sums of its threads over up to channel_sum_adds positions each
+                    per_elem = _rnd(y) + (channel_sum_adds(npos, y.Cp) + 1) * F32_EPS
+                    tol = tol + per_elem * ref.abs().sum(dim=(2, 3, 4)).cpu()
+                r = float(((sums - ref_s).abs() / tol).max())
+                assert r <= 1.0, "se_sums: err/tol %.3g" % r
+                out.append(("se_sums", r))
+    elif k == "tap_sum":
+        x, y = inp["x"], spec["y"]
+        co, kt, st, pt, dil = y.C, spec["kt"], spec["st"], spec["pt"], spec["dil"]
+        cop = PK.pad8(co)
+        Ti, To = x.shape[1], y.T
+        acc = torch.zeros(n, To, y.H, y.W, co, dtype=torch.float64, device=x.device)
+        aab = torch.zeros_like(acc)
+        for t in range(To):
+            for d in range(kt):
+                ti = t * st + d * dil - pt
+                if 0 <= ti < Ti:
+                    tap = x[:, ti, :, :, d * cop:d * cop + co]
+                    acc[:, t] += tap
+                    aab[:, t] += tap.abs()
+        sc, bi = spec["scale"].double().to(x.device), spec["bias"].double().to(x.device)
+        pre = acc * sc + bi
+        act = _ACT_NAMES[spec["act"]]
+        absref = LIP[act] * (aab * sc.abs() + bi.abs())
+        got = ndhwc(y, clips) if live else None
+        bound(got, act64(pre, act), absref, kt + 2, acc_eps=SUM_EPS, extra=act_err64(pre, act), rnd=_rnd(y))
+    elif k == "fused_block":
+        y = spec["y"]
+        wa, wb, wc = (_wq(spec[m], y) for m in ("wa", "wb", "wc"))
+        ws = _wq(spec["ws"], y) if spec["ws"] is not None else None
+        yr, _, _, Y, prop = fused_block_ref64(inp["x"], wa, wb, wc, ws, spec["folds"], spec["kt"], spec["sb"],
+                                              _ACT_NAMES[spec["act"]])
+        K = wa.shape[0] + (wa.shape[1] if ws is not None else 0)
+        got = ncdhw64(y, clips) if live else None
+        bound(got, yr, Y, K, extra=prop, rnd=_rnd(y))
+    elif k == "pool":
+        x, y, cls = spec["x"], spec["y"], spec["cls"]
+        thw = spec.get("thw", (x.T, x.H, x.W))
+        g = _grid(inp["x"], cls, thw)
+        kk, s, p = spec["kernel"], spec["stride"], spec["padding"]
+        pad = (p[2], p[2], p[1], p[1], p[0], p[0])
+        got = rows64(y, clips)[:, cls:] if live else None
+        if spec["mode"] == L.POOL_MAX:
+            ref = F.max_pool3d(F.pad(g, pad, value=-math.inf), kk, s)
+            exact(got.to(_tdt(y)) if live else None, _rows_of(ref).to(_tdt(y)))
+        else:
+            ref = F.avg_pool3d(F.pad(g, pad), kk, s)
+            absref = F.avg_pool3d(F.pad(g.abs(), pad), kk, s)
+            glob = "global_pool_kernel" in launched
+            K = (math.ceil(math.prod(thw) / 32) + 32) if glob else math.prod(kk)
+            bound(got, _rows_of(ref), _rows_of(absref), K, acc_eps=SUM_EPS, rnd=_rnd(y))
+    elif k == "token_conv":
+        x, y, cls = spec["x"], spec["y"], spec["cls"]
+        g = _grid(inp["x"], cls, spec["thw"])
+        w = _wq(spec["weight"], y)
+        C = w.shape[0]
+        ones = torch.ones(C, dtype=torch.float64)
+        got = rows64(y, clips)[:, cls:] if live else None
+        if not spec["prologue"]:
+            ref, absref = conv_ref64(g, w, ones, torch.zeros_like(ones), spec["stride"], spec["padding"],
+                                     spec["dilation"], C, "none", None)
+            bound(got, _rows_of(ref), _rows_of(absref), math.prod(w.shape[2:]), rnd=_rnd(y))
+        else:
+            ref, absref, u, pre = prologue_conv_ref64(g, spec["pre_scale"], spec["pre_bias"], w, ones,
+                                                      torch.zeros_like(ones), spec["stride"], spec["padding"],
+                                                      spec["dilation"])
+            # the prologue's own error carried by the stencil: GELU in fp32 (act_err64) at an argument rounded once,
+            # and the f16 rounding of u where the TMA kernels stage it in shared memory
+            eu = act_err64(pre, "gelu") + LIP["gelu"] * F32_EPS * pre.abs() + _rnd(y) * u.abs()
+            extra = F.conv3d(eu, w.abs().to(eu.device), None, spec["stride"], spec["padding"], spec["dilation"], C)
+            bound(got, _rows_of(ref), _rows_of(absref), math.prod(w.shape[2:]), extra=_rows_of(extra), rnd=_rnd(y))
+    elif k == "channel_affine":
+        y = spec["y"]
+        v = inp["x"]
+        sc, sh = (spec[m].double().to(v.device) for m in ("scale", "shift"))
+        got = rows64(y, clips) if live else None
+        bound(got, v * sc + sh, v.abs() * sc.abs() + sh.abs(), 1, rnd=_rnd(y))
+    elif k == "copy_cls":
+        exact(rows64(spec["y"], clips)[:, 0].to(_tdt(spec["y"])) if live else None,
+              inp["x_raw"].reshape(n, -1, spec["x"].C)[:, 0])
+    elif k == "pos_cls":
+        y = spec["y"]
+        xr = inp["x_raw"].reshape(n, -1, spec["x"].C).float()
+        pos = spec["pos"].to(xr.device)
+        hc = 1 if spec["has_cls"] else 0
+        want = torch.empty(n, hc + xr.shape[1], xr.shape[2], dtype=torch.float32, device=xr.device)
+        if hc:
+            want[:, 0] = pos[0]
+        want[:, hc:] = xr + pos[hc:]
+        got = ndhwc(y, clips).reshape(n, y.npos, y.C) if live else None
+        exact(got, want.to(_tdt(y)))
+    elif k == "head_reduce":
+        x64 = inp["x"]
+        C = x64.shape[2]
+        got = buf_view(spec["out"], (spec["x"].N, C))[clips] if live else None
+        if not spec["softmax"]:
+            bound(got, x64.mean(1), x64.abs().mean(1), x64.shape[1] + 1, acc_eps=SUM_EPS, rnd=F32_EPS)
+        else:
+            p = torch.softmax(x64, 2)
+            d = x64 - x64.max(2, keepdim=True).values
+            rel = 2.0 ** -22 + F32_EPS * d.abs()
+            extra = (p * (rel + rel.max(2, keepdim=True).values)).mean(1)
+            D = -(-C // 256) + 13
+            bound(got, p.mean(1), p.mean(1), x64.shape[1] + D + 3, acc_eps=SUM_EPS, extra=extra, rnd=F32_EPS)
+    elif k == "se_gate":
+        x = spec["x"]
+        dev = inp["sums"].device
+        mean = inp["sums"] / x.npos
+        w1, b1, w2, b2 = (spec[m].double().to(dev) for m in ("w1", "b1", "w2", "b2"))
+        hid = (b1 + mean @ w1.t()).clamp_min(0)
+        a = b2 + hid @ w2.t()
+        gate = torch.sigmoid(a)
+        Hm = b1.abs() + mean.abs() @ w1.abs().t()
+        A = b2.abs() + Hm @ w2.abs().t()
+        extra = gate * (1 - gate) * (2 + 1.173 * a.abs()) * 2.0 ** -23 + F32_EPS * gate
+        got = buf_view(spec["gate"], (x.N, x.Cp))[clips, :x.C] if live else None
+        bound(got, gate, 0.25 * A, x.C + w1.shape[0] + 3, acc_eps=SUM_EPS, extra=extra, rnd=F32_EPS)
+    elif k == "scale_act":
+        y = spec["y"]
+        v = inp["x"]
+        if inp["gate"] is not None:
+            v = v * inp["gate"].unsqueeze(1)
+        act = _ACT_NAMES[spec["act"]]
+        got = rows64(y, clips) if live else None
+        bound(got, act64(v, act), LIP[act] * v.abs(), 0, acc_eps=F32_EPS, extra=act_err64(v, act), rnd=_rnd(y))
+    elif k == "layernorm":
+        v = inp["x"][:, :1] if spec["first_row_only"] else inp["x"]
+        C = v.shape[2]
+        name = next(iter(launched))
+        _, lpr, nch = ln_dispatch(C) if name in ("layernorm_reg_kernel", "add_layernorm_kernel") else \
+            ("layernorm_kernel", 32, -(-(-(-C // 8)) // 32))
+        ref, absref, K, extra = ln_ref64(v.reshape(-1, 1, C), spec["gamma"].view(1, -1), spec["beta"].view(1, -1), 1,
+                                         nch * 8 + int(math.log2(lpr)), spec["eps"])
+        got = rows64(spec["y"], clips).reshape(-1, 1, C) if live else None
+        bound(got, ref, absref, K, acc_eps=SUM_EPS, extra=extra, rnd=_rnd(spec["y"]))
+    elif k == "add_layernorm":
+        s = inp["a"] + inp["br"]                               # fp32, as the kernel adds
+        if spec["s"] is not None:
+            exact(ndhwc(spec["s"], clips).reshape(s.shape) if live else None, s, what="add_layernorm.sum")
+        if spec["y"] is not None:
+            C = s.shape[2]
+            _, lpr, nch = ln_dispatch(C)
+            ref, absref, K, extra = ln_ref64(s.reshape(-1, 1, C), spec["gamma"].view(1, -1),
+                                             spec["beta"].view(1, -1), 1, nch * 8 + int(math.log2(lpr)), spec["eps"])
+            got = rows64(spec["y"], clips).reshape(-1, 1, C) if live else None
+            bound(got, ref, absref, K, acc_eps=SUM_EPS, extra=extra, rnd=_rnd(spec["y"]))
+    elif k == "layernorm_sets":
+        y, cls, hd = spec["y"], spec["cls"], spec["head_dim"]
+        v = inp["y"].clone()
+        if cls:
+            v[:, 0] = inp["x"][:, 0]
+        C = v.shape[2]
+        G = C // hd
+        nsets = spec["gamma"].numel() // hd
+        name = next(iter(launched))
+        _, lpr, nch = ln_dispatch(hd) if name == "layernorm_reg_kernel" else \
+            ("layernorm_kernel", 32, -(-(-(-hd // 8)) // 32))
+        ref, absref, K, extra = ln_ref64(v.reshape(-1, G, hd), spec["gamma"].view(nsets, hd),
+                                         spec["beta"].view(nsets, hd), G // nsets, nch * 8 + int(math.log2(lpr)),
+                                         spec["eps"])
+        got = rows64(y, clips).reshape(-1, G, hd) if live else None
+        bound(got, ref, absref, K, acc_eps=SUM_EPS, extra=extra, rnd=_rnd(y))
+    elif k == "attention":
+        H, o, norm = spec["heads"], spec["o"], spec["normalize"]
+        q, kk, v = (_heads(inp[m], H) for m in ("q", "k", "v"))
+        ref, absref = attn_ref64(q, kk, v, spec["scale"], spec["residual"], norm)
+        back = lambda t: t.permute(0, 2, 1, 3).reshape(n, t.shape[2], -1)        # noqa: E731
+        got = rows64(o, clips) if live else None
+        if norm:
+            # the linear mode: D-term dot products and an Nk-term sum, each rounding charged (f16: P rounded as well)
+            if _is32(o):
+                bound(got, back(ref), back(absref), kk.shape[2] + q.shape[3], acc_eps=ACC_EPS_ATTN_F32, rnd=F32_EPS)
+            else:
+                bound(got, back(ref), back(absref), 0, acc_eps=ACC_EPS_ATTN)
+        elif not _is32(o):
+            extra = back(attn_score_extra64(q, kk, v, spec["scale"]) + attn_p16_floor64(v, q.shape[2]))
+            bound(got, back(ref), back(absref), 0, acc_eps=ACC_EPS_ATTN, extra=extra)
+        else:
+            extra = back(attn_score_extra64(q, kk, v, spec["scale"]))
+            bound(got, back(ref), back(absref), kk.shape[2], acc_eps=ACC_EPS_ATTN_F32, extra=extra, rnd=F32_EPS)
+    elif k == "mask_force_first":
+        want = inp["src"].clone()
+        want[:, 0] = 1
+        if not live:
+            out.append((k, want.double()))
+        else:
+            o = spec["out"]
+            got = o.buf.tensor[:o.B * o.T].view(o.B, o.T)[clips]
+            assert torch.equal(got, want.to(got.device)), "mask_force_first: the mask copy differs"
+            out.append((k, 0.0))
+    elif k == "masked_pool":
+        x, y = inp["x"], spec["y"]
+        m = inp["mask"] if inp["mask"] is not None else torch.ones(x.shape[:2], dtype=torch.bool, device=x.device)
+        m = m.to(x.device)
+        cnt = m.sum(1, keepdim=True)
+        got = ndhwc(y, clips).reshape(n, y.C) if live else None
+        if spec["mode"] == L.MPOOL_MAX:
+            # the largest valid step; a row without one pools to 0
+            ref = x.masked_fill(~m[..., None], -math.inf).max(1).values
+            exact(got, torch.where(cnt > 0, ref, torch.zeros_like(ref)))
+        else:
+            # fp32 sum over the valid steps in order, then (avg) one division by the valid count (1 when none)
+            mf = m[..., None].double()
+            ref, absref = (x * mf).sum(1), (x.abs() * mf).sum(1)
+            if spec["mode"] == L.MPOOL_AVG:
+                ref, absref = ref / cnt.clamp_min(1), absref / cnt.clamp_min(1)
+            bound(got.double() if live else None, ref, absref, x.shape[1] + 2, acc_eps=SUM_EPS, rnd=_rnd(y))
+    elif k == "masked_default":
+        # x * a + default * (1 - a) in fp32, a = 1 where the row has a valid step: x or the default, exactly
+        y = spec["y"]
+        xr = inp["x_raw"].reshape(n, y.C).float()
+        a = (inp["mask"].any(1, keepdim=True) if inp["mask"] is not None else
+             torch.ones(n, 1, dtype=torch.bool)).float().to(xr.device)
+        want = xr * a + spec["default"].to(xr.device).view(1, -1) * (1 - a)
+        exact(ndhwc(y, clips).reshape(n, y.C) if live else None, want.to(_tdt(y)))
+    elif k == "copy_tokens":
+        x, y, r0 = spec["x"], spec["y"], spec["row0"]
+        got = ndhwc(y, clips).reshape(n, y.npos, y.C)[:, r0:r0 + x.npos] if live else None
+        exact(got, inp["x_raw"].reshape(n, x.npos, x.C))
+    elif k == "reduce_fusion":
+        y, parts = spec["y"], inp["parts"]
+        got = ndhwc(y, clips).reshape(n, y.npos, y.C) if live else None
+        if spec["op"] == L.REDUCE_MAX:
+            ref = parts[0]
+            for t in parts[1:]:
+                ref = torch.maximum(ref, t)
+            exact(got, ref.to(_tdt(y)))
+        else:
+            ref, absref = parts[0], parts[0].abs()
+            for t in parts[1:]:
+                ref, absref = (ref + t, absref + t.abs()) if spec["op"] == L.REDUCE_SUM else (ref * t, absref * t.abs())
+            bound(got.double() if live else None, ref, absref, len(parts), acc_eps=SUM_EPS, rnd=_rnd(y))
+    elif k == "attention_masked":
+        H, o = spec["heads"], spec["o"]
+        q, kk, v = (_heads(inp[m], H) for m in ("q", "k", "v"))
+        ref, absref = attn_ref64(q, kk, v, spec["scale"], False, mask=inp["mask"])
+        back = lambda t: t.permute(0, 2, 1, 3).reshape(n, t.shape[2], -1)        # noqa: E731
+        got = rows64(o, clips) if live else None
+        if not _is32(o):
+            extra = back(attn_score_extra64(q, kk, v, spec["scale"], inp["mask"]) +
+                         attn_p16_floor64(v, q.shape[2], inp["mask"]))
+            bound(got, back(ref), back(absref), 0, acc_eps=ACC_EPS_ATTN, extra=extra)
+        else:
+            extra = back(attn_score_extra64(q, kk, v, spec["scale"], inp["mask"]))
+            bound(got, back(ref), back(absref), kk.shape[2], acc_eps=ACC_EPS_ATTN_F32, extra=extra, rnd=F32_EPS)
+    elif k == "attention_weights":
+        H, wb = spec["heads"], spec["w"]
+        q, kk = (_heads(inp[m], H) for m in ("q", "k"))
+        Nq, Nk = q.shape[2], kk.shape[2]
+        ref, err = attn_weights_err64(q, kk, spec["scale"], inp["mask"])
+        got = buf_view(wb, (spec["q"].N, Nq, Nk))[clips] if live else None
+        bound(got, ref, err, 0, acc_eps=1.0, rnd=F32_EPS)
+    elif k == "lstm":
+        y, Hd, nd = spec["y"], spec["hidden"], spec["dirs"]
+        g = inp["g"]
+        T = g.shape[1]
+        m = inp["mask"]
+        lengths = (m.sum(1) if m is not None else torch.full((n,), T)).clamp(1, T)
+        cluster = "lstm_cluster_kernel" in launched
+        W = spec["w_hh_t"].half() if cluster else spec["w_hh_t"]
+        ref, err = lstm_ref64(g, W, lengths, Hd, nd, h16=cluster)
+        got = ndhwc(y, clips).reshape(n, -1) if live else None
+        # the propagated fp32 error is the whole accumulation term (acc_eps = 1, k_len = 0)
+        bound(got, ref, err, 0, acc_eps=1.0, rnd=_rnd(y))
+    elif k == "roi_align":
+        x, y = spec["x"], spec["y"]
+        rois = [tuple(float(v) for v in r) for r in inp["rois"]]
+        ref, absref = roi_ref64(inp["x"].cpu(), rois, spec["geom"])
+        got = ndhwc(y, list(range(y.N)))[:, 0] if live else None
+        bound(got, ref, absref, 0, acc_eps=roi_acc_eps(rois, spec["geom"], x.H, x.W), rnd=_rnd(y))
+    else:
+        raise AssertionError("no reference for %s" % k)
+    return out
+
+
+def _outputs(spec):
+    from .engine.plan import TRef
+    return [t for t in record_io(spec)[1] if isinstance(t, TRef)]
+
+
+def check_layout(spec, before):
+    """Pad channels of every TRef output are zero; channels of its rows outside [ch_off, ch_off + Cp) are as they were
+    before the op (other producers' slices of a concat buffer)."""
+    for i, t in enumerate(_outputs(spec)):
+        rows = full_rows(t)
+        pad = rows[..., t.ch_off + t.C:t.ch_off + t.Cp]
+        assert not bool(pad.any()), "pad channels [%d, %d) not zero" % (t.C, t.Cp)
+        if before[i] is not None:
+            was = before[i]
+            keep = torch.ones(t.row_stride, dtype=torch.bool, device=rows.device)
+            keep[t.ch_off:t.ch_off + t.Cp] = False
+            same = torch.equal(rows[..., keep], was[..., keep])
+            assert same, "channels outside this op's slice of the shared buffer changed"
+
+
+def channel_sum_adds(npos, C):
+    """The most positions one thread of pv_channel_sum adds in fp32 before its fixed-point atomic (chunks of at most
+    2048 positions, at most 1024 chunks; 256 threads share a chunk, 8 channels each)."""
+    chunks = min(-(-npos // 2048), 1024)
+    chunk = -(-npos // chunks)
+    per_iter = 256 // (-(-C // 8))
+    return chunk if per_iter == 0 else -(-chunk // per_iter)
+
+
+def audit_clips(B):
+    """The clips the audit compares: the first, the middle and the last (the first tiles, the middle and the last,
+    ragged tiles of every launch's walk)."""
+    return sorted({0, B // 2, B - 1})
+
+
+def audit_plan(plan, clips, corrupt=None, cpu_check=None):
+    """Walk the plan on one stream, comparing every op with its float64 reference.  Returns (failures, stats):
+    failures [(op index, name, message)], stats {family: (launches, largest err / tol, instances)}.
+    corrupt(i, spec): called after op i ran, before its comparison.  cpu_check: a dict filled with
+    {kind: largest relative difference between the float64 references computed on the GPU and on the CPU} for the
+    first op of each kind."""
+    from . import _lib as L
+    f32 = plan.dt == L.PV_F32
+    stream = torch.cuda.current_stream()
+    sp = stream.cuda_stream
+    failures, stats = [], {}
+    for i, ((name, fn), spec) in enumerate(zip(plan.ops, plan.op_spec)):
+        if spec is None:
+            assert name.endswith(NO_VALUE_SUFFIXES), name
+            fn(sp)
+            continue
+        try:
+            inp = gather_inputs(spec, clips)
+            before = [full_rows(t).clone() if (t.row_stride > t.Cp and t.padw is None) else None
+                      for t in _outputs(spec)]
+        except Exception as e:                          # noqa: BLE001 - reported with the op's name
+            failures.append((i, name, "reading inputs: %r" % e))
+            fn(sp)
+            continue
+        c0 = kernel_counts()
+        fn(sp)
+        torch.cuda.synchronize()
+        launched = kernel_count_diff(c0, kernel_counts())
+        fam = family_of(spec, f32)
+        key = spec["route"] if spec["kind"] == "conv" else spec["kind"]
+        if corrupt is not None:
+            corrupt(i, spec)
+        try:
+            assert launched and all(n.startswith(fam) for n in launched), \
+                "launched %s, outside the %s family" % (launched, key)
+            res = compare(spec, inp, clips, launched)
+            check_layout(spec, before)
+        except AssertionError as e:
+            failures.append((i, name, str(e)[:400]))
+            continue
+        if cpu_check is not None and spec["kind"] not in cpu_check:
+            gpu = compare(spec, inp, clips, launched, cpu_ref=torch.device("cuda"))
+            cpu = compare(spec, inp, clips, launched, cpu_ref=torch.device("cpu"))
+            rel = 0.0
+            for (_, g), (_, c) in zip(gpu, cpu):
+                g, c = g.double().cpu(), c.double().cpu()
+                rel = max(rel, float((g - c).abs().max()) / max(float(c.abs().max()), 1e-300))
+            cpu_check[spec["kind"]] = rel
+        n_, worst, inst = stats.get(key, (0, 0.0, set()))
+        stats[key] = (n_ + 1, max([worst] + [r for _, r in res]), inst | set(launched))
+    return failures, stats
+
+
+def _bits(t):
+    """Bit patterns: SE-sum buffers hold int64 fixed-point sums in f32 storage, some of which read as NaN."""
+    return t.view({torch.float16: torch.int16, torch.float32: torch.int32}.get(t.dtype, t.dtype))
+
+
+def check_graph_replay(cm, ins, alt):
+    """Capture the compiled model's plan as it runs in service (lanes on side streams, one CUDA graph) and replay it
+    on ``ins``, on ``alt`` and on ``ins`` again: after the first and the last replay every plan buffer must equal the
+    single-stream run that left the buffers as they are now, bit for bit (a lane reading a buffer before its
+    producer finished would see the other input's values).  Returns (lanes, buffers)."""
+    plan = cm.plan
+    single = [b.tensor.clone() for b in plan.bufs]
+    for b in plan.bufs:
+        b.tensor.zero_()
+    cm._capture()
+    for k, inputs in enumerate((ins, alt, ins)):
+        for s, t in zip(cm.static_in, inputs):
+            s.copy_(t)
+        cm.graph.replay()
+        torch.cuda.synchronize()
+        if k == 1:
+            continue
+        bad = [i for i, (b, s) in enumerate(zip(plan.bufs, single)) if not torch.equal(_bits(b.tensor), _bits(s))]
+        assert not bad, "replay %d: %d of %d buffers differ from the single-stream run (first: buffer %d)" % (
+            k, len(bad), len(single), bad[0])
+    return len(plan.sched["lanes"]), len(single)
+
 # ---- Non-local block cases (tests/golden/nonlocal.pt): name -> (create_nonlocal kwargs, input shape) ---------------
 NONLOCAL_CASES = {
     # I3D-NLN res3 / res4 widths (softmax, (1,2,2) pool): the wide tensor-core kernel at D = 256 / 512
@@ -565,6 +1539,24 @@ def build_nonlocal_case(name, create_nonlocal, seed=91):
     g = torch.Generator(device="cpu")
     g.manual_seed(seed + 1)
     return m, f16_exact(torch.randn(shape, generator=g))
+
+
+# I3D-R50 with the I3D-NLN layout of Non-local blocks: blocks[3] = res3, blocks[4] = res4 (blocks[2] is the stage-1
+# pool); block index -> residual blocks followed by a NonLocal of half their width
+I3D_NLN_LAYOUT = {3: (1, 3), 4: (1, 3, 5)}
+
+
+def build_i3d_nln(hub_module, create_nonlocal):
+    """(model, clip) of the I3D-NLN case: hub i3d_r50 with Non-local blocks after the I3D_NLN_LAYOUT residual blocks,
+    weights and a 2 x 8 x 224^2 clip on the f16 grid."""
+    model = hub_module.i3d_r50()
+    for stage, idx in I3D_NLN_LAYOUT.items():
+        blocks = model.blocks[stage].res_blocks
+        for i in idx:
+            c = blocks[i].branch2.conv_c.out_channels
+            blocks[i] = nn.Sequential(blocks[i], create_nonlocal(dim_in=c, dim_inner=c // 2, pool_size=(1, 2, 2)))
+    model = randomize_model(model, seed=1234, f16_weights=True).eval()
+    return model, synthetic_clip(2, 8, 224, 224, seed=42, f16_values=True)
 
 
 # ---- audio model / layer cases (tests/golden/audio.pt): name -> (builder, kwargs, inputs) ----------------------------
@@ -681,6 +1673,18 @@ def build_masked_case(name, ns, seed=1234):
         for p in m.parameters():
             p.copy_(torch.randn(p.shape) * (0.5 / max(1, p.shape[-1]) ** 0.5 if p.dim() > 1 else 0.2))
     return m.eval()
+
+
+def masked_namespace():
+    """This package's masked_multistream classes, ``PositionalEncoding`` and ``make_fusion_layer``: the namespace
+    build_masked_case takes."""
+    import types
+    import pytorchvideo_b200.layers as ML
+    import pytorchvideo_b200.models as MM
+    names = ("MaskedTemporalPooling", "LearnMaskedDefault", "TransposeMultiheadAttention", "TransposeTransformerEncoder",
+             "LSTM", "MaskedSequential", "MaskedMultiPathWay")
+    return types.SimpleNamespace(make_fusion_layer=ML.make_fusion_layer, PositionalEncoding=ML.PositionalEncoding,
+                                 **{n: getattr(MM, n) for n in names})
 
 
 def masked_engine_args(name, x, mask):

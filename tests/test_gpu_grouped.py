@@ -376,12 +376,10 @@ def test_grouped_expansion_instance(row):
         ops.conv3d_bn_act, x.to(_dev()), w, None, bn, s, p, dil, groups, act, None if res is None else res.to(_dev()), dtype)
     assert "grouped" not in stats and not any("grouped" in n for n in launched), (stats, launched)
     if dtype == "f32":
-        # f32 storage: one f32 rounding of the result plus the accumulation term of assert_close_to_f64
-        err = (got.double().cpu() - ref).abs()
-        tol = 2.0 ** -23 * ref.abs() + TS.ACC_EPS * (1 + ci // groups * int(np.prod(k)) / 64.0) * absref + 2.0 ** -40
+        # f32 storage: one fp32 rounding of the result plus the accumulation term of assert_close_to_f64
         assert any(n.startswith(name) for n in launched), launched
-        assert bool((err <= tol).all()), float((err / tol).max())
-        print("RATIO expanded %s-f32 %.4f %s" % (_gid(row), float((err / tol).max()), sorted(launched)))
+        ratio = TS.assert_close_to_f64(got, ref, absref, ci // groups * int(np.prod(k)), what=name, rnd_eps=TS.F32_EPS)
+        print("RATIO expanded %s-f32 %.4f %s" % (_gid(row), ratio[0], sorted(launched)))
         return
     _check_row(row, got, ref, absref, launched, "expanded")
 

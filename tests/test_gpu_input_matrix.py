@@ -35,7 +35,6 @@ import re
 import shutil
 import subprocess
 import zlib
-from fractions import Fraction
 
 import numpy as np
 import pytest
@@ -580,119 +579,16 @@ def test_rrc_window_edge_row(row):
 f32 = np.float32
 
 
-def _round32(q):
-    """A Fraction rounded to the nearest float32 (ties to even), without double rounding through float64."""
-    r = f32(float(q))
-    best = r
-    for cand in (np.nextafter(r, f32(-np.inf)), np.nextafter(r, f32(np.inf))):
-        d0, d1 = abs(Fraction(float(best)) - q), abs(Fraction(float(cand)) - q)
-        if d1 < d0 or (d1 == d0 and int(np.array(cand).view(np.int32)) % 2 == 0):
-            best = cand
-    return best
-
-
-def fma32(a, b, c):
-    return _round32(Fraction(float(a)) * Fraction(float(b)) + Fraction(float(c)))
-
-
-def roi_geometry(box, H, W, ph_n, pw_n, scale, sr, contract=False, mutation=None):
-    """torchvision's fp32 sampling geometry of one RoI (oracle.interp.roi_align_ref's arithmetic): per bin, the list
-    of kept samples (y_low, x_low, y_high, x_high, w1, w2, w3, w4), the count, and (grid_h, grid_w).
-    contract=True evaluates `end * scale - start` and `start + ph * bin` as single-rounding FMAs, as nvcc contracts
-    them unless told not to; mutation injects a known bug."""
-    s = f32(scale)
-    x1, y1, x2, y2 = (f32(v) for v in box[1:5])
-    sw, sh = x1 * s, y1 * s
-    if contract:
-        rw, rh = fma32(x2, s, -sw), fma32(y2, s, -sh)
-    else:
-        rw, rh = x2 * s - sw, y2 * s - sh
-    rw, rh = max(rw, f32(1)), max(rh, f32(1))
-    bh, bw = rh / f32(ph_n), rw / f32(pw_n)
-    rnd = np.floor if mutation == "floor" else np.ceil
-    gh = sr if sr > 0 else int(rnd(rh / f32(ph_n)))
-    gw = sr if sr > 0 else int(rnd(rw / f32(pw_n)))
-    count = max(gh * gw, 1)
-    half = f32(0) if mutation == "iy" else f32(0.5)
-    bins = []
-    for ph in range(ph_n):
-        st_y = fma32(f32(ph), bh, sh) if contract else sh + f32(ph) * bh
-        for pw in range(pw_n):
-            st_x = fma32(f32(pw), bw, sw) if contract else sw + f32(pw) * bw
-            samples = []
-            for iy in range(gh):
-                yy0 = st_y + (f32(iy) + half) * bh / f32(gh)
-                for ix in range(gw):
-                    xx = st_x + (f32(ix) + half) * bw / f32(gw)
-                    yy = yy0
-                    y_out = (yy >= H) if mutation == "ge_H" else (yy > H)
-                    if yy < -1 or y_out or xx < -1 or xx > W:
-                        continue
-                    yy, xx = max(yy, f32(0)), max(xx, f32(0))
-                    yl, xl = int(yy), int(xx)
-                    if yl >= H - 1:
-                        yh = yl = H - 1
-                        yy = f32(yl)
-                    else:
-                        yh = yl + 1
-                    if xl >= W - 1:
-                        xh = xl = W - 1
-                        xx = f32(xl)
-                    else:
-                        xh = xl + 1
-                    ly, lx = yy - f32(yl), xx - f32(xl)
-                    hy, hx = f32(1) - ly, f32(1) - lx
-                    samples.append((yl, xl, yh, xh, hy * hx, hy * lx, ly * hx, ly * lx))
-            bins.append(samples)
-    return bins, count, (gh, gw)
-
-
 def contraction_discontinuity(box, H, W, ph_n, pw_n, scale, sr):
     """Where the contracted geometry differs from torchvision's at a discontinuity: 'grid' (another ceil count) or
     'cutoff' (a sample on the other side of -1 / H / W), else None."""
-    a = roi_geometry(box, H, W, ph_n, pw_n, scale, sr)
-    b = roi_geometry(box, H, W, ph_n, pw_n, scale, sr, contract=True)
+    a = TS.roi_geometry(box, H, W, ph_n, pw_n, scale, sr)
+    b = TS.roi_geometry(box, H, W, ph_n, pw_n, scale, sr, contract=True)
     if a[2] != b[2]:
         return "grid"
     if [len(s) for s in a[0]] != [len(s) for s in b[0]]:
         return "cutoff"
     return None
-
-
-def roi_ref64(x, rois, row, mutation=None, emulate=False, contract=False):
-    """x [N, H, W, C]; returns (ref, absref) [K, ph, pw, C] in float64 (weights from the fp32 geometry), or the fp32
-    emulation in the kernel's order (acc += w1 v1 + w2 v2 + w3 v3 + w4 v4 per sample, then / count).  Invalid batch
-    indices give zeros.  contract: the geometry as nvcc contracts it (see roi_geometry)."""
-    N, H, W, C = x.shape
-    ph_n, pw_n, scale, sr = row[5], row[6], row[7], row[8]
-    dt = torch.float32 if emulate else torch.float64
-    X = x.to(dt)
-    out = torch.zeros(len(rois), ph_n * pw_n, C, dtype=dt)
-    absout = torch.zeros(len(rois), ph_n * pw_n, C, dtype=torch.float64)
-    for k, box in enumerate(rois):
-        n = int(box[0])
-        if not 0 <= n < N:
-            continue
-        bins, count, _ = roi_geometry(box, H, W, ph_n, pw_n, scale, sr, contract=contract, mutation=mutation)
-        Xn = X[n]
-        for b, samples in enumerate(bins):
-            acc = torch.zeros(C, dtype=dt)
-            mag = torch.zeros(C, dtype=torch.float64)
-            for (yl, xl, yh, xh, w1, w2, w3, w4) in samples:
-                v = (Xn[yl, xl], Xn[yl, xh], Xn[yh, xl], Xn[yh, xh])
-                acc = acc + (float(w1) * v[0] + float(w2) * v[1] + float(w3) * v[2] + float(w4) * v[3])
-                if not emulate:
-                    mag = mag + sum(float(w) * t.abs() for w, t in zip((w1, w2, w3, w4), v))
-            out[k, b] = acc / float(count)
-            absout[k, b] = mag / float(count)
-    shape = (len(rois), ph_n, pw_n, C)
-    return out.view(shape), absout.view(shape)
-
-
-def roi_acc_eps(rois, row, H, W):
-    """About 4 roundings per sample (the four products summed, the accumulation) plus one for the division."""
-    grids = [roi_geometry(b, H, W, row[5], row[6], row[7], row[8])[2] for b in rois]
-    return (4 * max(gh * gw for gh, gw in grids) + 1) * U
 
 
 # Boxes where nvcc's contraction of torchvision's geometry crosses a discontinuity and moves the result past its bound,
@@ -803,10 +699,10 @@ def test_roi_align_row(row):
     mask[:K * ph_n * pw_n * yrs].view(-1, yrs)[:, :C] = True
     _assert_untouched(out, mask, "y")
     got = out[:K * ph_n * pw_n * yrs].view(K, ph_n, pw_n, yrs)[..., :C]
-    ref, absref = roi_ref64(x, rois, row)
+    ref, absref = TS.roi_ref64(x, rois, row[5:9])
     if kind == "badn":
         assert bool((got[:2] == 0).all())
-    _ratio("roi", row, _bound(got, ref, absref, roi_acc_eps(rois, row, H, W), _rnd(dt), _rid(row)), launched)
+    _ratio("roi", row, _bound(got, ref, absref, TS.roi_acc_eps(rois, row[5:9], H, W), _rnd(dt), _rid(row)), launched)
 
 
 # =====================================================================================================================
@@ -896,10 +792,10 @@ def _check_batch(row, mutation=None):
 
 def _check_roi(row, mutation=None):
     x, rois = roi_inputs(row)
-    ref, absref = roi_ref64(x, rois, row)
-    emu, _ = roi_ref64(x, rois, row, mutation=mutation, emulate=True)
+    ref, absref = TS.roi_ref64(x, rois, row[5:9])
+    emu, _ = TS.roi_ref64(x, rois, row[5:9], mutation=mutation, emulate=True)
     got = _store(emu, row[0], mutation)
-    return _bound(got, ref, absref, roi_acc_eps(rois, row, row[2], row[3]), _rnd(row[0]),
+    return _bound(got, ref, absref, TS.roi_acc_eps(rois, row[5:9], row[2], row[3]), _rnd(row[0]),
                   "%s %s" % (_rid(row), mutation))
 
 
@@ -978,7 +874,7 @@ def test_roi_geometry_is_the_oracle():
     from oracle.interp import roi_align_ref
     for row in (ROI_ROWS[0], ROI_ROWS[3], ROI_ROWS[8], ROI_ROWS[-1]):
         x, rois = roi_inputs(row)
-        emu, _ = roi_ref64(x, rois, row, emulate=True)
+        emu, _ = TS.roi_ref64(x, rois, row[5:9], emulate=True)
         want = roi_align_ref(x.permute(0, 3, 1, 2), torch.tensor(rois, dtype=torch.float32), (row[5], row[6]), row[7],
                              row[8]).permute(0, 2, 3, 1)
         assert torch.equal(emu, want), _rid(row)
@@ -1009,21 +905,21 @@ def test_contraction_boxes_are_visible(i):
     for dt in ("f16", "f32"):
         row = _contract_row(dt, (scale, ph_n, pw_n, sr))
         x = roi_inputs(row)[0]
-        ref, absref = roi_ref64(x, [box], row)
-        eps = roi_acc_eps([box], row, row[2], row[3])
-        good, _ = roi_ref64(x, [box], row, emulate=True)
+        ref, absref = TS.roi_ref64(x, [box], row[5:9])
+        eps = TS.roi_acc_eps([box], row[5:9], row[2], row[3])
+        good, _ = TS.roi_ref64(x, [box], row[5:9], emulate=True)
         _bound(_store(good, dt), ref, absref, eps, _rnd(dt), "uncontracted")
-        bad, _ = roi_ref64(x, [box], row, emulate=True, contract=True)
+        bad, _ = TS.roi_ref64(x, [box], row[5:9], emulate=True, contract=True)
         with pytest.raises(AssertionError):
             _bound(_store(bad, dt), ref, absref, eps, _rnd(dt), "contracted")
 
 
 def test_rows_have_grids_of_one_and_of_at_least_eight():
-    grids = {roi_geometry(b, r[2], r[3], r[5], r[6], r[7], r[8])[2] for r in ROI_ROWS if r[8] == 0
+    grids = {TS.roi_geometry(b, r[2], r[3], r[5], r[6], r[7], r[8])[2] for r in ROI_ROWS if r[8] == 0
              for b in roi_inputs(r)[1]}
     assert (1, 1) in grids and any(min(g) >= 8 for g in grids)
     big = ROI_ROWS[4]
-    assert big[4] == 2048 and (9, 9) in {roi_geometry(b, big[2], big[3], big[5], big[6], big[7], 0)[2]
+    assert big[4] == 2048 and (9, 9) in {TS.roi_geometry(b, big[2], big[3], big[5], big[6], big[7], 0)[2]
                                           for b in roi_inputs(big)[1]}
 
 

@@ -11,7 +11,11 @@ brackets the largest share of the accumulation term a result used beyond its own
 accumulation constant; a correctly rounded f16 result may use nearly all of the rounding term):
   igemm 0.992 (0.017), window-mode igemm 0.920 (0.011), gather 0.989 (0.011), stem rows incl. the factored temporal
   stem 0.990 (0.133), depthwise 0.995 (0.020), attention wgmma 0.196 (0.097), attention mma 0.180 (0.092),
-  attention CUDA-core f16 / f32 0.142 / 0.0003 (0.0001).
+  attention CUDA-core f16 0.142.
+The f32 rows are held to fp32 bounds: the fp32 rounding term, and for attention_kernel<float, D> the fp32 attention
+bound (testing.ACC_EPS_ATTN_F32 over Nk, testing.attn_score_extra64).  Measured on an NVIDIA H100 80GB HBM3 (700 W
+power limit): attention CUDA-core f32 0.0087 (0.033), depthwise f32 0.133 (0.099), conv3d_direct_kernel<float>
+(DIRECT_F32_ROWS) 0.097 (0.084).
 
 The fused bottleneck block keeps its intermediates a and b in f16, so its bound also carries their rounding error
 propagated to y (fused_block_ref64).  Measured on an NVIDIA H100 80GB HBM3 (132 SMs, 700 W power limit) over every
@@ -236,7 +240,8 @@ def test_depthwise_instance(row):
         ops.conv3d_bn_act, x.to(_dev()), w, None, bn, s, p, (1, 1, 1), Cc, None, None, dtype, None, se_sums=se)
     assert name in launched, "expected %s, launched %s" % (name, launched)
     ntaps = int(np.prod(k))
-    ratio = TS.assert_close_to_f64(got, ref, absref, ntaps, what=name)
+    ratio = TS.assert_close_to_f64(got, ref, absref, ntaps, what=name,
+                                   rnd_eps=TS.F32_EPS if dtype == "f32" else TS.F16_EPS)
     print("RATIO depthwise %s %.4f %.4f %s" % (_row_id(row), ratio[0], ratio[1], sorted(launched)))
     if se:
         # fp32 sums of the pre-rounding outputs, quantised to 2^-24 per add: bounded by the per-element bound times
@@ -250,6 +255,59 @@ def test_depthwise_instance(row):
             # the generic path sums the STORED outputs (pv_channel_sum after the stencil): one rounding per element
             tol = tol + (TS.F16_EPS if dtype == "f16" else 2.0 ** -24) * ref.abs().sum(dim=(2, 3, 4))
         assert bool(((sums - ref_s).abs() <= tol).all()), float(((sums - ref_s).abs() / tol).max())
+
+
+# ---- the fp32 dense convolution (f32 parity mode: every dense convolution) ------------------------------------------
+# (N, Ci, T, H, W, Co, kernel, stride, padding, dilation, act, residual, addend): conv3d_direct_kernel<float> at its
+# edges - M (output rows) not a multiple of 64, Co not a multiple of 64, K = Ci * taps not a multiple of 16, strides,
+# dilations, paddings, a residual, and an addend per output frame (T' = To) or per clip (T' = 1) added after the
+# activation from a channel offset of a wider tensor.
+DIRECT_F32_ROWS = [
+    (1, 3, 4, 9, 11, 20, (3, 3, 3), (1, 1, 1), (1, 1, 1), (1, 1, 1), "relu", False, None),
+    (2, 24, 3, 10, 10, 72, (1, 3, 3), (1, 2, 2), (0, 1, 1), (1, 1, 1), "swish", True, None),
+    (1, 40, 5, 9, 9, 64, (3, 1, 1), (2, 1, 1), (2, 0, 0), (2, 1, 1), None, False, "frame"),
+    (2, 16, 2, 7, 13, 130, (1, 3, 3), (1, 1, 1), (0, 2, 2), (1, 2, 2), "gelu", True, "clip"),
+    (1, 8, 1, 5, 5, 8, (1, 1, 1), (1, 1, 1), (0, 0, 0), (1, 1, 1), "sigmoid", False, None),
+    (1, 200, 2, 6, 6, 96, (1, 1, 1), (1, 1, 1), (0, 0, 0), (1, 1, 1), "hswish", True, "clip"),
+]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("row", DIRECT_F32_ROWS,
+                         ids=["x".join(str(v) for v in r[:6]) + "-%s" % r[12] for r in DIRECT_F32_ROWS])
+def test_direct_f32_instance(row):
+    from pytorchvideo_b200 import _lib as L
+    from pytorchvideo_b200.engine import packing as PK
+    from pytorchvideo_b200.engine.plan import Plan
+    N, Ci, T, H, W, Co, k, s, p, dil, act, use_res, addend = row
+    g = torch.Generator().manual_seed(N + Ci + Co + T)
+    x = torch.randn(N, Ci, T, H, W, generator=g)
+    w = torch.randn(Co, Ci, *k, generator=g) * (2.0 / (Ci * int(np.prod(k)))) ** 0.5
+    bn = _bn(Co, Co + 1)
+    scale, bias = PK.fold_bn(None, bn, Co, Co)
+    To, Ho, Wo = F.conv3d(x[:1, :1], w[:1, :1], None, s, p, dil).shape[2:]
+    res = torch.randn(N, Co, To, Ho, Wo, generator=g) if use_res else None
+    off, ca = 8, Co + 16
+    add = torch.randn(N, ca, To if addend == "frame" else 1, 1, 1, generator=g) if addend else None
+    plan = Plan(_dev(), L.PV_F32)
+    xr = plan.emit_input_ncdhw(x.to(_dev()), Ci, PK.pad8(Ci))
+    rr = plan.materialize_input(plan.emit_input_ncdhw(res.to(_dev()), Co, PK.pad8(Co))) if use_res else None
+    ar = plan.materialize_input(plan.emit_input_ncdhw(add.to(_dev()), ca, PK.pad8(ca))) if addend else None
+    acts = {None: L.ACT_NONE, "relu": L.ACT_RELU, "swish": L.ACT_SWISH, "gelu": L.ACT_GELU, "sigmoid": L.ACT_SIGMOID,
+            "hswish": L.ACT_HSWISH}
+    y = plan.emit_conv(xr, w, None, bn, s, p, dil, 1, acts[act], rr, "conv", addend=(ar, off) if addend else None)
+    out, shape = plan.emit_to_ncdhw(y)
+    plan.finalize()
+    got, launched = TS.launched_kernels(lambda: (plan.run(torch.cuda.current_stream().cuda_stream),
+                                                 torch.cuda.synchronize()))
+    assert launched.get("conv3d_direct_kernel<float>") == 1, launched
+    got = out.tensor[:int(np.prod(shape))].view(*shape).cpu()
+    ref, absref = conv_ref64(x, w, scale, bias, s, p, dil, 1, act, res)
+    if addend:
+        a64 = add[:, off:off + Co].double()
+        ref, absref = ref + a64, absref + a64.abs()
+    ratio = TS.assert_close_to_f64(got, ref, absref, Ci * int(np.prod(k)), what="direct f32", rnd_eps=TS.F32_EPS)
+    print("RATIO direct-f32 %s %.4f %.4f" % ("x".join(str(v) for v in row[:6]), ratio[0], ratio[1]))
 
 
 # ---- attention -----------------------------------------------------------------------------------------------------
@@ -308,7 +366,12 @@ def test_attention_instance(row):
         want = (v.float() + (q.float() if resid else 0)).expand(B, H, Nq, D)     # the kernels' one fp32 add
         want = want if mode == "f32" else want.half().float()
         assert torch.equal(got.cpu(), want), float((got.cpu() - want).abs().max())
-    ratio = TS.assert_close_to_f64(got, ref, absref, 0, acc_eps=ACC_EPS_ATTN, what=name)
+    if mode == "f32":
+        # fp32 probabilities: the fp32 attention bound (ACC_EPS_ATTN_F32 over Nk, attn_score_extra64), fp32 rounding
+        ratio = TS.assert_close_to_f64(got, ref, absref, Nk, acc_eps=TS.ACC_EPS_ATTN_F32, what=name,
+                                       extra64=TS.attn_score_extra64(q, k, v, scale), rnd_eps=TS.F32_EPS)
+    else:
+        ratio = TS.assert_close_to_f64(got, ref, absref, 0, acc_eps=ACC_EPS_ATTN, what=name)
     print("RATIO attention %s-%s-%dx%d-D%d %.4f %.4f" % (name, mode, Nq, Nk, D, ratio[0], ratio[1]))
 
 

@@ -14,7 +14,6 @@ after a nested forward, one plan replayed with two masks, caller tensors left un
 import ctypes as C
 import os
 import re
-import types
 
 import pytest
 import torch
@@ -37,12 +36,7 @@ MASKED_F16_BOUNDS = {"pool_max": 6e-4, "pool_avg": 1e-3, "pool_sum": 9e-4, "pool
 
 
 def _ns():
-    import pytorchvideo_b200.layers as ML
-    import pytorchvideo_b200.models as MM
-    names = ("MaskedTemporalPooling", "LearnMaskedDefault", "TransposeMultiheadAttention", "TransposeTransformerEncoder",
-             "LSTM", "MaskedSequential", "MaskedMultiPathWay")
-    return types.SimpleNamespace(make_fusion_layer=ML.make_fusion_layer, PositionalEncoding=ML.PositionalEncoding,
-                                 **{n: getattr(MM, n) for n in names})
+    return TS.masked_namespace()
 
 
 def _lib():
@@ -310,12 +304,9 @@ def _desc(dtype, B, H, N, D, W):
 def _ref64(qkv, B, H, N, D, mask):
     x = qkv.double().cpu()
     q, k, v = (x[..., i * H * D:(i + 1) * H * D].reshape(B, N, H, D).transpose(1, 2) for i in range(3))
-    s = (q * D ** -0.5) @ k.transpose(-1, -2)
-    s = s.masked_fill(~mask[:, None, None, :], float("-inf"))
-    p = torch.softmax(s, -1).nan_to_num(0.0)
-    o = (p @ v).transpose(1, 2).reshape(B, N, H * D)
-    ao = (p @ v.abs()).transpose(1, 2).reshape(B, N, H * D)
-    return o, ao, p
+    o, ao = TS.attn_ref64(q, k, v, D ** -0.5, False, mask=mask)
+    p = TS.attn_probs64(q, k, D ** -0.5, mask)
+    return o.transpose(1, 2).reshape(B, N, H * D), ao.transpose(1, 2).reshape(B, N, H * D), p
 
 
 @pytest.mark.gpu
@@ -372,27 +363,6 @@ def test_gpu_all_valid_mask_is_bitwise_unmasked(dtype, D, aligned):
     assert torch.equal(o, o2)
 
 
-def _lstm_ref64(G, W, lengths, H, nd, h16=False):
-    """float64 restatement of the recurrence on the operands the kernel received: G [B][T][nd*4H], W^T [nd][H][4H];
-    h16: h enters the product rounded to f16 (the tensor-core operand of the f16 kernel)."""
-    G, W = G.double().cpu(), W.double().cpu()
-    B = G.shape[0]
-    out = torch.zeros(B, nd * H, dtype=torch.float64)
-    for b in range(B):
-        n = int(lengths[b])
-        for d in range(nd):
-            h = torch.zeros(H, dtype=torch.float64)
-            c = torch.zeros(H, dtype=torch.float64)
-            for s in range(n):
-                t = s if d == 0 else n - 1 - s
-                z = G[b, t, d * 4 * H:(d + 1) * 4 * H] + (h.half().double() if h16 else h) @ W[d]
-                i, f, g, o = z[:H].sigmoid(), z[H:2 * H].sigmoid(), z[2 * H:3 * H].tanh(), z[3 * H:].sigmoid()
-                c = f * c + i * g
-                h = o * c.tanh()
-            out[b, d * H:(d + 1) * H] = h
-    return out
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("row", LSTM_ROWS, ids=[r[0] for r in LSTM_ROWS])
 @pytest.mark.parametrize("B,T,H,nd", LSTM_SHAPES)
@@ -429,7 +399,8 @@ def _lstm_check(inst, dtype, B, T, H, nd):
         torch.cuda.synchronize()
     _, launched = TS.launched_kernels(run)
     assert launched == {inst: 1}
-    ref = _lstm_ref64(G, W.half() if inst == "lstm_cluster_kernel" else W, lengths, H, nd, h16=inst == "lstm_cluster_kernel")
+    ref, _ = TS.lstm_ref64(G, W.half() if inst == "lstm_cluster_kernel" else W, lengths, H, nd,
+                           h16=inst == "lstm_cluster_kernel")
     err = float((y[:, :nd * H].double().cpu() - ref).abs().max())
     assert err <= (2e-3 if dtype == "f16" else 2e-5), err
     assert bool((y[:, nd * H:] == 9.0).all())                       # nothing written past the row

@@ -166,10 +166,6 @@ PRE_CASES = [
 ]
 
 
-def _gelu64(v):
-    return 0.5 * v * (1.0 + torch.erf(v / 2.0 ** 0.5))
-
-
 def _run_pre(dtype, T, H, k, s, C, N, entry, seed):
     g = torch.Generator().manual_seed(seed)
     tdt = torch.float16 if dtype == "f16" else torch.float32
@@ -211,11 +207,9 @@ def _run_pre(dtype, T, H, k, s, C, N, entry, seed):
         torch.cuda.synchronize()
     _, ran = TS.launched_kernels(launch)
     xin = x[:, 1:, :C].double().cpu().reshape(N, T, H, H, C).permute(0, 4, 1, 2, 3)
-    u = _gelu64(xin * pre_s.double().view(1, C, 1, 1, 1) + pre_b.double().view(1, C, 1, 1, 1))
     w64 = w.double()
-    sc, bi = scale.double().view(1, C, 1, 1, 1), bias.double().view(1, C, 1, 1, 1)
-    ref = F.conv3d(u, w64, stride=s, padding=pad, groups=C) * sc + bi
-    absref = F.conv3d(u.abs(), w64.abs(), stride=s, padding=pad, groups=C) * sc.abs() + bi.abs()
+    ref, absref, u, _ = TS.prologue_conv_ref64(xin, pre_s, pre_b, w64, scale, bias, s, pad)
+    sc = scale.double().view(1, C, 1, 1, 1)
     got = y[:, 1:].float().cpu().reshape(N, To, Ho, Ho, C).permute(0, 4, 1, 2, 3)
     return got, ref, absref, y, ran, u, w64, sc, pad
 

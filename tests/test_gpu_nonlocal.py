@@ -232,19 +232,7 @@ def test_instance_ledger_covers_every_wide_instance():
 
 def _ref64(q, k, v, scale, normalize, resid=False):
     """q [B,Nq,D], k / v [B,Nk,D] on the f16 grid -> (ref64, absref64)."""
-    q64, k64, v64 = q.double(), k.double(), v.double()
-    s = (q64 @ k64.transpose(-2, -1)) * scale
-    if normalize:
-        nk = k.shape[1]
-        p = s / nk
-        absp = (q64.abs() @ k64.abs().transpose(-2, -1)) * abs(scale) / nk
-    else:
-        p = s.softmax(-1)
-        absp = p
-    ref, absref = p @ v64, absp @ v64.abs()
-    if resid:
-        ref, absref = ref + q64, absref + q64.abs()
-    return ref, absref
+    return TS.attn_ref64(q, k, v, scale, resid, normalize)
 
 
 ACC_EPS_ATTN = 2.0 ** -9       # P is rounded to f16 before P.V (tests/test_gpu_kernel_matrix.py, same bound)
@@ -440,21 +428,10 @@ def test_nonlocal_transmute_route():
 
 
 # ---- GPU model: i3d_r50 with the I3D-NLN layout of Non-local blocks ----------------------------------------------
-NL_LAYOUT = {3: (1, 3), 4: (1, 3, 5)}      # blocks[3] = res3, blocks[4] = res4 (blocks[2] is the stage-1 pool)
-
-
 def _i3d_nln():
     import pytorchvideo_b200.models.hub as PH
     from pytorchvideo_b200.layers.nonlocal_net import create_nonlocal
-    model = PH.i3d_r50()
-    for stage, idx in NL_LAYOUT.items():
-        blocks = model.blocks[stage].res_blocks
-        for i in idx:
-            C_ = blocks[i].branch2.conv_c.out_channels
-            blocks[i] = nn.Sequential(blocks[i], create_nonlocal(dim_in=C_, dim_inner=C_ // 2, pool_size=(1, 2, 2)))
-    model = TS.randomize_model(model, seed=1234, f16_weights=True).eval()
-    clip = TS.synthetic_clip(2, 8, 224, 224, seed=42, f16_values=True)
-    return model, clip
+    return TS.build_i3d_nln(PH, create_nonlocal)
 
 
 # (min fraction of logits inside rtol 1e-3 / atol 1e-4*scale, max |d|/max|ref|): measured values with a small margin.
