@@ -265,7 +265,9 @@ extern "C" int pv_dwplane_fwd(const pv_conv3d_desc* d, const void* x, const void
   P.nt_n = (d->N + P.bn - 1) / P.bn; P.nt_h = (d->Ho + P.bh - 1) / P.bh; P.nt_w = (d->Wo + P.bw - 1) / P.bw;
   const long long tiles = (long long)P.nt_n * P.nt_h * P.nt_w;
   if (tiles > 0x7fffffffll || chunks > 65535) { set_error("pv_dwplane_fwd: grid too large"); return PV_ERR_UNSUPPORTED; }
-  {
+  // stride 4 reads x straight from global memory: no tensor map (its box, sized without the shared-memory budget, can
+  // be one the driver rejects, as for the image MViT's 56x56 K/V pool at batch 3)
+  if (S != 4) {
     const long long rs = d->x_row_stride * 2;
     const long long xbs = (d->x_batch_stride ? d->x_batch_stride : (long long)d->Hi * d->Wi * d->x_row_stride) * 2;
     cuuint64_t gdim[5] = {(cuuint64_t)d->Ci, (cuuint64_t)d->Wi, (cuuint64_t)d->Hi, 1, (cuuint64_t)d->N};

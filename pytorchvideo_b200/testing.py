@@ -892,8 +892,7 @@ def mask_bool(mask, clips):
     """The (n, T) bool mask a MaskRef holds for the selected clips (None: every step valid)."""
     if mask is None:
         return None
-    t = mask.tensor if mask.tensor is not None else mask.buf.tensor[:mask.B * mask.T].view(mask.B, mask.T)
-    return t.view(mask.B, mask.T)[clips] != 0
+    return record_rows(None, mask)[clips] != 0
 
 
 def io_buffers(items):
@@ -942,14 +941,76 @@ def rows64(t, clips):
     return ndhwc(t, clips).reshape(len(clips), t.npos, t.C).double()
 
 
+def span64(spec, t, clips, role):
+    """[n, rows, C] float64 of the token rows of TRef t the record's op reads or writes (record_rows)."""
+    return record_rows(spec, t, role)[clips].reshape(len(clips), -1, t.C).double()
+
+
 def buf_view(b, shape):
     n = math.prod(shape)
     return b.tensor[:n].view(*shape)
 
 
-def se_sums64(b, N, Cp, C, clips):
-    """The int64 fixed-point (2^-24) per-(sample, channel) sums an SE accumulator holds, as float64."""
-    return b.tensor[:2 * N * Cp].view(torch.int64).view(N, Cp)[clips, :C].double() * 2.0 ** -24
+def token_span(spec, t, role):
+    """The token rows of TRef t that the record's op reads (role "read") or writes ("write") when that is not all of
+    them (a slice), else None: the class-token rows another op writes, or the one row an op takes from its input."""
+    k, cls = spec["kind"], spec.get("cls") or 0
+    x, y = spec.get("x"), spec.get("y")
+    if role == "write" and t is y:
+        if k in ("pool", "token_conv") and cls:
+            return slice(cls, None)
+        if k == "copy_cls":
+            return slice(0, 1)
+        if k == "copy_tokens":
+            return slice(spec["row0"], spec["row0"] + x.npos)
+    if role == "read" and x is not y:
+        if k in ("pool", "token_conv") and cls and t is x:
+            return slice(cls, None)
+        if k == "layernorm_sets" and cls and (t is x or t is y):
+            return slice(0, cls) if t is x else slice(cls, None)      # the class rows from x, the others in place
+        if (k == "copy_cls" or (k == "layernorm" and spec["first_row_only"])) and t is x:
+            return slice(0, 1)
+    return None
+
+
+def record_rows(spec, t, role=None):
+    """The values an operand of a record holds, as a view [N, ...] whose first axis is the clip (the RoI for the
+    tensors a RoIAlign head computes per box), without the pad channels and without the other producers' channels of
+    a shared buffer.  t: a TRef, a MaskRef, a Buf the record reads or writes (its layout follows from the record's
+    kind), the record's RoIs (their coordinates), or a plain tensor (a staged plan input, taken as it is).  role
+    "read" / "write": only the token rows the op reads / writes (token_span), as [N, rows, C]."""
+    from .engine.plan import MaskRef, TRef
+    if torch.is_tensor(t):
+        return t
+    if isinstance(t, TRef):
+        v = full_rows(t)[..., t.ch_off:t.ch_off + t.C]
+        span = token_span(spec, t, role) if role is not None else None
+        return v if span is None else v.reshape(t.N, t.npos, t.C)[:, span]
+    if spec is not None and t is spec.get("rois"):
+        return t.tensor[:, 1:]
+    if isinstance(t, MaskRef) or all(hasattr(t, a) for a in ("B", "T", "tensor", "buf")):
+        return (t.tensor if t.tensor is not None else t.buf.tensor[:t.B * t.T]).view(t.B, t.T)
+    for v in spec.values():
+        if isinstance(v, MaskRef) and v.buf is t:
+            return record_rows(spec, v)
+    k = spec["kind"]
+    if k == "to_f32":
+        x = spec["x"]
+        return buf_view(t, (x.N, x.C, x.T, x.H, x.W) if spec["layout"] == "ncdhw" else (x.N, x.npos, x.C))
+    if k == "head_reduce":
+        return buf_view(t, (spec["x"].N, spec["x"].C))
+    if t is spec.get("gate"):
+        x = spec["x"]
+        return buf_view(t, (x.N, x.Cp))[:, :x.C]
+    if t is spec.get("sums") or t is spec.get("se_sums"):
+        # an SE accumulator: int64 fixed-point (2^-24) sums per (sample, channel)
+        x = spec["y"] if k == "conv" else spec["x"]
+        return t.tensor[:2 * x.N * x.Cp].view(torch.int64).view(x.N, x.Cp)[:, :x.C]
+    if t is spec.get("lse"):
+        return buf_view(t, (spec["q"].N, spec["heads"] * spec["q"].npos))
+    if k == "attention_weights" and t is spec["w"]:
+        return buf_view(t, (spec["q"].N, spec["q"].npos, spec["k"].npos))
+    raise AssertionError("%s: no per-clip layout for operand %r" % (k, t))
 
 
 def _grid(rows, cls, thw):
@@ -1003,24 +1064,22 @@ def gather_inputs(spec, clips):
         return {"x": ncdhw64(spec["x"], clips)}
     if k in ("pool", "token_conv", "copy_cls", "pos_cls", "head_reduce", "layernorm", "to_f32", "copy",
              "channel_affine"):
-        return {"x": rows64(spec["x"], clips), "x_raw": ndhwc(spec["x"], clips)}
+        return {"x": span64(spec, spec["x"], clips, "read"), "x_raw": ndhwc(spec["x"], clips)}
     if k == "se_gate":
         x = spec["x"]
-        return {"sums": se_sums64(spec["sums"], x.N, x.Cp, x.C, clips)}
+        return {"sums": record_rows(spec, spec["sums"])[clips].double() * 2.0 ** -24}
     if k == "scale_act":
         x = spec["x"]
-        g = buf_view(spec["gate"], (x.N, x.Cp))[clips, :x.C].double() if spec["gate"] is not None else None
+        g = record_rows(spec, spec["gate"])[clips].double() if spec["gate"] is not None else None
         return {"x": rows64(x, clips), "gate": g}
     if k == "add_layernorm":
         return {"a": rows64(spec["a"], clips).float(), "br": rows64(spec["br"], clips).float()}
     if k == "layernorm_sets":
-        return {"x": rows64(spec["x"], clips), "y": rows64(spec["y"], clips)}
+        return {"x": span64(spec, spec["x"], clips, "read"), "y": span64(spec, spec["y"], clips, "read")}
     if k == "attention":
         return {n: rows64(spec[n], clips) for n in ("q", "k", "v")}
     if k == "mask_force_first":
-        m = spec["mask"]
-        src = m.tensor if m.tensor is not None else m.buf.tensor[:m.B * m.T]
-        return {"src": src.view(m.B, m.T)[clips].clone()}
+        return {"src": record_rows(spec, spec["mask"])[clips].clone()}
     if k in ("masked_pool", "masked_default", "copy_tokens"):
         return {"x": rows64(spec["x"], clips), "x_raw": ndhwc(spec["x"], clips),
                 "mask": mask_bool(spec.get("mask"), clips)}
@@ -1086,11 +1145,9 @@ def compare(spec, inp, clips, launched, cpu_ref=False):
         x, o = spec["x"], spec["out"]
         if spec["layout"] == "ncdhw":
             want = inp["x_raw"].permute(0, 4, 1, 2, 3)
-            got = buf_view(o, (x.N, x.C, x.T, x.H, x.W))[clips] if live else None
         else:
             want = inp["x_raw"].reshape(n, x.npos, x.C)
-            got = buf_view(o, (x.N, x.npos, x.C))[clips] if live else None
-        exact(got, want.float())
+        exact(record_rows(spec, o)[clips] if live else None, want.float())
     elif k == "copy":
         exact(ndhwc(spec["y"], clips) if live else None, inp["x_raw"])
     elif k == "conv":
@@ -1114,7 +1171,7 @@ def compare(spec, inp, clips, launched, cpu_ref=False):
                 out.append(("se_sums", ref_s))
             else:
                 # the SE-sum bound of test_depthwise_instance (fp32 sums of the pre-rounding outputs, fixed point)
-                sums = se_sums64(spec["se_sums"], y.N, y.Cp, y.C, clips).cpu()
+                sums = (record_rows(spec, spec["se_sums"])[clips].double() * 2.0 ** -24).cpu()
                 ref_s, absref_s = ref_s.cpu(), absref.sum(dim=(2, 3, 4)).cpu()
                 tol = 2.0 ** -20 * (1 + ntaps / 64.0) * absref_s + npos * 2.0 ** -23 + 2.0 ** -22 * ref_s.abs()
                 if any(i.startswith(("dwconv3d_kernel<", "dwconv3d_w4_kernel<")) for i in launched):
@@ -1157,10 +1214,10 @@ def compare(spec, inp, clips, launched, cpu_ref=False):
     elif k == "pool":
         x, y, cls = spec["x"], spec["y"], spec["cls"]
         thw = spec.get("thw", (x.T, x.H, x.W))
-        g = _grid(inp["x"], cls, thw)
+        g = _grid(inp["x"], 0, thw)
         kk, s, p = spec["kernel"], spec["stride"], spec["padding"]
         pad = (p[2], p[2], p[1], p[1], p[0], p[0])
-        got = rows64(y, clips)[:, cls:] if live else None
+        got = span64(spec, y, clips, "write") if live else None
         if spec["mode"] == L.POOL_MAX:
             ref = F.max_pool3d(F.pad(g, pad, value=-math.inf), kk, s)
             exact(got.to(_tdt(y)) if live else None, _rows_of(ref).to(_tdt(y)))
@@ -1172,11 +1229,11 @@ def compare(spec, inp, clips, launched, cpu_ref=False):
             bound(got, _rows_of(ref), _rows_of(absref), K, acc_eps=SUM_EPS, rnd=_rnd(y))
     elif k == "token_conv":
         x, y, cls = spec["x"], spec["y"], spec["cls"]
-        g = _grid(inp["x"], cls, spec["thw"])
+        g = _grid(inp["x"], 0, spec["thw"])
         w = _wq(spec["weight"], y)
         C = w.shape[0]
         ones = torch.ones(C, dtype=torch.float64)
-        got = rows64(y, clips)[:, cls:] if live else None
+        got = span64(spec, y, clips, "write") if live else None
         if not spec["prologue"]:
             ref, absref = conv_ref64(g, w, ones, torch.zeros_like(ones), spec["stride"], spec["padding"],
                                      spec["dilation"], C, "none", None)
@@ -1197,8 +1254,7 @@ def compare(spec, inp, clips, launched, cpu_ref=False):
         got = rows64(y, clips) if live else None
         bound(got, v * sc + sh, v.abs() * sc.abs() + sh.abs(), 1, rnd=_rnd(y))
     elif k == "copy_cls":
-        exact(rows64(spec["y"], clips)[:, 0].to(_tdt(spec["y"])) if live else None,
-              inp["x_raw"].reshape(n, -1, spec["x"].C)[:, 0])
+        exact(record_rows(spec, spec["y"], "write")[clips] if live else None, inp["x"])
     elif k == "pos_cls":
         y = spec["y"]
         xr = inp["x_raw"].reshape(n, -1, spec["x"].C).float()
@@ -1213,7 +1269,7 @@ def compare(spec, inp, clips, launched, cpu_ref=False):
     elif k == "head_reduce":
         x64 = inp["x"]
         C = x64.shape[2]
-        got = buf_view(spec["out"], (spec["x"].N, C))[clips] if live else None
+        got = record_rows(spec, spec["out"])[clips] if live else None
         if not spec["softmax"]:
             bound(got, x64.mean(1), x64.abs().mean(1), x64.shape[1] + 1, acc_eps=SUM_EPS, rnd=F32_EPS)
         else:
@@ -1234,7 +1290,7 @@ def compare(spec, inp, clips, launched, cpu_ref=False):
         Hm = b1.abs() + mean.abs() @ w1.abs().t()
         A = b2.abs() + Hm @ w2.abs().t()
         extra = gate * (1 - gate) * (2 + 1.173 * a.abs()) * 2.0 ** -23 + F32_EPS * gate
-        got = buf_view(spec["gate"], (x.N, x.Cp))[clips, :x.C] if live else None
+        got = record_rows(spec, spec["gate"])[clips] if live else None
         bound(got, gate, 0.25 * A, x.C + w1.shape[0] + 3, acc_eps=SUM_EPS, extra=extra, rnd=F32_EPS)
     elif k == "scale_act":
         y = spec["y"]
@@ -1245,7 +1301,7 @@ def compare(spec, inp, clips, launched, cpu_ref=False):
         got = rows64(y, clips) if live else None
         bound(got, act64(v, act), LIP[act] * v.abs(), 0, acc_eps=F32_EPS, extra=act_err64(v, act), rnd=_rnd(y))
     elif k == "layernorm":
-        v = inp["x"][:, :1] if spec["first_row_only"] else inp["x"]
+        v = inp["x"]
         C = v.shape[2]
         name = next(iter(launched))
         _, lpr, nch = ln_dispatch(C) if name in ("layernorm_reg_kernel", "add_layernorm_kernel") else \
@@ -1267,9 +1323,7 @@ def compare(spec, inp, clips, launched, cpu_ref=False):
             bound(got, ref, absref, K, acc_eps=SUM_EPS, extra=extra, rnd=_rnd(spec["y"]))
     elif k == "layernorm_sets":
         y, cls, hd = spec["y"], spec["cls"], spec["head_dim"]
-        v = inp["y"].clone()
-        if cls:
-            v[:, 0] = inp["x"][:, 0]
+        v = torch.cat([inp["x"], inp["y"]], 1) if cls and spec["x"] is not y else inp["y"]
         C = v.shape[2]
         G = C // hd
         nsets = spec["gamma"].numel() // hd
@@ -1305,8 +1359,7 @@ def compare(spec, inp, clips, launched, cpu_ref=False):
         if not live:
             out.append((k, want.double()))
         else:
-            o = spec["out"]
-            got = o.buf.tensor[:o.B * o.T].view(o.B, o.T)[clips]
+            got = record_rows(spec, spec["out"])[clips]
             assert torch.equal(got, want.to(got.device)), "mask_force_first: the mask copy differs"
             out.append((k, 0.0))
     elif k == "masked_pool":
@@ -1335,9 +1388,8 @@ def compare(spec, inp, clips, launched, cpu_ref=False):
         want = xr * a + spec["default"].to(xr.device).view(1, -1) * (1 - a)
         exact(ndhwc(y, clips).reshape(n, y.C) if live else None, want.to(_tdt(y)))
     elif k == "copy_tokens":
-        x, y, r0 = spec["x"], spec["y"], spec["row0"]
-        got = ndhwc(y, clips).reshape(n, y.npos, y.C)[:, r0:r0 + x.npos] if live else None
-        exact(got, inp["x_raw"].reshape(n, x.npos, x.C))
+        x, y = spec["x"], spec["y"]
+        exact(record_rows(spec, y, "write")[clips] if live else None, inp["x_raw"].reshape(n, x.npos, x.C))
     elif k == "reduce_fusion":
         y, parts = spec["y"], inp["parts"]
         got = ndhwc(y, clips).reshape(n, y.npos, y.C) if live else None
@@ -1369,7 +1421,7 @@ def compare(spec, inp, clips, launched, cpu_ref=False):
         q, kk = (_heads(inp[m], H) for m in ("q", "k"))
         Nq, Nk = q.shape[2], kk.shape[2]
         ref, err = attn_weights_err64(q, kk, spec["scale"], inp["mask"])
-        got = buf_view(wb, (spec["q"].N, Nq, Nk))[clips] if live else None
+        got = record_rows(spec, wb)[clips] if live else None
         bound(got, ref, err, 0, acc_eps=1.0, rnd=F32_EPS)
     elif k == "lstm":
         y, Hd, nd = spec["y"], spec["hidden"], spec["dirs"]
@@ -1508,6 +1560,482 @@ def check_graph_replay(cm, ins, alt):
         assert not bad, "replay %d: %d of %d buffers differ from the single-stream run (first: buffer %d)" % (
             k, len(bad), len(single), bad[0])
     return len(plan.sched["lanes"]), len(single)
+
+
+# ---- the audit catalogue at any batch, and bitwise invariance across clip positions and batch sizes ----------------
+# (tests/test_gpu_model_audit.py, tests/test_gpu_batch_audit.py)
+def audit_catalogue(workloads):
+    """[(family, case, is a workload shape)] in a fixed order: every case the suite compiles.  workloads: bench.py's
+    WORKLOADS (the architecture / shape pairs the workload audit runs in f16)."""
+    shapes = {(v[0], v[2], v[3], v[4]) for v in workloads.values()}
+    cases = []
+    for name, (hub, kw, B, T, H, W, _) in sorted(MODEL_CASES.items()):
+        if name[:3] in ("c1_", "c2_", "c3_", "c4_") or name.endswith("_f16w"):
+            continue
+        cases.append(("model", name, not kw and (hub, T, H, W) in shapes))
+    cases += [("hub_tail", c, False) for c in sorted(HUB_TAIL_CASES)]
+    cases += [("grouped", c, False) for c in sorted(GROUPED_MODEL_CASES) if not c.endswith("_f16w")]
+    cases += [("detection", c, False) for c in sorted(DETECTION_CASES)]
+    cases += [("audio", c, False) for c in sorted(AUDIO_CASES)]
+    cases += [("efficient", c, False) for c in sorted(EFFICIENT_CASES)]
+    cases += [("mvit_variant", c, False) for c in sorted(MVIT_VARIANT_CASES)]
+    cases += [("nonlocal", c, False) for c in sorted(NONLOCAL_CASES)]
+    cases += [("nonlocal", "i3d_nln", False)]
+    cases += [("masked", c, False) for c in MASKED_CASES]
+    return cases
+
+
+def audit_cases(workloads):
+    """[(precision, family, case)] the model audit runs: f16 less the workload shapes, f32 all of them."""
+    cat = audit_catalogue(workloads)
+    return [("f16", f, c) for f, c, w in cat if not w] + [("f32", f, c) for f, c, _ in cat]
+
+
+def batch_sweep(workloads):
+    """[(precision, family, case, batch, checks)] of the batch audit; checks "abc" = float64 on every clip, position
+    invariance and batch-size invariance, "bc" = the two bitwise checks (the workload audit runs float64 there)."""
+    rows = []
+    for arch in sorted(workloads):
+        for B in ((1, 3) if arch == "x3d_xs" else (2, 3)):
+            rows.append(("f16", "model", arch, B, "abc"))
+        rows.append(("f16", "model", arch, workloads[arch][1], "bc"))
+    rows += [("f16", f, c, 3, "abc") for p, f, c in audit_cases(workloads) if p == "f16"]
+    rows += [("f32", "model", c, 3, "abc") for c in ("x3d_xs", "mvit_base_8x112")]
+    rows += [("f32", "masked", c, 3, "abc") for c in MASKED_CASES]
+    rows += [("f32", "detection", c, 3, "abc") for c in sorted(DETECTION_CASES)]
+    rows += [(p, "ssl", c, B, "abc") for p in ("f16", "f32") for c in SSL_TRUNK_CASES for B in (1, 2, 3)]
+    return rows
+
+
+def build_audit_case(family, case):
+    """(model, engine inputs (a tensor or a list), extra, indices of inputs that stay fixed on the replay) of a case of
+    the audit catalogue."""
+    import pytorchvideo_b200.models as M
+    import pytorchvideo_b200.models.hub as PH
+    extra, fixed = (), set()
+    if family == "model":
+        m, x, _ = build_case(case, PH)
+    elif family == "hub_tail":
+        m, x = build_hub_tail_case(case, PH)
+    elif family == "grouped":
+        m, x, _ = build_grouped_case(case, PH)
+    elif family == "detection":
+        m, x, boxes, _ = build_detection_case(case, PH)
+        x = (x if isinstance(x, list) else [x]) + [boxes]
+        fixed = {len(x) - 1}
+    elif family == "audio":
+        m, x = build_audio_case(case, M)
+    elif family == "efficient":
+        m, x = build_efficient_case(case, efficient_namespace())
+    elif family == "mvit_variant":
+        from pytorchvideo_b200.layers.attention import MultiScaleBlock
+        from pytorchvideo_b200.models.vision_transformers import create_multiscale_vision_transformers
+        m, x, ex = build_mvit_variant_case(case, create_multiscale_vision_transformers, MultiScaleBlock)
+        extra = tuple(tuple(e) for e in ex)
+    elif family == "nonlocal":
+        from pytorchvideo_b200.layers.nonlocal_net import create_nonlocal
+        if case == "i3d_nln":
+            m, x = build_i3d_nln(PH, create_nonlocal)
+        else:
+            m, x = build_nonlocal_case(case, create_nonlocal)
+    elif family == "ssl":
+        m, x = build_ssl_trunk(case)
+    else:
+        m = build_masked_case(case, masked_namespace())
+        x, mask = masked_case_inputs(case)
+        x, extra = masked_engine_args(case, x, mask)
+        fixed = {i for i, t in enumerate(x if isinstance(x, list) else [x]) if t.dtype == torch.bool}
+    return m, x, extra, fixed
+
+
+SSL_TRUNK_CASES = ("embedding_chain", "moco_key")
+
+
+def build_ssl_trunk(case):
+    """(module, clip) of a self-supervised trunk as the models lower it: "embedding_chain" is the video SimCLR case's
+    Slow-R50 trunk and its 2048-2048-128 BatchNorm1d projector as one EmbeddingChain (one plan with fused rows);
+    "moco_key" is the chain MoCo v2's slow_r50 case compiles for its momentum (key) encoder."""
+    import types
+    from .layers import make_multilayer_perceptron
+    from .models import moco_v2
+    from .models.embedding import EmbeddingChain
+    from .models.resnet import create_resnet
+    from .models.simclr import SimCLR
+    if case == "embedding_chain":
+        ns = types.SimpleNamespace(SimCLR=SimCLR, create_resnet=create_resnet,
+                                   make_multilayer_perceptron=make_multilayer_perceptron)
+        m, (x1, _) = build_ssl_case("simclr_video", ns)
+        return EmbeddingChain(m.backbone, m.mlp).eval(), x1[:1].contiguous()
+    ns = types.SimpleNamespace(MOCO=moco_v2.MOCO, create_moco_resnet_50=moco_v2.create_moco_resnet_50,
+                               create_mlp_util=moco_v2.create_mlp_util, create_resnet=create_resnet)
+    m, views, _, _ = build_moco_case("moco_slow_r50", ns)
+    return m._state()["mmt"].eval(), views[0][:1].contiguous()
+
+
+def _roll_clip(t, k):
+    """Clip k of a pool made from the clips of ``t``: clip k % B0 itself for k < B0, else that clip rolled along its
+    last axis by k // B0 places (the same values, on the same grid, at other positions)."""
+    c = t[k % t.shape[0]]
+    return c if k < t.shape[0] else c.roll(k // t.shape[0], -1)
+
+
+def _pool_boxes(H, W, pool):
+    """[K, 5] boxes over ``pool`` clips, grouped by clip in clip order: clip 0 takes the three boundary boxes of
+    synthetic_boxes (outside the frame, smaller than a feature cell, the whole frame), clip 1 none, every further clip
+    two of the case's random boxes."""
+    rows = [torch.cat([torch.zeros(1), b[1:]]) for b in synthetic_boxes(3, 1, H, W)]
+    rnd = synthetic_boxes(max(5, 2 * pool), 1, H, W, seed=19)[3:]
+    for c in range(2, pool):
+        for b in rnd[2 * (c - 2):2 * (c - 1)]:
+            rows.append(torch.cat([torch.tensor([float(c)]), b[1:]]))
+    return torch.stack(rows).contiguous()
+
+
+class BatchCase:
+    """A catalogue case at any batch B <= pool: its model, and inputs whose clip j is the same tensor at every B (a
+    pool of ``pool`` clips is drawn once; a batch is its first B clips).  Per-clip side inputs follow their clip:
+    masks are rows of the pool, detection boxes carry their clip's batch index (clip 1 has none)."""
+
+    def __init__(self, family, case, pool):
+        self.family, self.case, self.pool = family, case, pool
+        self.model, x, self.extra, fixed = build_audit_case(family, case)
+        self.multi = isinstance(x, (list, tuple))
+        xs = list(x) if self.multi else [x]
+        self.box_slot = len(xs) - 1 if family == "detection" else None
+        self.inputs = []
+        for i, t in enumerate(xs):
+            if i == self.box_slot:
+                H, W = xs[0].shape[-2:]
+                self.inputs.append(_pool_boxes(H, W, pool))
+            else:
+                self.inputs.append(torch.stack([_roll_clip(t, k) for k in range(pool)]))
+
+    def boxes_of(self, B):
+        """Per clip of a batch of B: the rows of its boxes (None without boxes)."""
+        if self.box_slot is None:
+            return None
+        idx = self.inputs[self.box_slot][:, 0].long()
+        keep = [int(i) for i in torch.nonzero(idx < B).flatten()]
+        return [[r for r, i in enumerate(keep) if int(idx[i]) == c] for c in range(B)]
+
+    def batch(self, B, rotate=False):
+        """The engine inputs of the first B clips; rotate: clip c at position (c + 1) % B, boxes re-indexed."""
+        out = []
+        for i, t in enumerate(self.inputs):
+            if i == self.box_slot:
+                t = t[t[:, 0] < B].clone()
+                if rotate:
+                    t[:, 0] = (t[:, 0] + 1) % B
+            else:
+                t = t[:B].roll(1, 0) if rotate else t[:B]
+            out.append(t.contiguous())
+        return out
+
+    def single(self, c):
+        """The engine inputs of clip c alone (a clip without boxes gets two whole-frame boxes, whose rows nothing
+        compares, so that its plan has the same ops)."""
+        out = []
+        for i, t in enumerate(self.inputs):
+            if i == self.box_slot:
+                t = t[t[:, 0] == c].clone()
+                t[:, 0] = 0
+                if not len(t):
+                    H, W = self.inputs[0].shape[-2:]
+                    t = torch.tensor([[0.0, 0.0, 0.0, float(W), float(H)]] * 2)
+            else:
+                t = t[c:c + 1]
+            out.append(t.contiguous())
+        return out
+
+    def example(self, ins):
+        return ins if self.multi else ins[0]
+
+
+def clip_rows_fn(B, boxes=None, perm=None, n_rois=None):
+    """clip_rows for clip_digests: a per-clip operand (B rows) holds clip c in row perm[c] (default c); a per-RoI one
+    (n_rois rows, default all of boxes) holds clip c in the rows boxes[c]."""
+    perm = list(range(B)) if perm is None else perm
+    n_rois = sum(len(b) for b in boxes) if n_rois is None and boxes is not None else n_rois
+
+    def rows(n, per_roi):
+        if per_roi:
+            assert boxes is not None and n == n_rois, (n, n_rois)
+            return boxes
+        assert n == B, (n, B)
+        return [[perm[c]] for c in range(B)]
+    return rows
+
+
+def clip_operands(spec):
+    """(operands a record reads, operands it writes) with the staged inputs that are not plan buffers (the source
+    clip, a staged mask, the RoIs of a RoIAlign), each to be sliced by record_rows."""
+    from .engine.plan import MaskRef
+    ins, outs = record_io(spec)
+    ins = list(ins)
+    k = spec["kind"]
+    if k in ("to_ndhwc", "tokens_in"):
+        ins.append(spec["src"])
+    m = spec.get("mask")
+    if isinstance(m, MaskRef) and m.tensor is not None:
+        ins.append(m)
+    if k == "roi_align":
+        ins.append(spec["rois"])
+    return ins, list(outs)
+
+
+def _buf_id(t):
+    from .engine.plan import Buf
+    if isinstance(t, Buf):
+        return id(t)
+    b = getattr(t, "buf", None)
+    return id(b) if b is not None and not torch.is_tensor(t) else None
+
+
+_DIGEST_W = {}
+
+
+def _digest_weights(n, device):
+    """Odd 64-bit weights w_i, a fixed function of the index i (a multiplicative hash)."""
+    w = _DIGEST_W.get(device)
+    if w is None or w.numel() < n:
+        i = torch.arange(max(n, 1 << 20), dtype=torch.int64, device=device)
+        w = i * -7046029254386353131
+        w = w ^ (w >> 31)
+        w = (w * -4658895280553007687) | 1
+        _DIGEST_W[device] = w
+    return w[:n]
+
+
+def row_digests(v):
+    """One 64-bit digest per row of v [N, ...]: sum_i bits_i * w_i mod 2^64 over the bit patterns of the row, with odd
+    weights w_i, so a change of any one element always changes the digest (a change of several cancels with
+    probability ~2^-64).  Computed on the tensor's device; the digest includes the row's shape."""
+    n = v.shape[0]
+    if n == 0:
+        return []
+    v = v.contiguous().reshape(n, -1)
+    if v.dtype == torch.bool:
+        v = v.to(torch.uint8)
+    v = v.view({torch.float16: torch.int16, torch.float32: torch.int32, torch.float64: torch.int64}.get(v.dtype, v.dtype))
+    w = _digest_weights(v.shape[1], v.device)
+    d = torch.stack([(r.long() * w).sum() for r in v])
+    return [(v.shape[1], h) for h in d.tolist()]
+
+
+def _clip_digests_of(spec, items, role, clip_rows, per_roi):
+    per_clip = None
+    for t in items:
+        rows = record_rows(spec, t, role)
+        dig = row_digests(rows)
+        sel = clip_rows(rows.shape[0], per_roi(t))
+        if per_clip is None:
+            per_clip = [[] for _ in sel]
+        for c, r in enumerate(sel):
+            per_clip[c].append(tuple(dig[j] for j in r))
+    return [tuple(d) for d in per_clip] if per_clip is not None else None
+
+
+def clip_digests(plan, clip_rows, corrupt=None):
+    """Run the plan op by op on one stream and digest, for every op with a record and every clip, the rows of each
+    operand it reads (just before it runs) and of each it writes (just after), the rows the op reads / writes
+    (record_rows with a role).  clip_rows(n, per_roi): for an operand with n rows, the rows of each clip.  An operand
+    is per RoI when it is a RoIAlign's RoIs or a buffer an op wrote from a per-RoI operand (the plan's data flow, not
+    its row count).  corrupt(i, spec): called after op i ran, before its digests.
+    Returns {(op name, occurrence): (launched instances, [input digests per clip], [output digests per clip], ids of
+    the buffers the op reads, ids of those it writes)}."""
+    sp = torch.cuda.current_stream().cuda_stream
+    out, seen, roi_bufs = {}, {}, set()
+    for i, ((name, fn), spec) in enumerate(zip(plan.ops, plan.op_spec)):
+        key = (name, seen.get(name, 0))
+        seen[name] = key[1] + 1
+        if spec is None:
+            fn(sp)
+            continue
+        ins, outs = clip_operands(spec)
+
+        def per_roi(t):
+            return t is spec.get("rois") or _buf_id(t) in roi_bufs
+        d_in = _clip_digests_of(spec, ins, "read", clip_rows, per_roi)
+        roi_op = any(per_roi(t) for t in ins)
+        reads = frozenset(b for b in map(_buf_id, ins) if b is not None)
+        writes = frozenset(b for b in map(_buf_id, outs) if b is not None)
+        roi_bufs = (roi_bufs | writes) if roi_op else (roi_bufs - writes)
+        c0 = kernel_counts()
+        fn(sp)
+        torch.cuda.synchronize()
+        launched = frozenset(kernel_count_diff(c0, kernel_counts()))
+        if corrupt is not None:
+            corrupt(i, spec)
+        out[key] = (launched, d_in, _clip_digests_of(spec, outs, "write", clip_rows, per_roi), reads, writes)
+    return out
+
+
+def invariance_failures(want, got, exempt_prefixes=()):
+    """Bitwise invariance between two runs' clip_digests, clip by clip (the lists are matched by position): where an
+    op launched the same instances in both runs and read bit-equal rows for a clip, it must write bit-equal rows for
+    that clip.  An op that launched other instances, or an instance named by exempt_prefixes (kernels whose bits
+    depend on the batch by design), makes no claim (exempt).  Returns (failures [(op key, clips)],
+    held [op keys whose claim was checked on every clip], exempt [(op key, instances in want, instances in got)],
+    unexplained [op keys neither held, exempt nor failed that read no buffer written downstream of an exempt op in
+    want's plan]).  With no failure and no exemption every op must be held: any other op read a row the two runs
+    wrote differently without an op that wrote it being named."""
+    assert list(want) == list(got), sorted(set(want) ^ set(got))[:10]
+    failures, held, exempt, unexplained = [], [], [], []
+    tainted = set()
+    for key, w in want.items():
+        inst_w, in_w, out_w, reads, writes = w
+        inst_g, in_g, out_g = got[key][:3]
+        if inst_w != inst_g or (exempt_prefixes and any(n.startswith(tuple(exempt_prefixes)) for n in inst_w)):
+            exempt.append((key, sorted(inst_w), sorted(inst_g)))
+            tainted |= writes
+            continue
+        n = len(out_w)
+        same_in = [in_w is None or in_w[c] == in_g[c] for c in range(n)]
+        bad = [c for c in range(n) if same_in[c] and out_w[c] != out_g[c]]
+        if bad:
+            failures.append((key, bad))
+        elif all(same_in):
+            held.append(key)
+        elif reads & tainted:
+            tainted |= writes
+        else:
+            unexplained.append(key)
+    return failures, held, exempt, unexplained
+
+
+def merge_single(digests):
+    """The clip_digests of the batch-1 runs of clips 0..B-1 as one run of B clips (for invariance_failures), with the
+    instances all the runs launched (they differ only where the clips' plans do: the RoI count of a detection head)."""
+    out = {}
+    for k in digests[0]:
+        inst = frozenset().union(*(d[k][0] for d in digests))
+        ins = None if digests[0][k][1] is None else [d[k][1][0] for d in digests]
+        out[k] = (inst, ins, [d[k][2][0] for d in digests])
+    return out
+
+
+# ---- the batch audit's runs (tests/test_gpu_batch_audit*.py): one (precision, case, batch) row -----------------------
+BATCH_AUDIT_PARTS = ("workloads", "models", "families", "layers", "ssl")
+
+
+def batch_sweep_part(row, workloads):
+    """The file of the batch audit a sweep row runs in, each about ten minutes on an H100: "workloads" the bench
+    architectures but csn_r101, "models" csn_r101 and the other f16 MODEL_CASES, "families" the grouped, hub-tail,
+    detection and Non-local cases in f16, "ssl" the SSL trunks, "layers" the rest (audio, efficient, MViT variants,
+    masked in f16; every f32 row but the trunks)."""
+    p, f, c = row[:3]
+    if f == "ssl":
+        return "ssl"
+    if p == "f16" and f == "model":
+        return "workloads" if c in workloads and c != "csn_r101" else "models"
+    if p == "f16" and f in ("grouped", "hub_tail", "detection", "nonlocal"):
+        return "families"
+    return "layers"
+
+
+def batch_pools(sweep):
+    """(family, case) -> the largest batch the sweep runs it at (the size of its clip pool)."""
+    pools = {}
+    for r in sweep:
+        pools[r[1:3]] = max(pools.get(r[1:3], 1), r[3])
+    return pools
+
+
+_BATCH_CASE = {}
+_BATCH_SINGLE = {}           # (precision, family, case, clip) -> clip_digests of the clip's batch-1 plan
+
+
+def batch_case(family, case, pool):
+    """The BatchCase of a case (one kept at a time)."""
+    key = (family, case, pool)
+    if key not in _BATCH_CASE:
+        _BATCH_CASE.clear()
+        _BATCH_CASE[key] = BatchCase(family, case, pool)
+    return _BATCH_CASE[key]
+
+
+def batch_compile(bc, ins, prec):
+    from .engine import compile_model
+    return compile_model(bc.model, bc.example([t.cuda() for t in ins]), dtype=prec, use_graph=False, extra=bc.extra)
+
+
+def batch_digests(cm, ins, rows, corrupt=None):
+    for s, t in zip(cm.static_in, ins):
+        s.copy_(t)
+    torch.cuda.synchronize()
+    with torch.no_grad():
+        return clip_digests(cm.plan, rows, corrupt)
+
+
+def batch_single_digests(prec, bc, B):
+    """clip_digests of the batch-1 plan of clips 0..B-1 (compiled once per case; per clip with boxes, whose RoI count
+    is the plan's)."""
+    cm = None
+    for c in range(B):
+        key = (prec, bc.family, bc.case, c)
+        if key in _BATCH_SINGLE:
+            continue
+        ins = bc.single(c)
+        if cm is None or bc.box_slot is not None:
+            cm = batch_compile(bc, ins, prec)
+        boxes = None
+        if bc.box_slot is not None:
+            boxes = [list(range(len(bc.boxes_of(c + 1)[c])))]
+        _BATCH_SINGLE[key] = batch_digests(cm, ins, clip_rows_fn(1, boxes, n_rois=None if boxes is None else
+                                                                 len(ins[bc.box_slot])))
+    del cm
+    torch.cuda.empty_cache()
+    return [_BATCH_SINGLE[(prec, bc.family, bc.case, c)] for c in range(B)]
+
+
+def _fmt_keys(items):
+    return "; ".join("%s#%d%s" % (k[0], k[1], "" if c is None else " on clips %s" % c) for k, c in items[:20])
+
+
+def run_batch_audit(prec, family, case, B, checks, pool, batch_dependent=()):
+    """One row of the batch audit: (a) audit_plan on every clip (when "a" in checks), (b) position invariance under a
+    rotation of the clips, in which every op must be held, (c) batch-size invariance against each clip's batch-1 plan,
+    in which every op is held, exempt (other instances, or one of ``batch_dependent``'s instance prefixes) or reads
+    what an exempt op's data flow wrote.  Returns the report lines (RESULT, EXEMPT, INSTANCES)."""
+    import time
+    t0 = time.time()
+    bc = batch_case(family, case, pool)
+    ins = bc.batch(B)
+    cm = batch_compile(bc, ins, prec)
+    plan = cm.plan
+    boxes = bc.boxes_of(B)
+    line = "RESULT %s %s b%d:" % (prec, case, B)
+    if "a" in checks:
+        for s, t in zip(cm.static_in, ins):
+            s.copy_(t)
+        torch.cuda.synchronize()
+        with torch.no_grad():
+            failures, stats = audit_plan(plan, list(range(B)))
+        assert not failures, "\n".join("op %d %s: %s" % f for f in failures[:20])
+        n_checked = sum(v[0] for v in stats.values())
+        assert n_checked + sum(1 for s in plan.op_spec if s is None) == len(plan.ops)
+        line += " (a) %d launches on %d clips, largest err/tol %s;" % (
+            n_checked, B, ", ".join("%s %.3f" % (k, v[1]) for k, v in sorted(stats.items())))
+    want = batch_digests(cm, ins, clip_rows_fn(B, boxes))
+    rot = batch_digests(cm, bc.batch(B, rotate=True), clip_rows_fn(B, boxes, perm=[(c + 1) % B for c in range(B)]))
+    del cm, plan
+    torch.cuda.empty_cache()
+    fb, held_b, ex_b, un_b = invariance_failures(want, rot)
+    assert not fb, "position invariance: " + _fmt_keys(fb)
+    not_held = [(k, None) for k in want if k not in set(held_b)]
+    assert not ex_b and not not_held, "position invariance: not held: " + _fmt_keys(not_held)
+    fc, held_c, exempt, un_c = invariance_failures(want, merge_single(batch_single_digests(prec, bc, B)),
+                                                   exempt_prefixes=batch_dependent)
+    assert not fc, "batch-size invariance against batch 1: " + _fmt_keys(fc)
+    assert not un_c, "batch-size invariance: read differing rows downstream of no exempt op: " + _fmt_keys(
+        [(k, None) for k in un_c])
+    line += " (b) %d of %d ops held; (c) %d held, %d exempt, %d downstream of an exempt op; %.1f s" % (
+        len(held_b), len(want), len(held_c), len(exempt), len(want) - len(held_c) - len(exempt), time.time() - t0)
+    return [line,
+            "EXEMPT %s %s b%d: %s" % (prec, case, B, "; ".join("%s: %s -> %s" % (k[0], ",".join(w), ",".join(g))
+                                                              for k, w, g in exempt)),
+            "INSTANCES %s %s b%d: %s" % (prec, case, B, "; ".join("%s=%s" % (k[0], ",".join(sorted(v[0])))
+                                                                 for k, v in want.items()))]
 
 # ---- Non-local block cases (tests/golden/nonlocal.pt): name -> (create_nonlocal kwargs, input shape) ---------------
 NONLOCAL_CASES = {

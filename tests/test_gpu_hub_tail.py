@@ -139,6 +139,7 @@ PLANE_CASES = [
     (56, 1, 96, 96, 0, 1),         # 56x56 out                              <1,4,4>
     (14, 1, 768, 1152, 384, 5),    # blocks 3-13 K|V                        <1,2,7>
     (7, 1, 1536, 2304, 768, 3),    # blocks 14-15 K|V                       <1,2,7>
+    (56, 4, 192, 288, 96, 3),      # block 0 K|V at batch 3 (the unused stride-4 tensor map was rejected)  <4,1,2>
 ]
 
 
@@ -179,7 +180,15 @@ def _run_plane(H, s, C, rs, off, N, seed):
     return got, ref, absref, y, ran
 
 
-@pytest.mark.parametrize("case", PLANE_CASES, ids=["h%d_s%d_c%d" % c[:3] for c in PLANE_CASES])
+def _plane_ids():
+    ids = []
+    for c in PLANE_CASES:
+        i = "h%d_s%d_c%d" % c[:3]
+        ids.append(i if i not in ids else i + "_n%d" % c[5])      # a repeated shape at another batch
+    return ids
+
+
+@pytest.mark.parametrize("case", PLANE_CASES, ids=_plane_ids())
 def test_plane_kernel_against_float64(case):
     H, s, C, rs, off, N = case
     got, ref, absref, y, ran = _run_plane(H, s, C, rs, off, N, seed=H * 31 + s * 7 + C)

@@ -46,10 +46,12 @@ each now charged beside its reference in testing.py:
   - x3d_m / x3d_l (f32): pv_channel_sum adds up to a few hundred stored outputs per thread in fp32 before its
     fixed-point atomic (channel_sum_adds); in f16 the storage rounding term had covered it.
 
-Not verified: batch sizes other than each case's own; clips other than the audited ones (eval forward couples no
-clips, but a tile-walk fault confined to another clip would pass); the SSL / MoCo trunks and the transform, bank,
-contrastive and JPEG kernels (not plan ops); instances no catalogue case reaches (the kernel matrices cover those per
-instance); the run time in a single pytest process.
+test_gpu_batch_audit.py runs the same audit at other batch sizes on every clip, with the SSL / MoCo trunks, and checks
+each clip's bits under reordering the batch and against the batch-1 plan.
+
+Not verified: batch sizes other than each case's own and the batch audit's sweep; SM counts other than the test
+machine's (the routes read the device's); the transform, bank, contrastive and JPEG kernels (not plan ops); instances
+no catalogue case reaches (the kernel matrices cover those per instance); the run time in a single pytest process.
 """
 import math
 import os
@@ -69,75 +71,10 @@ from pytorchvideo_b200 import _lib as L  # noqa: E402
 from pytorchvideo_b200 import testing as TS  # noqa: E402
 from pytorchvideo_b200.engine.plan import Buf, TRef  # noqa: E402
 
-# architecture / shape pairs the workload audit already runs in f16 (at bench.py's batch)
-_WORKLOAD_SHAPES = {(v[0], v[2], v[3], v[4]) for v in bench.WORKLOADS.values()}
-
-
-def _model_cases():
-    out = []
-    for name, (hub, kw, B, T, H, W, _) in sorted(TS.MODEL_CASES.items()):
-        if name[:3] in ("c1_", "c2_", "c3_", "c4_") or name.endswith("_f16w"):
-            continue
-        out.append(("model", name, not kw and (hub, T, H, W) in _WORKLOAD_SHAPES))
-    return out
-
-
-def _catalogue():
-    """[(family, case, is a workload shape)] in a fixed order."""
-    cases = _model_cases()
-    cases += [("hub_tail", c, False) for c in sorted(TS.HUB_TAIL_CASES)]
-    cases += [("grouped", c, False) for c in sorted(TS.GROUPED_MODEL_CASES) if not c.endswith("_f16w")]
-    cases += [("detection", c, False) for c in sorted(TS.DETECTION_CASES)]
-    cases += [("audio", c, False) for c in sorted(TS.AUDIO_CASES)]
-    cases += [("efficient", c, False) for c in sorted(TS.EFFICIENT_CASES)]
-    cases += [("mvit_variant", c, False) for c in sorted(TS.MVIT_VARIANT_CASES)]
-    cases += [("nonlocal", c, False) for c in sorted(TS.NONLOCAL_CASES)]
-    cases += [("nonlocal", "i3d_nln", False)]
-    cases += [("masked", c, False) for c in TS.MASKED_CASES]
-    return cases
-
-
-CATALOGUE = _catalogue()
-CASES = [("f16", f, c) for f, c, w in CATALOGUE if not w] + [("f32", f, c) for f, c, _ in CATALOGUE]
+CATALOGUE = TS.audit_catalogue(bench.WORKLOADS)
+CASES = TS.audit_cases(bench.WORKLOADS)
 IDS = ["%s-%s-%s" % c for c in CASES]
-
-
-def build(family, case):
-    """(model, engine inputs (a tensor or a list), extra, indices of inputs that stay fixed on the replay)."""
-    import pytorchvideo_b200.models as M
-    import pytorchvideo_b200.models.hub as PH
-    extra, fixed = (), set()
-    if family == "model":
-        m, x, _ = TS.build_case(case, PH)
-    elif family == "hub_tail":
-        m, x = TS.build_hub_tail_case(case, PH)
-    elif family == "grouped":
-        m, x, _ = TS.build_grouped_case(case, PH)
-    elif family == "detection":
-        m, x, boxes, _ = TS.build_detection_case(case, PH)
-        x = (x if isinstance(x, list) else [x]) + [boxes]
-        fixed = {len(x) - 1}
-    elif family == "audio":
-        m, x = TS.build_audio_case(case, M)
-    elif family == "efficient":
-        m, x = TS.build_efficient_case(case, TS.efficient_namespace())
-    elif family == "mvit_variant":
-        from pytorchvideo_b200.layers.attention import MultiScaleBlock
-        from pytorchvideo_b200.models.vision_transformers import create_multiscale_vision_transformers
-        m, x, ex = TS.build_mvit_variant_case(case, create_multiscale_vision_transformers, MultiScaleBlock)
-        extra = tuple(tuple(e) for e in ex)
-    elif family == "nonlocal":
-        from pytorchvideo_b200.layers.nonlocal_net import create_nonlocal
-        if case == "i3d_nln":
-            m, x = TS.build_i3d_nln(PH, create_nonlocal)
-        else:
-            m, x = TS.build_nonlocal_case(case, create_nonlocal)
-    else:
-        m = TS.build_masked_case(case, TS.masked_namespace())
-        x, mask = TS.masked_case_inputs(case)
-        x, extra = TS.masked_engine_args(case, x, mask)
-        fixed = {i for i, t in enumerate(x if isinstance(x, list) else [x]) if t.dtype == torch.bool}
-    return m, x, extra, fixed
+build = TS.build_audit_case
 
 
 def _flat(x):
@@ -213,10 +150,19 @@ def test_f32_audit_names_a_tile_the_parity_tolerance_misses():
 # =====================================================================================================================
 # CPU: records and declared I/O over the whole catalogue
 # =====================================================================================================================
-@pytest.mark.parametrize("prec,family,case", CASES, ids=IDS)
-def test_every_launch_has_a_checked_record(prec, family, case):
+# every case at its own batch, and every (case, batch) of test_gpu_batch_audit.py's sweep
+_RECORD_CASES = [c + (None,) for c in CASES] + [r[:4] for r in TS.batch_sweep(bench.WORKLOADS)]
+_RECORD_IDS = IDS + ["%s-%s-%s-b%d" % r[:4] for r in TS.batch_sweep(bench.WORKLOADS)]
+
+
+@pytest.mark.parametrize("prec,family,case,batch", _RECORD_CASES, ids=_RECORD_IDS)
+def test_every_launch_has_a_checked_record(prec, family, case, batch):
     from pytorchvideo_b200.engine.lower import lower_only
-    m, x, extra, _ = build(family, case)
+    if batch is None:
+        m, x, extra, _ = build(family, case)
+    else:
+        bc = TS.BatchCase(family, case, batch)
+        m, x, extra = bc.model, bc.example(bc.batch(batch)), bc.extra
     plan, _ = lower_only(m, x, dtype=prec, extra=extra)
     assert len(plan.op_spec) == len(plan.ops)
     missing = [n for (n, _), s in zip(plan.ops, plan.op_spec)
