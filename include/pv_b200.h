@@ -192,6 +192,22 @@ typedef struct pv_boxes_desc {
 int pv_clip_boxes_transform(const pv_boxes_desc* d, const void* boxes_in, const int32_t* box_start,
                             const int32_t* geom, void* boxes_out, float* rois_out, void* stream);
 
+/* Ragged mode of the box transform: the boxes of a batch whose clips come from frames of their own sizes (the
+ * companion of pv_clip_transform_ragged).  geom is the DEVICE int32 table pv_clip_transform_ragged reads, one row
+ * {in_h, in_w, new_h, new_w, top, left, hflip} per clip, and geom_host the same table in host memory, which the call
+ * validates (every size >= 1, the out_h x out_w window at (top, left) inside new_h x new_w).  Each clip takes its own
+ * in_h / in_w for PV_BOX_CLIP_SRC and PV_BOX_SCALE (the scale's in_w < in_h test is made per clip); the descriptor's
+ * in_*, new_*, top, left and hflip are ignored, and out_h / out_w (both >= 1) are read from it.  One more step bit,
+ * accepted only here, runs before all the others:
+ *   PV_BOX_DENORM     x = x * T(in_w), y = y * T(in_h), one rounding each   ([0, 1] coordinates to source pixels)
+ * box_start, boxes_out == boxes_in, rois_out and the rounding are as in pv_clip_boxes_transform.  One launch;
+ * n_boxes == 0 launches nothing.                                                                                */
+#define PV_BOX_DENORM 64
+
+int pv_clip_boxes_transform_ragged(const pv_boxes_desc* d, const void* boxes_in, const int32_t* box_start,
+                                   const int32_t* geom, const int32_t* geom_host,
+                                   void* boxes_out, float* rois_out, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Video augmentation (transforms/augmentations.py, rand_augment.py, augmix.py): a batch of clips of (T, 3, H, W)
  * frames, each clip with its own op per layer step.

@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_DIR = os.path.join(_HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libpvb200.so")
-SOURCES = ["pv_api.cu", "pv_transform.cu", "pv_augment.cu", "pv_roi.cu", "pv_simt.cu", "pv_igemm.cu", "pv_igemm_gather.cu", "pv_dwconv.cu", "pv_dwlane.cu", "pv_dwplane.cu","pv_fastblock.cu", "pv_stem.cu", "pv_stem_stream.cu", "pv_attention.cu", "pv_attention_mma.cu", "pv_attention_wgmma.cu", "pv_attention_wide.cu", "pv_mix.cu", "pv_masked.cu", "pv_lstm.cu", "pv_boxes.cu", "pv_contrastive.cu", "pv_colorjitter.cu", "pv_bank.cu", "pv_jpeg.cu"]
+SOURCES = ["pv_api.cu", "pv_transform.cu", "pv_augment.cu", "pv_roi.cu", "pv_simt.cu", "pv_igemm.cu", "pv_igemm_gather.cu", "pv_dwconv.cu", "pv_dwlane.cu", "pv_dwplane.cu","pv_fastblock.cu", "pv_stem.cu", "pv_stem_stream.cu", "pv_attention.cu", "pv_attention_mma.cu", "pv_attention_wgmma.cu", "pv_attention_wide.cu", "pv_mix.cu", "pv_masked.cu", "pv_lstm.cu", "pv_boxes.cu", "pv_boxes_ragged.cu", "pv_contrastive.cu", "pv_colorjitter.cu", "pv_bank.cu", "pv_jpeg.cu"]
 ARCH = "arch=compute_90a,code=sm_90a"
 NVCC_FLAGS = [
     "-gencode", ARCH, "-O3", "-lineinfo", "-std=c++17",

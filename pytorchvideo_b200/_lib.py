@@ -40,6 +40,7 @@ class ClipBatchDesc(C.Structure):
 
 BOX_F32, BOX_F64 = 1, 3                             # pv_boxes_desc.dtype
 BOX_CLIP_SRC, BOX_SCALE, BOX_CROP, BOX_CLIP_CROP, BOX_FLIP, BOX_CLIP_OUT = 1, 2, 4, 8, 16, 32   # pv_boxes_desc.steps
+BOX_DENORM = 64                                     # pv_clip_boxes_transform_ragged only
 
 
 class BoxesDesc(C.Structure):
@@ -170,6 +171,7 @@ SIGNATURES = {
     "pv_clip_transform_rrc": (C.c_int, [C.POINTER(ClipBatchDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_clip_transform_ragged": (C.c_int, [C.POINTER(ClipBatchDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_clip_boxes_transform": (C.c_int, [C.POINTER(BoxesDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "pv_clip_boxes_transform_ragged": (C.c_int, [C.POINTER(BoxesDesc), c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_augment_stats": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, c_vp]),
     "pv_augment_apply": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, c_vp, c_vp, c_vp]),
     "pv_augment_mix": (C.c_int, [C.POINTER(AugmentDesc), c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp]),

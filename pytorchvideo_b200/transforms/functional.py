@@ -345,12 +345,26 @@ def clip_transform_ragged(src, frame_off, geom, out_hw, mean=None, std=None, div
     if out_dtype not in (torch.float16, torch.float32):
         raise RuntimeError("the ragged mode writes float16 or float32")
     offs, rows = ragged_tables(frame_off, geom, out_hw)
-    B, n_t = len(geom), offs.numel() // len(geom)
+    check_ragged_offsets(src, offs, geom)
+    return launch_clip_ragged(src, offs.to(src.device), rows.to(src.device), rows, len(geom), out_hw, mean, std,
+                              div255, out_dtype, slow_alpha)
+
+
+def check_ragged_offsets(src, offs, geom):
+    """Raise unless every frame of the flat offset table ``offs`` lies inside ``src``."""
+    n_t = offs.numel() // len(geom)
     sizes = torch.tensor([g[0][0] * g[0][1] * 3 for g in geom], dtype=torch.int64).repeat_interleave(n_t)
     if int(offs.min()) < 0 or int((offs + sizes).max()) > src.numel():
         raise RuntimeError("a frame offset lies outside the source buffer")
+
+
+def launch_clip_ragged(src, offs_d, rows_d, rows, B, out_hw, mean=None, std=None, div255=False,
+                       out_dtype=torch.float16, slow_alpha=None):
+    """The pv_clip_transform_ragged launch of ``clip_transform_ragged`` on tables already on the device and checked:
+    ``offs_d`` / ``rows_d`` the device copies of ``ragged_tables``' offsets and rows, ``rows`` the host rows."""
     lib = L.load()
     dev = src.device
+    n_t = offs_d.numel() // B
     oh, ow = (int(v) for v in out_hw)
     d = L.ClipBatchDesc()
     d.C, d.n_clips, d.n_t, d.out_h, d.out_w = 3, B, n_t, oh, ow
@@ -363,8 +377,6 @@ def clip_transform_ragged(src, frame_off, geom, out_hw, mean=None, std=None, div
         slow_d, d.n_slow = _slow_table(n_t, slow_alpha, dev)
         out_slow = torch.empty((B, 3, d.n_slow, oh, ow), dtype=out_dtype, device=dev)
         d.d_slow_clip = out_slow.stride(0)
-    offs_d = offs.to(dev)
-    rows_d = rows.to(dev)
     L.check(lib.pv_clip_transform_ragged(C.byref(d), src.data_ptr(), offs_d.data_ptr(), rows_d.data_ptr(),
                                          rows.data_ptr(), slow_d.data_ptr() if slow_d is not None else None,
                                          out.data_ptr(), out_slow.data_ptr() if out_slow is not None else None,
@@ -625,6 +637,37 @@ def clip_boxes_transform(boxes, steps, in_hw=(0, 0), new_hw=(0, 0), offset=(0, 0
                                              geom.data_ptr() if geom is not None else None, out.data_ptr(),
                                              r.data_ptr() if r is not None else None,
                                              torch.cuda.current_stream(dev).cuda_stream), "pv_clip_boxes_transform")
+    out._pv_keepalive = (boxes, box_start, geom)     # inputs must outlive the asynchronous launch
+    return out, r
+
+
+def clip_boxes_transform_ragged(boxes, steps, box_start, geom, geom_host, out_hw, out=None, rois=False):
+    """Run pv_clip_boxes_transform_ragged: the boxes of clips with frames of their own sizes, in one launch.
+
+    boxes    : contiguous (K, 4) float32 / float64 CUDA tensor
+    steps    : mask of _lib.BOX_* steps; BOX_DENORM (x * in_w, y * in_h) runs first, then the others in their order
+    box_start: device int32 [n_clips + 1] offsets of each clip's boxes
+    geom     : device int32 [n_clips][7] {in_h, in_w, new_h, new_w, top, left, hflip}, the table
+               ``clip_transform_ragged`` reads (``ragged_tables``' rows); ``geom_host`` the same table on the host
+    out_hw   : crop / output frame of every clip
+    Returns (out, rois) as ``clip_boxes_transform`` does."""
+    dev = boxes.device
+    K = int(boxes.shape[0])
+    geom_host = geom_host.to(torch.int32).contiguous()
+    n_clips = geom_host.numel() // 7
+    if geom_host.device.type != "cpu" or geom_host.numel() != 7 * n_clips or n_clips < 1:
+        raise RuntimeError("geom_host must be a host table of 7 ints per clip")
+    if out is None:
+        out = torch.empty_like(boxes)
+    r = torch.empty((K, 5), dtype=torch.float32, device=dev) if rois else None
+    d = L.BoxesDesc()
+    d.n_clips, d.n_boxes, d.steps, d.dtype = n_clips, K, int(steps), _BOX_DT[boxes.dtype]
+    d.out_h, d.out_w = int(out_hw[0]), int(out_hw[1])
+    L.check(L.load().pv_clip_boxes_transform_ragged(C.byref(d), boxes.data_ptr(), box_start.data_ptr(),
+                                                    geom.data_ptr(), geom_host.data_ptr(), out.data_ptr(),
+                                                    r.data_ptr() if r is not None else None,
+                                                    torch.cuda.current_stream(dev).cuda_stream),
+            "pv_clip_boxes_transform_ragged")
     out._pv_keepalive = (boxes, box_start, geom)     # inputs must outlive the asynchronous launch
     return out, r
 

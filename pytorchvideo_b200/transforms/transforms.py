@@ -292,6 +292,17 @@ class FusedDetectionTransform(nn.Module):
         flip = bool(np.random.uniform() < self.hflip_prob) if self.hflip_prob > 0.0 else False
         return (nh, nw), (top, left, oh, ow), flip
 
+    def box_steps(self):
+        """The mask of _lib.BOX_* steps this chain runs on the boxes."""
+        steps = L.BOX_CLIP_SRC | L.BOX_CLIP_OUT
+        if self.short_side is not None or self.random_short_side is not None:
+            steps |= L.BOX_SCALE
+        if self.crop is not None:
+            steps |= L.BOX_CROP | L.BOX_CLIP_CROP
+        if self.hflip_prob > 0.0:
+            steps |= L.BOX_FLIP
+        return steps
+
     def _boxes(self, boxes, B, dev):
         """The box lists as one contiguous (K, 4) device tensor and the host offsets of each clip's rows."""
         if torch.is_tensor(boxes) or isinstance(boxes, np.ndarray):
@@ -341,13 +352,7 @@ class FusedDetectionTransform(nn.Module):
                                          slow_alpha=self.slowfast_alpha)
         if clips.dim() == 4:
             inputs = [t[0] for t in inputs] if self.slowfast_alpha is not None else inputs[0]
-        steps = L.BOX_CLIP_SRC | L.BOX_CLIP_OUT
-        if self.short_side is not None or self.random_short_side is not None:
-            steps |= L.BOX_SCALE
-        if self.crop is not None:
-            steps |= L.BOX_CROP | L.BOX_CLIP_CROP
-        if self.hflip_prob > 0.0:
-            steps |= L.BOX_FLIP
+        steps = self.box_steps()
         if start[-1] == 0:
             return inputs, torch.empty((0, 5), dtype=torch.float32, device=dev)
         table = []
