@@ -82,6 +82,16 @@ class TRef:
             self.N, self.C, self.Cp, self.T, self.H, self.W, self.ch_off, self.row_stride)
 
 
+def _may_overlap(a, b):
+    """False only when two plan items of one buffer provably touch different elements: TRefs over the same rows whose
+    channel slices [ch_off, ch_off + Cp) do not meet (the parts of a concat buffer)."""
+    if not (isinstance(a, TRef) and isinstance(b, TRef)) or a.padw is not None or b.padw is not None:
+        return True
+    if a.row_stride != b.row_stride or a.N * a.npos != b.N * b.npos:
+        return True
+    return a.ch_off < b.ch_off + b.Cp and b.ch_off < a.ch_off + a.Cp
+
+
 def _conv_out(i, k, s, p, d):
     return (i + 2 * p - d * (k - 1) - 1) // s + 1
 
@@ -110,7 +120,7 @@ class Plan:
         self.stats = {"tcgen05": 0, "direct": 0, "depthwise": 0, "other": 0}
         # ---- lanes: independent branches of the network (SlowFast pathways) run on separate CUDA streams /
         #      graph branches.  Every op records the tensors it reads / writes; finalize() turns cross-lane
-        #      read-after-write pairs into event waits (see _schedule).
+        #      read-after-write, write-after-read and write-after-write pairs into event waits (see _schedule).
         self.lane = 0          # lane of the ops being emitted (set by the lowering)
         self.op_lane = []
         self.op_io = []        # (reads, writes) as lists of TRef / Buf, or None = unknown (acts as a full barrier)
@@ -148,21 +158,24 @@ class Plan:
         self.finalized = True
 
     def _schedule(self):
-        """Cross-lane dependencies.  For op i on lane L: for every other lane M, the LAST op j < i on M that wrote
-        a buffer op i reads (stream order covers the earlier ones).  Ops with unknown I/O are full barriers.  No
-        buffer is reused inside a plan, so read-after-write is the only hazard (two lanes writing one concat
-        buffer write disjoint channel slices)."""
-        def bufs_of(items):
+        """Cross-lane dependencies.  For op i on lane L: for every other lane M, the LAST op j < i on M that i
+        conflicts with (stream order covers the earlier ones): j wrote a buffer i reads (read-after-write), or i
+        writes elements j read or wrote (write-after-read, write-after-write: in-place ops such as the SE scale and
+        the activations, the SE-sum accumulators).  Writes are compared by element footprint (_may_overlap), so two
+        lanes writing disjoint channel slices of one concat buffer stay concurrent.  Ops with unknown I/O are full
+        barriers."""
+        def items_of(items):
             out = []
             for t in items or ():
                 b = t if isinstance(t, Buf) else getattr(t, "buf", None)
                 if b is not None:
-                    out.append(b)
+                    out.append((b, t))
             return out
         n = len(self.ops)
         lanes = sorted(set(self.op_lane)) if self.op_lane else [0]
         waits = [[] for _ in range(n)]      # op -> list of op indices (on other lanes) to wait for
         writers = {}                        # id(buf) -> {lane: last writer op}
+        touched = {}                        # id(buf) -> {lane: [(op, item)]} every read and write, in program order
         last_on_lane = {}
         last_barrier = None                 # last op with unknown I/O
         waited = {}                         # lane -> {other lane: latest op already waited for}
@@ -175,9 +188,14 @@ class Plan:
                     if M != L:
                         need[M] = j
             else:
-                for b in bufs_of(io[0]):
+                for b, _ in items_of(io[0]):
                     for M, j in writers.get(id(b), {}).items():
                         if M != L:
+                            need[M] = max(need.get(M, -1), j)
+                for b, t in items_of(io[1]):
+                    for M, acc in touched.get(id(b), {}).items():
+                        if M != L:
+                            j = next((j for j, u in reversed(acc) if _may_overlap(t, u)), -1)
                             need[M] = max(need.get(M, -1), j)
                 if last_barrier is not None and self.op_lane[last_barrier] != L:
                     M = self.op_lane[last_barrier]
@@ -193,7 +211,9 @@ class Plan:
             if io is None:
                 last_barrier = i
             else:
-                for b in bufs_of(io[1]):
+                for b, t in items_of(io[0]) + items_of(io[1]):
+                    touched.setdefault(id(b), {}).setdefault(L, []).append((i, t))
+                for b, _ in items_of(io[1]):
                     writers.setdefault(id(b), {})[L] = i
             last_on_lane[L] = i
         signals = sorted(set(j for w in waits for j in w))
@@ -510,7 +530,8 @@ class Plan:
                 "stride": tuple(stride), "padding": tuple(padding), "dilation": tuple(dilation), "groups": groups,
                 "act": act, "residual": residual, "addend": addend, "y": y, "se_sums": sums}
         self.add(name, fn_stem if stem_rows else (fn_dw if (depthwise and residual is None) else fn), kind, flops, nbytes,
-                 reads=(x,) + ((residual,) if residual is not None else ()) + ((a,) if addend is not None else ()),
+                 reads=(x,) + ((residual,) if residual is not None else ()) + ((a,) if addend is not None else ())
+                 + ((sums,) if sums is not None else ()),          # the SE sums accumulate onto the cleared buffer
                  writes=(y,) + ((sums,) if sums is not None else ()), spec=spec)
         if addend is not None:
             self.meta[-1]["addend"] = (a.buf, a_off)
@@ -698,10 +719,12 @@ class Plan:
             L.check(lib.pv_scale_act(x.ptr(), x.ptr(), x.dt, x.row_stride, x.row_stride, x.N, npos, Cp,
                                      gate.tensor.data_ptr(), act, stream), "pv_scale_act(%s)" % name)
         if fused is None:
-            self.add(name + ".sum", fn_sum, spec={"kind": "channel_sum", "x": x, "sums": sums})
-        self.add(name + ".gate", fn_gate, spec={"kind": "se_gate", "x": x, "sums": sums, "gate": gate, "w1": w1p[:, :Cc],
-                                                "b1": b1.detach().float().cpu(), "w2": w2p[:Cc], "b2": b2p[:Cc]})
-        self.add(name + ".apply", fn_apply, spec={"kind": "scale_act", "x": x, "y": x, "gate": gate, "act": act})
+            self.add(name + ".sum", fn_sum, reads=(x,), writes=(sums,), spec={"kind": "channel_sum", "x": x, "sums": sums})
+        self.add(name + ".gate", fn_gate, reads=(sums,), writes=(gate,),
+                 spec={"kind": "se_gate", "x": x, "sums": sums, "gate": gate, "w1": w1p[:, :Cc],
+                       "b1": b1.detach().float().cpu(), "w2": w2p[:Cc], "b2": b2p[:Cc]})
+        self.add(name + ".apply", fn_apply, reads=(x, gate), writes=(x,),
+                 spec={"kind": "scale_act", "x": x, "y": x, "gate": gate, "act": act})
         return x
 
     def raw_input(self, static_in):
@@ -735,7 +758,7 @@ class Plan:
         def fn(stream):
             L.check(lib.pv_scale_act(x.ptr(), x.ptr(), x.dt, x.row_stride, x.row_stride, x.N, x.npos, x.Cp,
                                      None, act, stream), "pv_scale_act(%s)" % name)
-        self.add(name, fn, spec={"kind": "scale_act", "x": x, "y": x, "gate": None, "act": act})
+        self.add(name, fn, reads=(x,), writes=(x,), spec={"kind": "scale_act", "x": x, "y": x, "gate": None, "act": act})
         return x
 
     def emit_head_reduce(self, x, softmax, name="head_reduce"):
@@ -903,7 +926,7 @@ def emit_add_layernorm(plan, a, br, ln, name="add_ln", want_sum=True):
                                      n_rows, C, g.data_ptr() if g is not None else None,
                                      b.data_ptr() if b is not None else None, eps, stream), "pv_add_layernorm(%s)" % name)
     plan.add(name, fn, "other", 0.0, n_rows * C * (_ESIZE[a.dt] + 2 + (4 if want_sum else 0) + (2 if ln is not None else 0)),
-             spec={"kind": "add_layernorm", "a": a, "br": br, "s": s, "y": y, "eps": eps,
+             reads=(a, br), writes=tuple(t for t in (s, y) if t is not None), spec={"kind": "add_layernorm", "a": a, "br": br, "s": s, "y": y, "eps": eps,
                    "gamma": ln.weight.detach().float().cpu() if ln is not None else None,
                    "beta": ln.bias.detach().float().cpu() if ln is not None else None})
     return s, y
@@ -1061,7 +1084,7 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool", norm_
                 L.check(lib.pv_dwconv3d_fwd(C_.byref(d), xp, w_d.data_ptr(), ones.data_ptr(), zeros.data_ptr(), yp,
                                             None, stream), "pv_dwconv3d_fwd(%s)" % name)
         plan.add(name + ".dwconv", fn, "depthwise", 2.0 * x.N * To * Ho * Wo * dim_all * k[0] * k[1] * k[2],
-                 (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz,
+                 (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz, reads=(x,), writes=(y,),
                  spec={"kind": "token_conv", "x": x, "y": y, "thw": (T, H, W), "cls": cls, "weight": w_full,
                        "stride": s, "padding": p, "dilation": dl, "prologue": norm_before_pool, "modules": pools,
                        "pre_scale": pre_vec[0] if pre_vec else None, "pre_bias": pre_vec[1] if pre_vec else None})
@@ -1080,7 +1103,7 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool", norm_
             L.check(lib.pv_pool3d_fwd(C_.byref(d), x.ptr() + cls * x.row_stride * esz,
                                       y.ptr() + cls * y.row_stride * esz, stream), "pv_pool3d_fwd(%s)" % name)
         plan.add(name + (".maxpool" if kind == "MaxPool3d" else ".avgpool"), fn, "other", 0.0,
-                 (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz,
+                 (x.N * T * H * W + x.N * To * Ho * Wo) * dim_all * esz, reads=(x,), writes=(y,),
                  spec={"kind": "pool", "x": x, "y": y, "mode": d.mode, "kernel": k, "stride": s, "padding": p,
                        "cls": cls, "thw": (T, H, W), "modules": pools})
     have_norm = [n is not None and type(n).__name__ != "Identity" and not norm_before_pool for n in norms]
@@ -1091,7 +1114,7 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool", norm_
             def fn_cls(stream):
                 L.check(lib.pv_copy_rows(x.ptr(), y.ptr(), x.dt, x.N, dim_all, x.npos * x.row_stride, y.npos * y.row_stride,
                                          stream), "pv_copy_rows(%s)" % name)
-            plan.add(name + ".cls", fn_cls, spec={"kind": "copy_cls", "x": x, "y": y})
+            plan.add(name + ".cls", fn_cls, reads=(x,), writes=(y,), spec={"kind": "copy_cls", "x": x, "y": y})
         return y, (To, Ho, Wo)
     for n in norms:
         if type(n).__name__ != "LayerNorm":
@@ -1110,7 +1133,7 @@ def emit_token_pool(plan, x, thw, pool, norm, heads, has_cls, name="pool", norm_
                                       g.data_ptr(), b.data_ptr(), dim // hd, x.ptr() if cls else None,
                                       x.npos * x.row_stride, y.npos, eps, stream), "pv_layernorm_sets(%s)" % name)
     plan.add(name + ".norm", fn_ln, "other", 0.0, 2 * y.N * y.npos * dim_all * esz,
-             spec={"kind": "layernorm_sets", "x": x, "y": y, "cls": cls, "head_dim": hd, "eps": eps,
+             reads=((x,) if cls else ()) + (y,), writes=(y,), spec={"kind": "layernorm_sets", "x": x, "y": y, "cls": cls, "head_dim": hd, "eps": eps,
                    "gamma": torch.cat([n.weight.detach().float().cpu() for n in norms]),
                    "beta": torch.cat([n.bias.detach().float().cpu() for n in norms])})
     return y, (To, Ho, Wo)
@@ -1134,7 +1157,7 @@ def emit_attention(plan, q, k, v, heads, scale, residual_pool, name="attn", norm
         d.v_batch_stride, d.o_batch_stride = Nk * v.row_stride, Nq * o.row_stride
         L.check(lib.pv_attention_fwd(C_.byref(d), q.ptr(), k.ptr(), v.ptr(), o.ptr(), stream), "pv_attention_fwd(%s)" % name)
     plan.add(name, fn, "attention", 4.0 * B * heads * Nq * Nk * (dim // heads),
-             (B * Nq * dim * 2 + 2 * B * Nk * dim) * _ESIZE[plan.dt],
+             (B * Nq * dim * 2 + 2 * B * Nk * dim) * _ESIZE[plan.dt], reads=(q, k, v), writes=(o,),
              spec={"kind": "attention", "q": q, "k": k, "v": v, "o": o, "heads": heads, "scale": d.scale,
                    "residual": bool(residual_pool), "normalize": d.normalize})
     plan.attention_calls.append({"name": name, "B": B, "H": heads, "Nq": Nq, "Nk": Nk, "D": dim // heads,

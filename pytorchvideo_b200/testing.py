@@ -851,7 +851,8 @@ def record_io(spec):
         ins = [spec["x"]] + [t for t in (spec["residual"],) if t is not None]
         if spec["addend"] is not None:
             ins.append(spec["addend"][0])
-        return ins, [spec["y"]] + ([spec["se_sums"]] if spec["se_sums"] is not None else [])
+        sums = [spec["se_sums"]] if spec["se_sums"] is not None else []      # accumulated onto: read and written
+        return ins + sums, [spec["y"]] + sums
     if k in ("to_ndhwc", "tokens_in"):
         return [], [spec["y"]]
     if k in ("head_reduce", "to_f32"):
@@ -865,7 +866,7 @@ def record_io(spec):
     if k == "add_layernorm":
         return [spec["a"], spec["br"]], [t for t in (spec["s"], spec["y"]) if t is not None]
     if k == "layernorm_sets":
-        return [spec["x"], spec["y"]], [spec["y"]]
+        return ([spec["x"]] if spec["cls"] else []) + [spec["y"]], [spec["y"]]
     if k == "attention":
         return [spec["q"], spec["k"], spec["v"]], [spec["o"]]
     if k == "mask_force_first":
@@ -915,6 +916,353 @@ def io_problems(plan):
         if not io_buffers(outs) <= io_buffers(io[1]):
             bad.append((n, "writes"))
     return bad
+
+
+# ---- declared footprints, the lanes' happens-before order and the footprint walk ------------------------------------
+# (tests/test_plan_schedule.py, tests/test_gpu_launch_footprint.py)
+class Footprint:
+    """A set of elements of plan buffers.  Per buffer, blocks (base, n, n_stride, rows, row_stride, width), each the
+    elements base + i * n_stride + r * row_stride + c for i < n, r < rows, c < width (in elements of the buffer)."""
+
+    def __init__(self):
+        self.blocks = {}            # id(buf) -> (buf, [block])
+
+    def add(self, buf, block):
+        self.blocks.setdefault(id(buf), (buf, []))[1].append(tuple(int(v) for v in block))
+
+    def bufs(self):
+        return [b for b, _ in self.blocks.values()]
+
+    def __contains__(self, buf):
+        return id(buf) in self.blocks
+
+    def extent(self, buf):
+        """One past the last element of ``buf`` the footprint covers (0 when it has none)."""
+        return max([base + (n - 1) * ns + (r - 1) * rs + w for base, n, ns, r, rs, w in self.blocks[id(buf)][1]
+                    if n and r and w] or [0])
+
+    def mark(self, buf, out, offset=0, scale=1):
+        """Set True the elements of ``buf`` the footprint covers in the flat bool tensor ``out``, which holds the
+        buffer from position ``offset`` in units of 1 / ``scale`` of its elements (scale = element size: a byte map)."""
+        for base, n, ns, r, rs, w in self.blocks.get(id(buf), (None, ()))[1]:
+            if n and r and w:
+                out.as_strided((n, r, w * scale), (ns * scale, rs * scale, 1), offset + base * scale).fill_(True)
+
+    def mask(self, buf):
+        """[numel] bool CPU tensor of the elements of ``buf`` the footprint covers."""
+        m = torch.zeros(max(buf.numel, self.extent(buf)), dtype=torch.bool)
+        self.mark(buf, m)
+        return m
+
+
+def footprint(item, span=None):
+    """The elements of its buffer a TRef, Buf or MaskRef covers.  A TRef covers its N * npos rows at row_stride,
+    channels [ch_off, ch_off + Cp) (the pad channels are part of the tensor); W-padded stem rows (padw) their whole
+    physical rows.  span: a slice of each sample's npos rows (token_span), else all of them.  A Buf or a plan-owned
+    mask covers its whole buffer."""
+    from .engine.plan import Buf, MaskRef, TRef
+    fp = Footprint()
+    if isinstance(item, MaskRef):
+        item = item.buf
+    if isinstance(item, Buf):
+        fp.add(item, (0, 1, 0, 1, 0, item.numel))
+    elif isinstance(item, TRef) and item.padw is not None:
+        fp.add(item.buf, (0, 1, 0, 1, 0, item.N * item.T * item.H * item.padw[1] * item.Cp))
+    elif isinstance(item, TRef):
+        r0, r1, _ = (span or slice(None)).indices(item.npos)
+        fp.add(item.buf, (item.ch_off + r0 * item.row_stride, item.N, item.npos * item.row_stride, max(r1 - r0, 0),
+                          item.row_stride, item.Cp))
+    return fp
+
+
+def op_footprints(plan, i):
+    """(read footprint, write footprint) of op i from its declared I/O (Plan.op_io), each TRef narrowed to the token
+    rows its record reads / writes (token_span); None when the op declares no I/O."""
+    io = plan.op_io[i]
+    if io is None:
+        return None
+    spec = plan.op_spec[i]
+    out = []
+    for items, role in ((io[0], "read"), (io[1], "write")):
+        fp = Footprint()
+        for t in items:
+            span = token_span(spec, t, role) if spec is not None and hasattr(t, "ch_off") else None
+            for buf, blocks in footprint(t, span).blocks.values():
+                for blk in blocks:
+                    fp.add(buf, blk)
+        out.append(fp)
+    return tuple(out)
+
+
+def happens_before(plan, waits=None):
+    """Vector clocks of the plan's multi-lane run (Plan.run): hb[i][M] is the last op of lane M ordered before op i or
+    op i itself.  Edges: stream order within a lane, the cross-lane waits (plan.sched["waits"], or ``waits``); every
+    lane starts after the fork, which precedes every op.  Op j reaches op i iff hb[i].get(lane of j, -1) >= j."""
+    waits = plan.sched["waits"] if waits is None else waits
+    hb, last = [], {}
+    for i, L in enumerate(plan.op_lane):
+        c = dict(hb[last[L]]) if L in last else {}
+        for j in waits[i]:
+            assert j < i, "op %d waits for a later op %d" % (i, j)
+            for M, k in hb[j].items():
+                if c.get(M, -1) < k:
+                    c[M] = k
+        c[L] = i
+        hb.append(c)
+        last[L] = i
+    return hb
+
+
+def schedule_conflicts(plan, waits=None):
+    """[(i, j, hazard, message)]: pairs of ops i < j on different lanes that no path of the happens-before graph
+    orders although they conflict: their declared footprints share an element and at least one of them writes it
+    (RAW, WAR or WAW), or one of them declares no I/O (it may touch anything)."""
+    hb = happens_before(plan, waits)
+    lane = plan.op_lane
+    names = [n for n, _ in plan.ops]
+    fps = [op_footprints(plan, i) for i in range(len(plan.ops))]
+    buf_no = {id(b): k for k, b in enumerate(plan.bufs)}
+    ordered = lambda j, i: hb[i].get(lane[j], -1) >= j        # noqa: E731
+
+    def msg(i, j, what):
+        return "op %d %s (lane %d) and op %d %s (lane %d): %s, and no wait orders them" % (
+            i, names[i], lane[i], j, names[j], lane[j], what)
+    bad = []
+    unknown = [i for i, f in enumerate(fps) if f is None]
+    for u in unknown:
+        for k in range(len(fps)):
+            if k != u and lane[k] != lane[u]:
+                i, j = min(u, k), max(u, k)
+                if not ordered(i, j):
+                    bad.append((i, j, "unknown", msg(i, j, "op %d declares no I/O" % u)))
+    access = {}                                   # id(buf) -> [(op, is write, footprint)]
+    for i, f in enumerate(fps):
+        if f is None:
+            continue
+        for w, fp in ((False, f[0]), (True, f[1])):
+            for b in fp.bufs():
+                access.setdefault(id(b), []).append((i, w, fp, b))
+    masks = {}
+
+    def mask(i, w, fp, b):
+        key = (i, w, id(b))
+        if key not in masks:
+            masks[key] = fp.mask(b)
+        return masks[key]
+    seen = set()
+    for acc in access.values():
+        for x in range(len(acc)):
+            for y in range(x + 1, len(acc)):
+                (i, wi, fi, b), (j, wj, fj, _) = sorted((acc[x], acc[y]), key=lambda a: a[0])
+                if i == j or lane[i] == lane[j] or not (wi or wj) or ordered(i, j):
+                    continue
+                mi, mj = mask(i, wi, fi, b), mask(j, wj, fj, b)
+                n = min(len(mi), len(mj))
+                hit = torch.nonzero(mi[:n] & mj[:n])
+                if len(hit) and (i, j, wi, wj) not in seen:
+                    seen.add((i, j, wi, wj))
+                    hazard = "WAW" if wi and wj else ("RAW" if wi else "WAR")
+                    bad.append((i, j, hazard, msg(i, j, "%s on buffer %d (%d shared elements, first %d)" % (
+                        hazard, buf_no.get(id(b), -1), len(hit), int(hit[0])))))
+    return sorted(bad)
+
+
+def legal_orders(plan):
+    """Two topological orders of the plan's happens-before graph (stream order + waits) for a single-stream run: the
+    highest lane's ops as early as their waits allow, and as late as they allow."""
+    n = len(plan.ops)
+    top = max(plan.op_lane)
+    preds = [set(plan.sched["waits"][i]) for i in range(n)]
+    prev = {}
+    for i, L in enumerate(plan.op_lane):
+        if L in prev:
+            preds[i].add(prev[L])
+        prev[L] = i
+    orders = []
+    for early in (True, False):
+        done, order = set(), []
+        heads = {}
+        for i, L in enumerate(plan.op_lane):
+            heads.setdefault(L, []).append(i)
+        pos = {L: 0 for L in heads}
+        while len(order) < n:
+            ready = [ops[pos[L]] for L, ops in heads.items() if pos[L] < len(ops) and preds[ops[pos[L]]] <= done]
+            assert ready, "the schedule has a cycle"
+            pick = min(ready, key=lambda i: ((plan.op_lane[i] != top) if early else (plan.op_lane[i] == top), i))
+            order.append(pick)
+            done.add(pick)
+            pos[plan.op_lane[pick]] += 1
+        orders.append(order)
+    return orders
+
+
+def address_buffers(plan):
+    """Plan buffers some op reads as addresses, counts or geometry: masks (MaskRef buffers) and every non-float
+    buffer.  The footprint walk never fills them with a canary (an arbitrary value could steer an address); it checks
+    them for undeclared writes only."""
+    from . import _lib as L
+    from .engine.plan import MaskRef
+    out = {id(b) for b in plan.bufs if b.dt not in (L.PV_F16, L.PV_F32)}
+    for spec in plan.op_spec:
+        for v in (spec or {}).values():
+            if isinstance(v, MaskRef) and v.buf is not None:
+                out.add(id(v.buf))
+    return out
+
+
+# byte patterns the walk fills undeclared elements with: all ones (NaN in f16 and fp32), and 0x7B (f16 60768, fp32
+# 1.3e36: large finite values), so that a value equal to one canary cannot hide a read
+FOOTPRINT_CANARIES = (0xFF, 0x7B)
+_ARENA_ALIGN = 1024            # byte alignment of each buffer in the arena, and the canary guard after each
+
+
+def _arenas(plan, n):
+    """Lay every plan buffer out in ``n`` flat byte arenas of one layout, each buffer 1 KiB aligned and followed by at
+    least 1 KiB of guard bytes that belong to no buffer, the first arena holding the buffers' current values.  Returns
+    (arenas, [(byte offset, byte size)] per buffer, per arena the byte view of every buffer, the buffers' dtypes)."""
+    layout, pos = [], _ARENA_ALIGN
+    for b in plan.bufs:
+        nbytes = b.tensor.numel() * b.tensor.element_size()
+        layout.append((pos, nbytes))
+        pos = -(-(pos + nbytes + _ARENA_ALIGN) // _ARENA_ALIGN) * _ARENA_ALIGN
+    arenas = [torch.zeros(pos + 64 * _ARENA_ALIGN, dtype=torch.uint8, device=plan.device) for _ in range(n)]
+    views = [[a[off:off + nbytes] for off, nbytes in layout] for a in arenas]
+    dts = [b.tensor.dtype for b in plan.bufs]
+    for b, v in zip(plan.bufs, views[0]):
+        v.view(b.tensor.dtype).copy_(b.tensor.reshape(-1))
+    return arenas, layout, views, dts
+
+
+def _point(plan, views, dts):
+    """Point every plan buffer at its byte view in one arena (the ops resolve their pointers when they run)."""
+    for b, v, dt in zip(plan.bufs, views, dts):
+        b.tensor = v.view(dt)
+
+
+def _locate(layout, plan, byte):
+    """'buffer k element e' (or 'guard after buffer k') for a byte offset of an arena."""
+    import bisect
+    k = bisect.bisect_right([o for o, _ in layout], byte) - 1
+    if k < 0:
+        return "guard before buffer 0"
+    off, nbytes = layout[k]
+    if byte >= off + nbytes:
+        return "guard after buffer %d" % k
+    return "buffer %d element %d" % (k, (byte - off) // plan.bufs[k].tensor.element_size())
+
+
+def footprint_walk(plan, static_in, check=None, canaries=FOOTPRINT_CANARIES):
+    """Run the plan op by op on one stream, in program order, and check that every launch touches only what it
+    declares (Plan.op_io, as op_footprints reads it).  With S_i the plan buffers just before op i and R = S_{i+1} its
+    result, for each canary: op i runs on a copy of the buffers in which every element (and every guard byte between
+    buffers) it does not declare as read holds the canary and every element it declares as read holds its value in
+    S_i; every element it declares as written must then equal R bit for bit (else it read something undeclared, or
+    left part of its declared output as it was), and every other byte must hold what it held (else it wrote outside
+    its declaration).  Buffers address_buffers names always hold their values in S_i, never a canary; they are only
+    checked for writes.  After the walk the constants and the staged inputs must be bit-unchanged.
+    The buffers live in two arenas of one layout: the true state, which every op advances, and the canary copy, which
+    holds the canary everywhere between ops, so each op costs its own buffers plus one word-wise comparison of the
+    canary arena with the canary.  check: the op indices to check (default all; the others only run).
+    Returns (ops checked, failures [(op index, name, message)], skipped [(op index, name, reason)])."""
+    (true, canary, start), layout, (tv, cv, _), dts = _arenas(plan, 3)
+    start.copy_(true)
+    kno = {id(b): k for k, b in enumerate(plan.bufs)}
+    addr = sorted(kno[a] for a in address_buffers(plan))
+    sp = torch.cuda.current_stream().cuda_stream
+    consts0 = [c.clone() for c in plan.consts]
+    static0 = [s.clone() for s in static_in]
+    words = canary.view(torch.int64)
+    flag = torch.empty(words.shape, dtype=torch.bool, device=words.device)
+    fps, failures, skipped, msgs = {}, [], [], {}
+    for i, (name, _) in enumerate(plan.ops):
+        if check is not None and i not in check:
+            continue
+        f = op_footprints(plan, i)
+        if f is None:
+            skipped.append((i, name, "no declared I/O"))
+            continue
+        over = [kno[id(b)] for fp in f for b in fp.bufs() if fp.extent(b) > b.tensor.numel()]
+        if over:
+            failures.append((i, name, "declared footprint runs past the end of buffer %s" % over))
+            continue
+        fps[i] = f
+    for K in canaries:
+        true.copy_(start)
+        canary.fill_(K)
+        kword = int.from_bytes(bytes([K]) * 8, "little", signed=True)
+        for i, (name, fn) in enumerate(plan.ops):
+            if i not in fps:
+                _point(plan, tv, dts)
+                fn(sp)
+                continue
+            rd, wr = fps[i]
+            touched = sorted({kno[id(b)] for b in rd.bufs() + wr.bufs()} | set(addr))
+            saved = []
+            for k in touched:
+                b, esz = plan.bufs[k], plan.bufs[k].tensor.element_size()
+                rb = torch.zeros(layout[k][1], dtype=torch.bool, device=flag.device)
+                wb = torch.zeros_like(rb)
+                if k in addr:
+                    rb.fill_(True)
+                rd.mark(b, rb, 0, esz)
+                wr.mark(b, wb, 0, esz)
+                s_k = tv[k].clone()
+                torch.where(rb, s_k, cv[k], out=cv[k])
+                saved.append((k, rb, wb, s_k))
+            _point(plan, cv, dts)
+            fn(sp)
+            _point(plan, tv, dts)
+            fn(sp)
+            n_r = n_w = 0
+            first_r = first_w = None
+            for k, rb, wb, s_k in saved:
+                want = torch.where(wb, tv[k], s_k.masked_fill(~rb, K))
+                bad = cv[k] != want
+                if bool(bad.any()):
+                    inw = bad & wb
+                    out = bad & ~wb
+                    if bool(inw.any()):
+                        n_r += int(inw.sum())
+                        first_r = first_r or _locate(layout, plan, layout[k][0] + int(torch.nonzero(inw)[0]))
+                    if bool(out.any()):
+                        n_w += int(out.sum())
+                        first_w = first_w or _locate(layout, plan, layout[k][0] + int(torch.nonzero(out)[0]))
+                cv[k].fill_(K)
+            torch.ne(words, kword, out=flag)
+            if bool(flag.any()):
+                bad = torch.nonzero(canary != K).flatten()
+                n_w += len(bad)
+                first_w = first_w or _locate(layout, plan, int(bad[0]))
+                canary.fill_(K)
+            parts = []
+            if n_r:
+                parts.append("%d bytes of its declared output differ from the true run (reads undeclared input or "
+                             "does not write all of it; first at %s)" % (n_r, first_r))
+            if n_w:
+                parts.append("%d bytes outside its declared output changed (first at %s)" % (n_w, first_w))
+            if parts:
+                msgs.setdefault(i, []).append("canary 0x%02X: %s" % (K, "; ".join(parts)))
+    _point(plan, tv, dts)
+    torch.cuda.synchronize()
+    failures += [(i, plan.ops[i][0], " | ".join(m)) for i, m in sorted(msgs.items())]
+    for k, (c, c0) in enumerate(zip(plan.consts, consts0)):
+        if not torch.equal(_bits(c), _bits(c0)):
+            failures.append((-1, "const %d" % k, "a plan constant changed during the walk"))
+    for k, (s, s0) in enumerate(zip(static_in, static0)):
+        if not torch.equal(_bits(s), _bits(s0)):
+            failures.append((-1, "input %d" % k, "a staged input changed during the walk"))
+    return len(fps), failures, skipped
+
+
+def run_in_order(plan, order):
+    """Zero every plan buffer and run the ops on one stream in ``order``; returns a copy of every buffer."""
+    sp = torch.cuda.current_stream().cuda_stream
+    for b in plan.bufs:
+        b.tensor.zero_()
+    for i in order:
+        plan.ops[i][1](sp)
+    torch.cuda.synchronize()
+    return [b.tensor.clone() for b in plan.bufs]
 
 
 # ---- reading plan tensors
@@ -1605,6 +1953,37 @@ def batch_sweep(workloads):
     rows += [("f32", "detection", c, 3, "abc") for c in sorted(DETECTION_CASES)]
     rows += [(p, "ssl", c, B, "abc") for p in ("f16", "f32") for c in SSL_TRUNK_CASES for B in (1, 2, 3)]
     return rows
+
+
+def multi_lane_case(family, case):
+    """True for the catalogue cases whose plans run on more than one lane: SlowFast (two pathways), Audiovisual
+    SlowFast (three) and the masked multipath models (one per stream)."""
+    if family == "model":
+        return bool(MODEL_CASES[case][6])
+    if family in ("hub_tail", "grouped", "detection"):
+        return case.startswith("slowfast")
+    return (family == "audio" and case.startswith("avsf")) or (family == "masked" and case.startswith("multipath"))
+
+
+FOOTPRINT_PARTS = ("f16", "f32")
+
+
+def footprint_cases(workloads, sweep=False):
+    """[(precision, family, case, batch or None = the case's own)] of the footprint checks: every audit_catalogue case
+    in f16 and in f32, and the multi-lane cases at batch 3 in both (tiles and the Fast-stem route change there).
+    sweep: the multi-lane cases also at every batch of batch_sweep."""
+    cat = audit_catalogue(workloads)
+    rows = [(p, f, c, None) for p in ("f16", "f32") for f, c, _ in cat]
+    multi = [(f, c) for f, c, _ in cat if multi_lane_case(f, c)]
+    extra = {(p, f, c, 3) for p in ("f16", "f32") for f, c in multi}
+    if sweep:
+        extra |= {(p, f, c, B) for p, f, c, B, _ in batch_sweep(workloads) if (f, c) in multi}
+    return rows + sorted(extra)
+
+
+def footprint_part(row):
+    """The file of the GPU footprint walk a footprint_cases row runs in: one per precision."""
+    return row[0]
 
 
 def build_audit_case(family, case):
